@@ -282,7 +282,8 @@ extern "C" int qipb200_launch_stats(const qipb200_ctx *ctx, uint64_t *out4) {
   return QIPB200_OK;
 }
 
-// Host-only (no GPU, no context): plan `ops` for an n-qubit single-device state, generate the specialised source
+// Host-only (no GPU, no context): plan `ops` for an n-qubit single-device state (sharded states plan with their own
+// geometry, f64 L = 5 instead of 4, so their passes are not among these programs), generate the specialised source
 // of every fused pass and compile it with NVRTC for sm_90a.  out[0] = passes planned, out[1] = passes the
 // generator covered, out[2] = of those compiled without error, out[3] = total NVRTC wall time (ms, all passes in
 // parallel on the worker pool), out[4] = sum of the per-program compile times (ms).

@@ -1076,10 +1076,19 @@ size_t pass_bytes(const HostPass &p) {
 
 }  // namespace
 
-PlanConfig default_plan_config(qip_prec prec, uint32_t n_local) {
+PlanConfig default_plan_config(qip_prec prec, uint32_t n_local, bool sharded) {
   PlanConfig c;
+  const char *j = getenv("QIPB200_JIT");
+  const bool jit_off = j && (!strcmp(j, "off") || !strcmp(j, "0"));
+  const bool generated = n_local >= 22 && !jit_off;  // passes run generated kernels (jit_runtime.cu: from 22 local qubits)
   c.T = prec == QIP_F32 ? 13 : 12;  // 64 KiB of amplitudes per tile
   c.L = prec == QIP_F32 ? 6 : 5;    // 512-byte contiguous runs in HBM
+  // f64 states on generated kernels: 256-byte contiguous runs (L = 4), i.e. 8 instead of 7 freely chosen tile bits.  On one
+  // H100 SXM (400 W power limit), N=30 f64 headline circuit, alternating runs: 21 passes, 285.9-287.2 ms against 25 passes,
+  // 329.5-332.2 ms with L = 5 (pass 13.2 vs 12.9 ms).  Passes whose generated kernel is not ready (or every pass, when NVRTC
+  // or the driver API is missing) run the interpreter kernel on the same L = 4 plan; its speed there is not measured.
+  // Sharded states keep L = 5: the migration protocols have not been run at L = 4.
+  if (prec == QIP_F64 && generated && !sharded) c.L = 4;
   // test / tuning knobs (tile geometry and grouping only; results are unaffected)
   if (const char *e = getenv("QIPB200_TILE_T")) c.T = std::min<uint32_t>((uint32_t)atoi(e), c.T);
   if (const char *e = getenv("QIPB200_TILE_L")) c.L = (uint32_t)atoi(e);
@@ -1104,13 +1113,9 @@ PlanConfig default_plan_config(qip_prec prec, uint32_t n_local) {
   // circuit) and FP64 work is worth saving (phases kept out of real 2x2 gates).  On one H100 SXM (700 W), N=30 f64:
   // 25 passes, 300-304 ms with both options vs 29 passes, 347 ms without.  (The interpreter kernel is bound by its own
   // instruction stream and does not gain from either.)
-  {
-    const char *j = getenv("QIPB200_JIT");
-    const bool jit_off = j && (!strcmp(j, "off") || !strcmp(j, "0"));
-    if (n_local >= 22 && !jit_off) {
-      if (!getenv("QIPB200_SEED_SEARCH")) c.seed_search = true;
-      if (!getenv("QIPB200_KEEP_REAL")) c.keep_real = true;
-    }
+  if (generated) {
+    if (!getenv("QIPB200_SEED_SEARCH")) c.seed_search = true;
+    if (!getenv("QIPB200_KEEP_REAL")) c.keep_real = true;
   }
   if (n_local < c.T) c.T = n_local;
   if (c.L > c.T) c.L = c.T;

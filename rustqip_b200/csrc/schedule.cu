@@ -222,7 +222,7 @@ int run_fused(qipb200_state *s, const qip_op *ops, size_t n_ops, const std::vect
     if (e != cudaSuccess) return report_cuda_error(s, e, "cudaFuncSetAttribute(tile pass)");
     s->ctx->tile_configured = true;
   }
-  PlanConfig cfg = default_plan_config(s->prec, s->n_local);
+  PlanConfig cfg = default_plan_config(s->prec, s->n_local, s->world > 1);
   if (s->world > 1 && overlap_exchange_enabled()) cfg.reserve_bit = (int)s->n_local - 1;  // passes splittable in halves
   // Paired send (QIPB200_PAIRED_SEND=1): the migration that ends an epoch is fused into the epoch's last tile pass and done
   // in place, tile by tile, against the partner's copy of the same pass.  Tiles pair up across GPUs, so every rank must

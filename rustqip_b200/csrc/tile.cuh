@@ -316,7 +316,7 @@ int plan_layout_restore(qip_prec prec, uint32_t n, const PlanConfig &cfg, uint32
 // records do not fit kMaxPassBytes (the planner bounds passes so that they do).
 bool serialise_pass(const HostPass &p, PassParams *out);
 
-// Tile geometry defaults per precision.
-PlanConfig default_plan_config(qip_prec prec, uint32_t n_local);
+// Tile geometry defaults per precision; `sharded`: the state is split over several GPUs.
+PlanConfig default_plan_config(qip_prec prec, uint32_t n_local, bool sharded = false);
 
 }  // namespace qipb200
