@@ -207,6 +207,16 @@ int qipb200_state_measure_prob(qipb200_state *state, uint64_t measured, const ui
  * supplied by the caller (the reference calls rand::random). */
 int qipb200_state_soft_measure(qipb200_state *state, const uint64_t *indices, uint32_t n_indices,
                                double r, uint64_t *measured);
+/* K = n_draws independent soft_measure draws (measurement_ops.rs:153-176) on one state, which is NOT collapsed:
+ * measured[k] is what qipb200_state_soft_measure(state, indices, n_indices, draws[k], ..) returns, up to
+ * summation order (a draw within rounding distance of a cumulative boundary may land on the neighbouring index).
+ * bit i of measured[k] <-> indices[i].  draws / measured are HOST arrays of n_draws entries; the draws are not
+ * range-checked (a draw at or above the state's total, or NaN, gives index 0, as in the reference).
+ * Reads the state at most twice whatever K (per-chunk sums, then only the chunks some draw landed in); the
+ * number of kernels does not depend on K; the same state and draws give bit-identical results.  Synchronises.
+ * n_draws == 0 is a no-op.  Sharded states: QIPB200_ERR_UNSUPPORTED. */
+int qipb200_state_sample(qipb200_state *state, const uint64_t *indices, uint32_t n_indices,
+                         const double *draws, uint64_t n_draws, uint64_t *measured);
 /* measure_state (measurement_ops.rs:220-269): zero the amplitudes that
  * contradict `measured`, scale the rest by 1/sqrt(measured_prob); in place. */
 int qipb200_state_collapse(qipb200_state *state, const uint64_t *indices, uint32_t n_indices,

@@ -221,6 +221,12 @@ class B200State {
     ctx_.check(qipb200_state_soft_measure(st_, indices.data(), (uint32_t)indices.size(), r, &m));
     return m;
   }
+  // draws.size() soft_measure draws on the uncollapsed state (shots without rerunning the circuit)
+  std::vector<uint64_t> sample(const std::vector<uint64_t> &indices, const std::vector<double> &draws) {
+    std::vector<uint64_t> m(draws.size());
+    ctx_.check(qipb200_state_sample(st_, indices.data(), (uint32_t)indices.size(), draws.data(), draws.size(), m.data()));
+    return m;
+  }
   void collapse(const std::vector<uint64_t> &indices, uint64_t measured, double prob) {  // measure_state, :220-269
     ctx_.check(qipb200_state_collapse(st_, indices.data(), (uint32_t)indices.size(), measured, prob));
   }

@@ -1581,6 +1581,38 @@ int soft_measure_impl(qipb200_state *s, const uint64_t *indices, uint32_t n_indi
   return QIPB200_OK;
 }
 
+// n_draws soft_measure draws on one unsharded state (kernels.cu: launch_sample): one upload of the draws, a constant
+// number of kernels, one download of the results.  The scan runs over canonical indices, so a permuted layout is
+// restored first.
+int sample_impl(qipb200_state *s, const uint64_t *indices, uint32_t n_indices, const double *draws, uint64_t n_draws,
+                uint64_t *measured) {
+  qipb200_ctx *ctx = s->ctx;
+  if (n_draws > 0xffffffffull) return set_err(ctx, QIPB200_ERR_UNSUPPORTED, "sample: more than 2^32-1 draws in one call");
+  CU(ctx, cudaSetDevice(ctx->device));
+  if (!layout_is_identity(s)) {
+    int st = restore_layout(s);
+    if (st != QIPB200_OK) return st;
+  }
+  SampleBits bits;
+  bits.n_bits = n_indices;
+  for (uint32_t i = 0; i < n_indices; ++i) bits.bitpos[i] = s->n - 1 - (uint32_t)indices[i];  // measurement_ops.rs:174-175
+  const size_t io = 16 * (size_t)n_draws;  // draws (double) + results (u64)
+  char *d = nullptr;
+  CU(ctx, cudaMallocAsync((void **)&d, io + sample_scratch_bytes(s->n_local, n_draws), ctx->stream));
+  double *d_draws = (double *)d;
+  uint64_t *d_out = (uint64_t *)(d + 8 * n_draws);
+  cudaError_t e = cudaMemcpyAsync(d_draws, draws, 8 * n_draws, cudaMemcpyHostToDevice, ctx->stream);
+  if (e == cudaSuccess)
+    e = launch_sample(s->prec, s->buf, s->n_local, d_draws, n_draws, bits, d + io, d_out, ctx->sm_count, ctx->stream,
+                      &ctx->launches);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(measured, d_out, 8 * n_draws, cudaMemcpyDeviceToHost, ctx->stream);
+  cudaError_t ef = cudaFreeAsync(d, ctx->stream);
+  if (e != cudaSuccess) return cuda_fail(ctx, e, "sample");
+  CU(ctx, ef);
+  CU(ctx, cudaStreamSynchronize(ctx->stream));
+  return QIPB200_OK;
+}
+
 int collapse_impl(qipb200_state *s, const uint64_t *indices, uint32_t n_indices, uint64_t measured, double measured_prob) {
   qipb200_ctx *ctx = s->ctx;
   if (measured_prob == 0.0) return QIPB200_OK;  // measurement_ops.rs:230: untouched
@@ -1648,6 +1680,20 @@ extern "C" int qipb200_state_soft_measure(qipb200_state *s, const uint64_t *indi
       return st;
     }
     return soft_measure_impl(s, indices, n_indices, r, measured);
+  });
+}
+
+extern "C" int qipb200_state_sample(qipb200_state *s, const uint64_t *indices, uint32_t n_indices, const double *draws,
+                                    uint64_t n_draws, uint64_t *measured) {
+  if (!s) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, "sample: NULL state");
+  return guarded(s->ctx, [&]() -> int {
+    int st = check_indices(s, indices, n_indices);
+    if (st != QIPB200_OK) return st;
+    if (s->world > 1 || !s->shards.empty())
+      return set_err(s->ctx, QIPB200_ERR_UNSUPPORTED, "sample: sharded states are not supported (use soft_measure per draw)");
+    if (n_draws == 0) return (int)QIPB200_OK;
+    if (!draws || !measured) return set_err(s->ctx, QIPB200_ERR_INVALID_ARG, "sample: NULL draws or measured");
+    return sample_impl(s, indices, n_indices, draws, n_draws, measured);
   });
 }
 

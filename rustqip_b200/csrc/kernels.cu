@@ -1274,6 +1274,310 @@ cudaError_t launch_chunk_sums(qip_prec prec, const void *psi, uint64_t len, uint
   return cudaGetLastError();
 }
 
+// ---------------------------------------------------------------------------------
+// sampling: many soft_measure draws on one state (qipb200_state_sample)
+// ---------------------------------------------------------------------------------
+// Every summation below runs in a fixed order (shuffles and shared memory, no floating-point atomics), so the same
+// state and draws give bit-identical results.  Integer atomics only count draws per chunk and hand out slots.
+
+static const uint32_t kScanPerThread = 4;
+static const uint32_t kScanTile = kThreads * kScanPerThread;  // elements per CTA of the first scan level
+
+// Exclusive prefix of v over the CTA in thread order; `total` receives the CTA's sum (all threads).
+template <typename T>
+__device__ __forceinline__ T block_exclusive_scan(T v, T &total) {
+  __shared__ T wsum[kThreads / 32];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  T x = v;
+  for (int o = 1; o < 32; o <<= 1) {
+    T u = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= o) x += u;
+  }
+  if (lane == 31) wsum[w] = x;
+  T ex = __shfl_up_sync(0xffffffffu, x, 1);
+  if (lane == 0) ex = T(0);
+  __syncthreads();
+  if (w == 0) {
+    T y = lane < kThreads / 32 ? wsum[lane] : T(0);
+    for (int o = 1; o < kThreads / 32; o <<= 1) {
+      T u = __shfl_up_sync(0xffffffffu, y, o);
+      if (lane >= o) y += u;
+    }
+    if (lane < kThreads / 32) wsum[lane] = y;
+  }
+  __syncthreads();
+  if (w > 0) ex = wsum[w - 1] + ex;
+  total = wsum[kThreads / 32 - 1];
+  __syncthreads();  // wsum may be reused by the next call
+  return ex;
+}
+
+// Scan level 1: inclusive scan of each kScanTile-element tile of `in` into `out`, tile totals into tile_tot.
+template <typename T>
+__global__ void __launch_bounds__(kThreads) k_scan_tiles(const T *__restrict__ in, T *__restrict__ out, uint64_t n,
+                                                         T *__restrict__ tile_tot) {
+  const uint64_t base = (uint64_t)blockIdx.x * kScanTile + (uint64_t)threadIdx.x * kScanPerThread;
+  T e[kScanPerThread];
+  T mine = T(0);
+#pragma unroll
+  for (uint32_t j = 0; j < kScanPerThread; ++j) {
+    e[j] = base + j < n ? in[base + j] : T(0);
+    mine += e[j];
+  }
+  T total;
+  T run = block_exclusive_scan(mine, total);
+#pragma unroll
+  for (uint32_t j = 0; j < kScanPerThread; ++j) {
+    run += e[j];
+    if (base + j < n) out[base + j] = run;
+  }
+  if (threadIdx.x == 0) tile_tot[blockIdx.x] = total;
+}
+
+// Scan level 2 (one CTA): tile totals -> exclusive tile offsets, in place.
+template <typename T>
+__global__ void __launch_bounds__(kThreads) k_scan_tile_offsets(T *tot, uint32_t n_tiles) {
+  const uint32_t per = (n_tiles + kThreads - 1) / kThreads;
+  const uint32_t b = threadIdx.x * per;
+  const uint32_t e = b + per < n_tiles ? b + per : n_tiles;
+  T mine = T(0);
+  for (uint32_t i = b; i < e; ++i) mine += tot[i];
+  T total;
+  T run = block_exclusive_scan(mine, total);
+  for (uint32_t i = b; i < e; ++i) {
+    const T t = tot[i];
+    tot[i] = run;
+    run += t;
+  }
+}
+
+// Scan level 3: add each tile's offset.
+template <typename T>
+__global__ void __launch_bounds__(kThreads) k_scan_add(T *out, uint64_t n, const T *__restrict__ tile_off) {
+  const uint64_t i = (uint64_t)blockIdx.x * kThreads + threadIdx.x;
+  if (i >= n || i < kScanTile) return;  // tile 0 has offset 0
+  out[i] = tile_off[i / kScanTile] + out[i];
+}
+
+template <typename T>
+static cudaError_t launch_inclusive_scan(const T *in, T *out, uint64_t n, T *tile_tot, cudaStream_t s,
+                                         uint64_t *launches) {
+  const uint64_t tiles = (n + kScanTile - 1) / kScanTile;
+  k_scan_tiles<T><<<(unsigned)tiles, kThreads, 0, s>>>(in, out, n, tile_tot);
+  k_scan_tile_offsets<T><<<1, kThreads, 0, s>>>(tile_tot, (uint32_t)tiles);
+  k_scan_add<T><<<grid_for(n), kThreads, 0, s>>>(out, n, tile_tot);
+  *launches += 3;
+  return cudaGetLastError();
+}
+
+// Locate: the smallest chunk c with r - cdf[c] <= 0 (else the last chunk), the draw's remainder r - cdf[c-1], and a
+// slot among the chunk's draws.  The first draw to arrive at a chunk appends it to the list of occupied chunks.
+__global__ void __launch_bounds__(kThreads)
+    k_sample_locate(const double *__restrict__ draws, uint64_t n_draws, const double *__restrict__ cdf, uint32_t chunks,
+                    uint32_t *counts, uint32_t *chunk_of, uint32_t *slot, double *resid, uint32_t *occ,
+                    uint32_t *n_occ) {
+  const uint64_t k = (uint64_t)blockIdx.x * kThreads + threadIdx.x;
+  if (k >= n_draws) return;
+  const double r = draws[k];
+  uint32_t lo = 0, hi = chunks - 1;  // r - cdf[c] is non-increasing in c
+  while (lo < hi) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (r - cdf[mid] <= 0.0)
+      hi = mid;
+    else
+      lo = mid + 1;
+  }
+  const uint32_t s = atomicAdd(&counts[lo], 1u);
+  if (s == 0) occ[atomicAdd(n_occ, 1u)] = lo;
+  chunk_of[k] = lo;
+  slot[k] = s;
+  resid[k] = lo ? r - cdf[lo - 1] : r;
+}
+
+// Group the draw ids by chunk: ids[start of chunk c + slot] = draw (ends = inclusive scan of the counts).
+__global__ void __launch_bounds__(kThreads)
+    k_sample_scatter(uint64_t n_draws, const uint32_t *__restrict__ chunk_of, const uint32_t *__restrict__ slot,
+                     const uint32_t *__restrict__ counts, const uint32_t *__restrict__ ends, uint32_t *ids) {
+  const uint64_t k = (uint64_t)blockIdx.x * kThreads + threadIdx.x;
+  if (k >= n_draws) return;
+  const uint32_t c = chunk_of[k];
+  ids[ends[c] - counts[c] + slot[k]] = (uint32_t)k;
+}
+
+static const uint32_t kSampleMaxChunkLog2 = 12;
+static const uint32_t kSampleRounds = (1u << kSampleMaxChunkLog2) / kThreads;  // 32-amplitude rounds per warp
+
+// A remainder that the in-chunk prefix leaves positive (chunk-level and in-chunk rounding disagree) continues
+// serially through the following chunks, as the reference's scan would; chunks whose sum is 0 cannot cross.
+template <typename R>
+__device__ uint64_t sample_continue(const R *__restrict__ psi, uint32_t chunk_log2, uint32_t chunks,
+                                    const double *__restrict__ sums, uint32_t c, double rem) {
+  for (; c < chunks; ++c) {
+    if (sums[c] == 0.0) continue;
+    const uint64_t b = (uint64_t)c << chunk_log2;
+    for (uint64_t i = b; i < b + (1ull << chunk_log2); ++i) {
+      typename Vec2<R>::type v = *reinterpret_cast<const typename Vec2<R>::type *>(psi + 2 * i);
+      rem -= (double)v.x * (double)v.x + (double)v.y * (double)v.y;
+      if (rem <= 0.0) return i;
+    }
+  }
+  return 0;  // no crossing: index 0, as the reference leaves it
+}
+
+// Resolve: one CTA per occupied chunk (grid-stride over the list).  Each warp loads a contiguous segment of the chunk
+// with 16-byte loads and scans it 32 amplitudes at a time; the warp offsets complete the chunk's inclusive prefix
+// in shared memory, which every draw of the chunk binary-searches.
+template <typename R>
+__global__ void __launch_bounds__(kThreads)
+    k_sample_resolve(const R *__restrict__ psi, uint32_t chunk_log2, uint32_t chunks, const double *__restrict__ sums,
+                     const uint32_t *__restrict__ occ, const uint32_t *__restrict__ n_occ,
+                     const uint32_t *__restrict__ counts, const uint32_t *__restrict__ ends,
+                     const uint32_t *__restrict__ ids, const double *__restrict__ resid, uint64_t *__restrict__ out,
+                     const __grid_constant__ SampleBits bits) {
+  __shared__ double q[1u << kSampleMaxChunkLog2];
+  __shared__ double wtot[kThreads / 32];
+  const uint32_t lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const uint32_t clen = 1u << chunk_log2;
+  const uint32_t seg = clen >= 32 * (kThreads / 32) ? clen / (kThreads / 32) : 32;  // amplitudes per warp
+  const uint32_t rounds = seg / 32;
+  const bool active = w * seg < clen;
+  const uint32_t n = *n_occ;
+  for (uint32_t oi = blockIdx.x; oi < n; oi += gridDim.x) {
+    const uint32_t c = occ[oi];
+    const R *src = psi + 2 * ((uint64_t)c << chunk_log2);
+    if (active) {
+      double p[kSampleRounds];
+#pragma unroll
+      for (uint32_t i = 0; i < kSampleRounds; ++i) {
+        const uint32_t j = w * seg + 32 * i + lane;
+        p[i] = 0.0;
+        if (i < rounds && j < clen) {
+          typename Vec2<R>::type v = *reinterpret_cast<const typename Vec2<R>::type *>(src + 2 * j);
+          p[i] = (double)v.x * (double)v.x + (double)v.y * (double)v.y;
+        }
+      }
+      double carry = 0.0;
+#pragma unroll
+      for (uint32_t i = 0; i < kSampleRounds; ++i) {
+        if (i < rounds) {
+          double x = p[i];
+          for (uint32_t o = 1; o < 32; o <<= 1) {
+            const double u = __shfl_up_sync(0xffffffffu, x, o);
+            if (lane >= o) x += u;
+          }
+          x = carry + x;
+          const uint32_t j = w * seg + 32 * i + lane;
+          if (j < clen) q[j] = x;
+          carry = __shfl_sync(0xffffffffu, x, 31);
+        }
+      }
+      if (lane == 0) wtot[w] = carry;
+    }
+    __syncthreads();
+    if (active && w > 0) {
+      double off = 0.0;
+      for (uint32_t v = 0; v < w; ++v) off += wtot[v];
+      for (uint32_t i = 0; i < rounds; ++i) {
+        const uint32_t j = w * seg + 32 * i + lane;
+        if (j < clen) q[j] = off + q[j];
+      }
+    }
+    __syncthreads();
+    const uint32_t m = counts[c], start = ends[c] - m;
+    for (uint32_t d = threadIdx.x; d < m; d += kThreads) {
+      const uint32_t k = ids[start + d];
+      const double rem = resid[k];
+      uint32_t lo = 0, hi = clen;  // smallest j with rem - q[j] <= 0, clen if none
+      while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (rem - q[mid] <= 0.0)
+          hi = mid;
+        else
+          lo = mid + 1;
+      }
+      const uint64_t idx = lo < clen ? ((uint64_t)c << chunk_log2) + lo
+                                     : sample_continue(psi, chunk_log2, chunks, sums, c + 1, rem - q[clen - 1]);
+      uint64_t mbits = 0;
+      for (uint32_t i = 0; i < bits.n_bits; ++i) mbits |= ((idx >> bits.bitpos[i]) & 1ull) << i;
+      out[k] = mbits;
+    }
+    __syncthreads();  // q and wtot are rewritten for the next chunk
+  }
+}
+
+// Device scratch of one sampling call, carved from a single allocation (base == nullptr: sizes only).
+struct SampleScratch {
+  double *sums, *cdf, *dtot, *resid;                                // chunk sums, chunk CDF, scan tile totals; per draw
+  uint32_t *counts, *ends, *utot, *occ, *n_occ;                     // per chunk; scan tile totals; occupied chunks
+  uint32_t *chunk_of, *slot, *ids;                                  // per draw
+  size_t bytes;
+  SampleScratch(char *base, uint64_t chunks, uint64_t n_draws) {
+    const uint64_t tiles = (chunks + kScanTile - 1) / kScanTile;
+    size_t off = 0;
+    auto take = [&](size_t b) {
+      void *q = base ? base + off : nullptr;
+      off += (b + 15) & ~(size_t)15;
+      return q;
+    };
+    sums = (double *)take(8 * chunks);
+    cdf = (double *)take(8 * chunks);
+    dtot = (double *)take(8 * tiles);
+    resid = (double *)take(8 * n_draws);
+    counts = (uint32_t *)take(4 * chunks);
+    ends = (uint32_t *)take(4 * chunks);
+    utot = (uint32_t *)take(4 * tiles);
+    occ = (uint32_t *)take(4 * chunks);
+    n_occ = (uint32_t *)take(4);
+    chunk_of = (uint32_t *)take(4 * n_draws);
+    slot = (uint32_t *)take(4 * n_draws);
+    ids = (uint32_t *)take(4 * n_draws);
+    bytes = off;
+  }
+};
+
+uint32_t sample_chunk_log2(uint32_t n_local) { return n_local > kSampleMaxChunkLog2 ? kSampleMaxChunkLog2 : n_local; }
+
+size_t sample_scratch_bytes(uint32_t n_local, uint64_t n_draws) {
+  return SampleScratch(nullptr, 1ull << (n_local - sample_chunk_log2(n_local)), n_draws).bytes;
+}
+
+cudaError_t launch_sample(qip_prec prec, const void *psi, uint32_t n_local, const double *d_draws, uint64_t n_draws,
+                          const SampleBits &bits, void *d_scratch, uint64_t *d_out, int sm_count, cudaStream_t s,
+                          uint64_t *launches) {
+  const uint32_t chunk_log2 = sample_chunk_log2(n_local);
+  const uint64_t len = 1ull << n_local, chunks = len >> chunk_log2;
+  if (n_draws == 0 || chunks > 0xffffffffull || n_draws > 0xffffffffull || bits.n_bits > 64) return cudaErrorInvalidValue;
+  const SampleScratch sc((char *)d_scratch, chunks, n_draws);
+  double *sums = sc.sums, *cdf = sc.cdf, *resid = sc.resid;
+  uint32_t *counts = sc.counts, *ends = sc.ends, *occ = sc.occ, *n_occ = sc.n_occ;
+  uint32_t *chunk_of = sc.chunk_of, *slot = sc.slot, *ids = sc.ids;
+  cudaError_t e;
+  if ((e = cudaMemsetAsync(counts, 0, 4 * chunks, s)) != cudaSuccess) return e;
+  if ((e = cudaMemsetAsync(n_occ, 0, 4, s)) != cudaSuccess) return e;
+  // (1) one read sweep: per-chunk sums; (2) chunk-level CDF
+  if ((e = launch_chunk_sums(prec, psi, len, chunk_log2, sums, s, launches)) != cudaSuccess) return e;
+  if ((e = launch_inclusive_scan<double>(sums, cdf, chunks, sc.dtot, s, launches)) != cudaSuccess) return e;
+  // (3) locate every draw; (4) group the draws by chunk
+  k_sample_locate<<<grid_for(n_draws), kThreads, 0, s>>>(d_draws, n_draws, cdf, (uint32_t)chunks, counts, chunk_of,
+                                                        slot, resid, occ, n_occ);
+  ++*launches;
+  if ((e = launch_inclusive_scan<uint32_t>(counts, ends, chunks, sc.utot, s, launches)) != cudaSuccess) return e;
+  k_sample_scatter<<<grid_for(n_draws), kThreads, 0, s>>>(n_draws, chunk_of, slot, counts, ends, ids);
+  ++*launches;
+  // (5) re-read only the occupied chunks (at most min(draws, chunks) of them)
+  const uint64_t occ_max = n_draws < chunks ? n_draws : chunks;
+  const uint64_t cap = (uint64_t)(sm_count > 0 ? sm_count : 132) * 8;
+  const unsigned grid = (unsigned)(occ_max < cap ? occ_max : cap);
+  if (prec == QIP_F32)
+    k_sample_resolve<float><<<grid, kThreads, 0, s>>>((const float *)psi, chunk_log2, (uint32_t)chunks, sums, occ,
+                                                      n_occ, counts, ends, ids, resid, d_out, bits);
+  else
+    k_sample_resolve<double><<<grid, kThreads, 0, s>>>((const double *)psi, chunk_log2, (uint32_t)chunks, sums, occ,
+                                                       n_occ, counts, ends, ids, resid, d_out, bits);
+  ++*launches;
+  return cudaGetLastError();
+}
+
 template <typename R>
 __global__ void __launch_bounds__(kThreads)
     k_collapse(R *__restrict__ psi, uint64_t len, uint64_t index_base, uint64_t row_mask,

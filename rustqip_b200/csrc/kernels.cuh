@@ -61,6 +61,20 @@ cudaError_t launch_measure_probs(qip_prec prec, const void *psi, uint64_t len, u
 // per-chunk sums of |a|^2 (chunk = 2^chunk_log2 amplitudes) for inverse-CDF sampling.
 cudaError_t launch_chunk_sums(qip_prec prec, const void *psi, uint64_t len, uint32_t chunk_log2,
                               double *d_sums, cudaStream_t s, uint64_t *launches);
+// Sampling (qipb200_state_sample): n_draws independent soft_measure draws (measurement_ops.rs:153-176) on an
+// unsharded state in canonical layout, which is not modified.  One read sweep of per-chunk sums (chunks of
+// 2^sample_chunk_log2(n_local) amplitudes), a chunk-level CDF, then a second read of only the chunks some draw landed
+// in.  d_out[k] gets bits bitpos[i] of draw k's index at bit i.  The number of kernels does not depend on n_draws.
+struct SampleBits {
+  uint32_t n_bits;
+  uint32_t bitpos[64];
+};
+uint32_t sample_chunk_log2(uint32_t n_local);
+// bytes of the device scratch launch_sample needs (one allocation, 16-byte aligned)
+size_t sample_scratch_bytes(uint32_t n_local, uint64_t n_draws);
+cudaError_t launch_sample(qip_prec prec, const void *psi, uint32_t n_local, const double *d_draws, uint64_t n_draws,
+                          const SampleBits &bits, void *d_scratch, uint64_t *d_out, int sm_count, cudaStream_t s,
+                          uint64_t *launches);
 // measure_state: zero where (index & row_mask) != measured_mask, else scale by p_mult.
 cudaError_t launch_collapse(qip_prec prec, void *psi, uint64_t len, uint64_t index_base,
                             uint64_t row_mask, uint64_t measured_mask, double p_mult, cudaStream_t s,

@@ -223,6 +223,21 @@ class State:
         self._chk(_lib.lib().qipb200_state_soft_measure(self._h, _ptr(idx), len(idx), float(r), C.byref(m)))
         return int(m.value)
 
+    def sample(self, indices: Sequence[int], draws=None, shots: Optional[int] = None, rng=None) -> np.ndarray:
+        """Many soft_measure draws on the uncollapsed state: out[k] == soft_measure(indices, draws[k]).
+
+        Without ``draws``, ``shots`` uniforms in [0, 1) are drawn from ``rng`` (a numpy Generator; a fresh
+        ``np.random.default_rng()`` when None).  Reads the state at most twice for any number of draws."""
+        idx = np.ascontiguousarray(np.asarray(list(indices), dtype=np.uint64))
+        if draws is None:
+            if shots is None:
+                raise ValueError("sample: give draws or shots")
+            draws = (rng if rng is not None else np.random.default_rng()).random(int(shots))
+        r = np.ascontiguousarray(np.asarray(draws, dtype=np.float64).reshape(-1))
+        out = np.zeros(r.shape[0], dtype=np.uint64)
+        self._chk(_lib.lib().qipb200_state_sample(self._h, _ptr(idx), len(idx), _ptr(r), r.shape[0], _ptr(out)))
+        return out
+
     def collapse(self, indices: Sequence[int], measured: int, prob: float):
         idx = np.ascontiguousarray(np.asarray(list(indices), dtype=np.uint64))
         self._chk(_lib.lib().qipb200_state_collapse(self._h, _ptr(idx), len(idx), int(measured), float(prob)))
