@@ -222,6 +222,25 @@ int qipb200_state_sample(qipb200_state *state, const uint64_t *indices, uint32_t
 int qipb200_state_collapse(qipb200_state *state, const uint64_t *indices, uint32_t n_indices,
                            uint64_t measured, double measured_prob);
 
+enum {
+  QIPB200_MEASURE_FORCED = 1u,      /* *measured is an input: MeasuredCondition { measured, prob: None } */
+  QIPB200_MEASURE_FORCED_PROB = 2u  /* with FORCED: *prob is an input too (prob: Some(p)); no read sweep */
+};
+/* measure (measurement_ops.rs:190-214): draw the outcome as soft_measure does with the uniform r in [0,1)
+ * (ignored when FORCED), take its probability as measure_prob does (unless FORCED_PROB), collapse as
+ * measure_state does, and return both.  bit i of *measured <-> indices[i].  Synchronises.
+ *   *measured is what qipb200_state_soft_measure(state, indices, n_indices, r, ..) returns, up to summation order
+ *   (as for qipb200_state_sample); *prob is qipb200_state_measure_prob(state, *measured, ..) up to summation order;
+ *   the state afterwards is qipb200_state_collapse(state, indices, n_indices, *measured, *prob).  *prob == 0 leaves
+ *   the state untouched.  The same state and arguments give bit-identical results.
+ * Unsharded states: one read sweep plus the chunk the draw landed in when every measured qubit q satisfies
+ * q <= n-13 (at most two sweeps otherwise), a fixed number of kernels, and no collapse sweep: the collapse is kept
+ * pending on the state and runs as diagonal gates inside the first tile pass of the next fused apply_schedule (any
+ * other call that touches the amplitudes applies it first; set_basis and load drop it).
+ * Sharded and multi-device states: soft_measure, measure_prob and collapse in turn (collective). */
+int qipb200_state_measure(qipb200_state *state, const uint64_t *indices, uint32_t n_indices, double r,
+                          uint32_t flags, uint64_t *measured, double *prob);
+
 /* ---- multi-GPU: the 2^n state sharded by its top log2(world) index bits,
  *      one process per GPU (absent in the reference; its only hook is the
  *      input_offset/output_offset slice model, matrix_ops.rs:74-89) -------------- */

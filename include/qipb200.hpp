@@ -20,6 +20,7 @@
 #include <complex>
 #include <cstdint>
 #include <memory>
+#include <optional>
 #include <stdexcept>
 #include <string>
 #include <utility>
@@ -226,6 +227,21 @@ class B200State {
     std::vector<uint64_t> m(draws.size());
     ctx_.check(qipb200_state_sample(st_, indices.data(), (uint32_t)indices.size(), draws.data(), draws.size(), m.data()));
     return m;
+  }
+  // measure (measurement_ops.rs:190-214): draw with r in [0,1), take the probability, collapse; returns (m, p)
+  std::pair<uint64_t, double> measure(const std::vector<uint64_t> &indices, double r) {
+    uint64_t m = 0;
+    double p = 0.0;
+    ctx_.check(qipb200_state_measure(st_, indices.data(), (uint32_t)indices.size(), r, 0u, &m, &p));
+    return {m, p};
+  }
+  // ... with a forced outcome, and its probability when known (MeasuredCondition { measured, prob })
+  std::pair<uint64_t, double> measure(const std::vector<uint64_t> &indices, uint64_t measured, std::optional<double> prob) {
+    uint64_t m = measured;
+    double p = prob ? *prob : 0.0;
+    const uint32_t flags = QIPB200_MEASURE_FORCED | (prob ? (uint32_t)QIPB200_MEASURE_FORCED_PROB : 0u);
+    ctx_.check(qipb200_state_measure(st_, indices.data(), (uint32_t)indices.size(), 0.0, flags, &m, &p));
+    return {m, p};
   }
   void collapse(const std::vector<uint64_t> &indices, uint64_t measured, double prob) {  // measure_state, :220-269
     ctx_.check(qipb200_state_collapse(st_, indices.data(), (uint32_t)indices.size(), measured, prob));

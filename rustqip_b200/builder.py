@@ -214,13 +214,10 @@ class B200Builder:
                 flush()
                 indices = entry[0]
                 if forced:
-                    m = forced.pop(0)
+                    measurements.append(st.measure(indices, measured=forced.pop(0)))
                 else:
                     r = rng.random() if rng is not None else float(np.random.random())
-                    m = st.soft_measure(indices, r)
-                p = st.measure_prob(m, indices)
-                st.collapse(indices, m, p)
-                measurements.append((m, p))
+                    measurements.append(st.measure(indices, r))
             flush()
             return st.download(), measurements
 

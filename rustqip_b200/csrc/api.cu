@@ -514,6 +514,35 @@ bool layout_is_identity(const qipb200_state *s) {
   return true;
 }
 
+// P::one() / measured_prob.sqrt() evaluated in the state's precision (measurement_ops.rs:231)
+double collapse_multiplier(qip_prec prec, double measured_prob) {
+  if (prec == QIP_F32) return (double)(1.0f / sqrtf((float)measured_prob));
+  return 1.0 / sqrt(measured_prob);
+}
+
+// measure_state with a known multiplier over this rank's amplitudes, under the current layout.
+int launch_collapse_on(qipb200_state *s, const uint64_t *qubits, uint32_t n_qubits, uint64_t measured, double p_mult) {
+  qipb200_ctx *ctx = s->ctx;
+  CU(ctx, cudaSetDevice(ctx->device));
+  uint64_t row_mask = 0, measured_mask = 0;
+  for (uint32_t i = 0; i < n_qubits; ++i) {
+    const uint32_t bit = s->phys_of_logical[s->n - 1 - (uint32_t)qubits[i]];
+    row_mask |= 1ull << bit;
+    measured_mask |= ((measured >> i) & 1ull) << bit;
+  }
+  CU(ctx, launch_collapse(s->prec, s->buf, 1ull << s->n_local, (uint64_t)s->rank << s->n_local, row_mask,
+                          measured_mask, p_mult, ctx->stream, &ctx->launches));
+  return QIPB200_OK;
+}
+
+// Apply the collapse qipb200_state_measure left pending, before anything reads or writes the amplitudes.
+int materialise_collapse(qipb200_state *s) {
+  if (!s->collapse_pending) return QIPB200_OK;
+  s->collapse_pending = false;
+  return launch_collapse_on(s, s->pend_qubits.data(), (uint32_t)s->pend_qubits.size(), s->pend_measured,
+                            s->pend_p_mult);
+}
+
 int check_barrier_error(qipb200_state *s) {
   uint32_t flag = 0;
   CU(s->ctx, cudaMemcpyAsync(&flag, s->flags + kFlagErrorSlot, sizeof(flag), cudaMemcpyDeviceToHost, s->ctx->stream));
@@ -1117,6 +1146,7 @@ static int set_basis_impl(qipb200_state *s, uint64_t index) {
   qipb200_ctx *ctx = s->ctx;
   if (index >> s->n) return set_err(ctx, QIPB200_ERR_BAD_INDEX, "initial index out of range");
   CU(ctx, cudaSetDevice(ctx->device));
+  s->collapse_pending = false;  // every amplitude is overwritten
   for (uint32_t b = 0; b < s->n; ++b) s->phys_of_logical[b] = b;  // a fresh state has the canonical layout
   const uint64_t len = 1ull << s->n_local;
   const bool owns = (index >> s->n_local) == (uint64_t)s->rank;
@@ -1142,8 +1172,10 @@ static int transfer_impl(qipb200_state *s, void *host, uint64_t offset, uint64_t
   if (len > (1ull << s->n_local) || offset > (1ull << s->n_local) - len)
     return set_err(ctx, QIPB200_ERR_SIZE_MISMATCH, std::string(what) + ": range exceeds the local state");
   CU(ctx, cudaSetDevice(ctx->device));
+  int st = materialise_collapse(s);  // a partial upload keeps the other amplitudes
+  if (st != QIPB200_OK) return st;
   if (!layout_is_identity(s)) {
-    int st = restore_layout(s);
+    st = restore_layout(s);
     if (st != QIPB200_OK) return st;
   }
   const size_t ab = amp_bytes(s->prec);
@@ -1191,8 +1223,10 @@ extern "C" int qipb200_state_download(qipb200_state *s, void *host, uint64_t off
 
 static int apply_op_impl(qipb200_state *s, const qip_op *op) {
   CU(s->ctx, cudaSetDevice(s->ctx->device));
+  int st = materialise_collapse(s);
+  if (st != QIPB200_OK) return st;
   FlatOp f;
-  int st = compile_and_localize(s, op, &f, nullptr);
+  st = compile_and_localize(s, op, &f, nullptr);
   if (st != QIPB200_OK) return st;
   return apply_flat_local(s, f);
 }
@@ -1205,6 +1239,34 @@ extern "C" int qipb200_state_apply_op(qipb200_state *s, const qip_op *op) {
   });
 }
 
+// A schedule on a state with a pending collapse.  Fused: the collapse goes in front of the schedule as one-qubit
+// diagonal gates (qipb200_collapse_ops), which the planner folds into the first tile pass.  A schedule that fails
+// validation keeps the collapse pending when none of its ops runs; when the ops before the bad one run, the collapse
+// is applied first.  QIPB200_SCHED_NO_FUSION keeps one sweep per entry: the collapse runs as its own sweep.
+static int schedule_after_measure(qipb200_state *s, const qip_op *ops, size_t n_ops, uint32_t flags) {
+  CU(s->ctx, cudaSetDevice(s->ctx->device));
+  size_t bad = n_ops;
+  for (size_t i = 0; i < n_ops && bad == n_ops; ++i) {
+    FlatOp f;
+    std::string err;
+    if (compile_op(&ops[i], s->prec, s->n, &f, &err) != QIPB200_OK) bad = i;
+  }
+  if ((flags & QIPB200_SCHED_NO_FUSION) || bad != n_ops) {
+    if (bad != 0) {
+      int st = materialise_collapse(s);
+      if (st != QIPB200_OK) return st;
+    }
+    return run_schedule(s, ops, n_ops, flags);
+  }
+  const uint32_t k = (uint32_t)s->pend_qubits.size();
+  std::vector<qip_op> all(k + n_ops);
+  std::vector<double> dense(8 * (size_t)k);  // 4 complex<prec> per op
+  qipb200_collapse_ops(s->prec, s->pend_qubits.data(), k, s->pend_measured, s->pend_p_mult, all.data(), dense.data());
+  std::copy(ops, ops + n_ops, all.begin() + k);
+  s->collapse_pending = false;
+  return run_schedule(s, all.data(), all.size(), flags);
+}
+
 extern "C" int qipb200_state_apply_schedule(qipb200_state *s, const qip_op *ops, size_t n_ops, uint32_t flags) {
   if (!s) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, "state is NULL");
   if (!ops && n_ops) return set_err(s->ctx, QIPB200_ERR_INVALID_ARG, "schedule: ops is NULL");
@@ -1214,6 +1276,7 @@ extern "C" int qipb200_state_apply_schedule(qipb200_state *s, const qip_op *ops,
       return run_schedule(sh, ops, n_ops, flags);
     };
     if (!s->shards.empty()) return each_shard(s, one);
+    if (s->collapse_pending) return schedule_after_measure(s, ops, n_ops, flags);
     return one(s, 0);
   });
 }
@@ -1222,8 +1285,10 @@ extern "C" int qipb200_state_apply_schedule(qipb200_state *s, const qip_op *ops,
 static int norm2_impl(qipb200_state *s, double *out) {
   qipb200_ctx *ctx = s->ctx;
   CU(ctx, cudaSetDevice(ctx->device));
+  int st = materialise_collapse(s);
+  if (st != QIPB200_OK) return st;
   CU(ctx, launch_norm2(s->prec, s->buf, 1ull << s->n_local, ctx->d_scalar, ctx->stream, &ctx->launches));
-  int st = allreduce_sum(s, ctx->d_scalar, 1);
+  st = allreduce_sum(s, ctx->d_scalar, 1);
   if (st != QIPB200_OK) return st;
   CU(ctx, cudaMemcpyAsync(out, ctx->d_scalar, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
   CU(ctx, cudaStreamSynchronize(ctx->stream));
@@ -1250,6 +1315,9 @@ static int max_abs_diff_impl(qipb200_state *a, qipb200_state *b, double *out) {
   if (a->phys_of_logical != b->phys_of_logical)
     return set_err(ctx, QIPB200_ERR_UNSUPPORTED, "max_abs_diff: the two sharded states hold different qubit layouts");
   CU(ctx, cudaSetDevice(ctx->device));
+  int st = materialise_collapse(a);
+  if (st == QIPB200_OK) st = materialise_collapse(b);
+  if (st != QIPB200_OK) return st;
   CU(ctx, launch_max_abs_diff(a->prec, a->buf, b->buf, 1ull << a->n_local, ctx->d_scalar, ctx->stream, &ctx->launches));
   CU(ctx, cudaMemcpyAsync(out, ctx->d_scalar, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
   CU(ctx, cudaStreamSynchronize(ctx->stream));
@@ -1371,6 +1439,10 @@ const size_t kFileChunkBytes = 64u << 20;  // host bounce buffer: the shard neve
 int state_file_impl(qipb200_state *s, const char *path, bool save) {
   qipb200_ctx *ctx = s->ctx;
   CU(ctx, cudaSetDevice(ctx->device));
+  if (save) {
+    int st = materialise_collapse(s);
+    if (st != QIPB200_OK) return st;
+  }
   if (!layout_is_identity(s)) {  // files hold the canonical layout (collective on a sharded state)
     int st = restore_layout(s);
     if (st != QIPB200_OK) return st;
@@ -1391,6 +1463,7 @@ int state_file_impl(qipb200_state *s, const char *path, bool save) {
     else if (h.prec != (uint32_t)s->prec || h.n_qubits != s->n || h.rank != (uint32_t)s->rank || h.world != (uint32_t)s->world ||
              h.n_amplitudes != len)
       st = set_err(ctx, QIPB200_ERR_SIZE_MISMATCH, "state file does not match the target state (prec/n/rank/world/length)");
+    if (st == QIPB200_OK) s->collapse_pending = false;  // every amplitude is overwritten
   }
   std::vector<char> bounce;
   if (st == QIPB200_OK) bounce.resize((size_t)std::min<uint64_t>(kFileChunkBytes, len * ab));
@@ -1456,6 +1529,8 @@ int measure_probs_impl(qipb200_state *s, const uint64_t *indices, uint32_t n_ind
   if (s->world > 1 && (1u << n_indices) > (uint32_t)kCommDoubles)
     return set_err(ctx, QIPB200_ERR_UNSUPPORTED, "measure_probs on a sharded state: more than 16 measured qubits");
   CU(ctx, cudaSetDevice(ctx->device));
+  int st = materialise_collapse(s);
+  if (st != QIPB200_OK) return st;
   uint32_t bitpos[32];
   for (uint32_t i = 0; i < n_indices; ++i) bitpos[i] = s->phys_of_logical[s->n - 1 - (uint32_t)indices[i]];
   double *d_hist = nullptr;
@@ -1463,7 +1538,7 @@ int measure_probs_impl(qipb200_state *s, const uint64_t *indices, uint32_t n_ind
   CU(ctx, launch_measure_probs(s->prec, s->buf, 1ull << s->n_local, (uint64_t)s->rank << s->n_local, bitpos,
                                n_indices, d_hist, ctx->stream, &ctx->launches));
   // measurement_ops.rs:115-127 sums over the WHOLE vector: per-rank histograms are added across the ranks
-  int st = allreduce_sum(s, d_hist, 1u << n_indices);
+  st = allreduce_sum(s, d_hist, 1u << n_indices);
   if (st == QIPB200_OK)
     CU(ctx, cudaMemcpyAsync(out, d_hist, sizeof(double) << n_indices, cudaMemcpyDeviceToHost, ctx->stream));
   CU(ctx, cudaFreeAsync(d_hist, ctx->stream));
@@ -1522,6 +1597,8 @@ int local_scan(qipb200_state *s, double rem, bool *crossed, uint64_t *idx_out) {
 int soft_measure_impl(qipb200_state *s, const uint64_t *indices, uint32_t n_indices, double r, uint64_t *measured) {
   qipb200_ctx *ctx = s->ctx;
   CU(ctx, cudaSetDevice(ctx->device));
+  int st0 = materialise_collapse(s);
+  if (st0 != QIPB200_OK) return st0;
   uint64_t idx = 0;  // the reference leaves measured_indx = 0 when the scan never crosses
   if (s->world == 1) {
     bool crossed = false;
@@ -1589,8 +1666,10 @@ int sample_impl(qipb200_state *s, const uint64_t *indices, uint32_t n_indices, c
   qipb200_ctx *ctx = s->ctx;
   if (n_draws > 0xffffffffull) return set_err(ctx, QIPB200_ERR_UNSUPPORTED, "sample: more than 2^32-1 draws in one call");
   CU(ctx, cudaSetDevice(ctx->device));
+  int st = materialise_collapse(s);
+  if (st != QIPB200_OK) return st;
   if (!layout_is_identity(s)) {
-    int st = restore_layout(s);
+    st = restore_layout(s);
     if (st != QIPB200_OK) return st;
   }
   SampleBits bits;
@@ -1614,23 +1693,58 @@ int sample_impl(qipb200_state *s, const uint64_t *indices, uint32_t n_indices, c
 }
 
 int collapse_impl(qipb200_state *s, const uint64_t *indices, uint32_t n_indices, uint64_t measured, double measured_prob) {
-  qipb200_ctx *ctx = s->ctx;
+  CU(s->ctx, cudaSetDevice(s->ctx->device));
+  int st = materialise_collapse(s);
+  if (st != QIPB200_OK) return st;
   if (measured_prob == 0.0) return QIPB200_OK;  // measurement_ops.rs:230: untouched
+  return launch_collapse_on(s, indices, n_indices, measured, collapse_multiplier(s->prec, measured_prob));
+}
+
+// measure on an unsharded single-device state (kernels.cu: launch_measure): one upload of the draw or the forced
+// outcome, a fixed number of kernels, one download of {m, p}.  The collapse is left pending on the state.
+int measure_impl(qipb200_state *s, const uint64_t *indices, uint32_t n_indices, double r, uint32_t flags,
+                 uint64_t *measured, double *prob) {
+  qipb200_ctx *ctx = s->ctx;
   CU(ctx, cudaSetDevice(ctx->device));
-  uint64_t row_mask = 0, measured_mask = 0;
-  for (uint32_t i = 0; i < n_indices; ++i) {
-    const uint32_t bit = s->phys_of_logical[s->n - 1 - (uint32_t)indices[i]];
-    row_mask |= 1ull << bit;
-    measured_mask |= ((measured >> i) & 1ull) << bit;
+  int st = materialise_collapse(s);
+  if (st != QIPB200_OK) return st;
+  MeasureRecord rec = {(flags & QIPB200_MEASURE_FORCED) ? *measured : 0, 0.0};
+  if (flags & QIPB200_MEASURE_FORCED_PROB) {
+    rec.p = *prob;
+  } else if ((flags & QIPB200_MEASURE_FORCED) && n_indices < 64 && (rec.m >> n_indices)) {
+    rec.p = 0.0;  // measure_prob of an outcome the index list cannot produce
+  } else {
+    if (!layout_is_identity(s)) {  // the scan and the chunk sums run over canonical indices
+      st = restore_layout(s);
+      if (st != QIPB200_OK) return st;
+    }
+    SampleBits bits;
+    bits.n_bits = n_indices;
+    for (uint32_t i = 0; i < n_indices; ++i) bits.bitpos[i] = s->n - 1 - (uint32_t)indices[i];  // measurement_ops.rs:174-175
+    char *d = nullptr;
+    CU(ctx, cudaMallocAsync((void **)&d, 32 + measure_scratch_bytes(s->n_local), ctx->stream));
+    MeasureRecord *d_rec = (MeasureRecord *)d;
+    double *d_draw = (double *)(d + 16);
+    const bool forced = (flags & QIPB200_MEASURE_FORCED) != 0;
+    cudaError_t e = forced ? cudaMemcpyAsync(d_rec, &rec, sizeof(rec), cudaMemcpyHostToDevice, ctx->stream)
+                           : cudaMemcpyAsync(d_draw, &r, sizeof(r), cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess)
+      e = launch_measure(s->prec, s->buf, s->n_local, forced ? nullptr : d_draw, bits, d + 32, d_rec, ctx->sm_count,
+                         ctx->stream, &ctx->launches);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&rec, d_rec, sizeof(rec), cudaMemcpyDeviceToHost, ctx->stream);
+    cudaError_t ef = cudaFreeAsync(d, ctx->stream);
+    if (e != cudaSuccess) return cuda_fail(ctx, e, "measure");
+    CU(ctx, ef);
   }
-  // P::one() / measured_prob.sqrt() evaluated in the state's precision (measurement_ops.rs:231)
-  double p_mult;
-  if (s->prec == QIP_F32)
-    p_mult = (double)(1.0f / sqrtf((float)measured_prob));
-  else
-    p_mult = 1.0 / sqrt(measured_prob);
-  CU(ctx, launch_collapse(s->prec, s->buf, 1ull << s->n_local, (uint64_t)s->rank << s->n_local, row_mask,
-                          measured_mask, p_mult, ctx->stream, &ctx->launches));
+  CU(ctx, cudaStreamSynchronize(ctx->stream));
+  if (rec.p != 0.0) {  // measurement_ops.rs:230: a zero probability leaves the state untouched
+    s->pend_qubits.assign(indices, indices + n_indices);
+    s->pend_measured = rec.m;
+    s->pend_p_mult = collapse_multiplier(s->prec, rec.p);
+    s->collapse_pending = true;
+  }
+  *measured = rec.m;
+  *prob = rec.p;
   return QIPB200_OK;
 }
 
@@ -1694,6 +1808,32 @@ extern "C" int qipb200_state_sample(qipb200_state *s, const uint64_t *indices, u
     if (n_draws == 0) return (int)QIPB200_OK;
     if (!draws || !measured) return set_err(s->ctx, QIPB200_ERR_INVALID_ARG, "sample: NULL draws or measured");
     return sample_impl(s, indices, n_indices, draws, n_draws, measured);
+  });
+}
+
+extern "C" int qipb200_state_measure(qipb200_state *s, const uint64_t *indices, uint32_t n_indices, double r,
+                                     uint32_t flags, uint64_t *measured, double *prob) {
+  if (!s || !measured || !prob)
+    return set_err(s ? s->ctx : nullptr, QIPB200_ERR_INVALID_ARG, "measure: NULL argument");
+  return guarded(s->ctx, [&]() -> int {
+    if ((flags & ~(uint32_t)(QIPB200_MEASURE_FORCED | QIPB200_MEASURE_FORCED_PROB)) ||
+        ((flags & QIPB200_MEASURE_FORCED_PROB) && !(flags & QIPB200_MEASURE_FORCED)))
+      return set_err(s->ctx, QIPB200_ERR_INVALID_ARG, "measure: unknown flags, or FORCED_PROB without FORCED");
+    int st = check_indices(s, indices, n_indices);
+    if (st != QIPB200_OK) return st;
+    if (s->world == 1 && s->shards.empty()) return measure_impl(s, indices, n_indices, r, flags, measured, prob);
+    // sharded and multi-device states: the collective calls in turn, collapsing at once
+    uint64_t m = *measured;
+    double p = *prob;
+    if (!(flags & QIPB200_MEASURE_FORCED) && (st = qipb200_state_soft_measure(s, indices, n_indices, r, &m)) != QIPB200_OK)
+      return st;
+    if (!(flags & QIPB200_MEASURE_FORCED_PROB) && (st = qipb200_state_measure_prob(s, m, indices, n_indices, &p)) != QIPB200_OK)
+      return st;
+    if ((st = qipb200_state_collapse(s, indices, n_indices, m, p)) != QIPB200_OK) return st;
+    if ((st = qipb200_state_sync(s)) != QIPB200_OK) return st;
+    *measured = m;
+    *prob = p;
+    return (int)QIPB200_OK;
   });
 }
 

@@ -1578,6 +1578,100 @@ cudaError_t launch_sample(qip_prec prec, const void *psi, uint32_t n_local, cons
   return cudaGetLastError();
 }
 
+// ---------------------------------------------------------------------------------
+// measure: one draw, the probability of its outcome (qipb200_state_measure)
+// ---------------------------------------------------------------------------------
+// The outcome rec->m is on the device (written by launch_sample, or by the host for a forced outcome).  Measured
+// bits at index bits >= chunk_log2 select whole chunks; those below select amplitudes inside a chunk.
+
+struct MeasureMasks {
+  uint64_t hmask, hval;  // over the chunk index (index bit b >= chunk_log2 <-> chunk bit b - chunk_log2)
+  uint32_t lmask, lval;  // over the position inside a chunk
+};
+
+__device__ __forceinline__ MeasureMasks measure_masks(uint64_t m, const SampleBits &bits, uint32_t chunk_log2) {
+  MeasureMasks k = {0, 0, 0, 0};
+  for (uint32_t i = 0; i < bits.n_bits; ++i) {
+    const uint32_t b = bits.bitpos[i];
+    const uint64_t v = (m >> i) & 1ull;
+    if (b >= chunk_log2) {
+      k.hmask |= 1ull << (b - chunk_log2);
+      k.hval |= v << (b - chunk_log2);
+    } else {
+      k.lmask |= 1u << b;
+      k.lval |= (uint32_t)v << b;
+    }
+  }
+  return k;
+}
+
+// Some measured bit lies inside the chunks: parts[c] = sum of |a|^2 over the amplitudes of chunk c whose low measured
+// bits match, for every chunk c whose high bits match (the other entries are not written).  Nothing to do otherwise.
+template <typename R>
+__global__ void __launch_bounds__(kThreads)
+    k_measure_parts(const R *__restrict__ psi, uint32_t chunk_log2, uint64_t chunks, const MeasureRecord *rec,
+                    const __grid_constant__ SampleBits bits, double *__restrict__ parts) {
+  const MeasureMasks k = measure_masks(rec->m, bits, chunk_log2);
+  if (k.lmask == 0) return;
+  const uint32_t clen = 1u << chunk_log2;
+  for (uint64_t c = blockIdx.x; c < chunks; c += gridDim.x) {
+    if ((c & k.hmask) != k.hval) continue;
+    const R *src = psi + 2 * (c << chunk_log2);
+    double acc = 0.0;
+    for (uint32_t j = threadIdx.x; j < clen; j += kThreads) {
+      if ((j & k.lmask) != k.lval) continue;
+      typename Vec2<R>::type v = *reinterpret_cast<const typename Vec2<R>::type *>(src + 2 * j);
+      acc += (double)v.x * (double)v.x + (double)v.y * (double)v.y;
+    }
+    acc = block_sum(acc);
+    if (threadIdx.x == 0) parts[c] = acc;
+    __syncthreads();  // block_sum's shared slots are reused by the next chunk
+  }
+}
+
+// One CTA: rec->p = the sum, in chunk order, of the matching chunks' sums (parts[] when some measured bit is low).
+__global__ void __launch_bounds__(kThreads)
+    k_measure_reduce(const double *__restrict__ sums, const double *__restrict__ parts, uint32_t chunk_log2,
+                     uint64_t chunks, MeasureRecord *rec, const __grid_constant__ SampleBits bits) {
+  const MeasureMasks k = measure_masks(rec->m, bits, chunk_log2);
+  const double *src = k.lmask ? parts : sums;
+  double acc = 0.0;
+  for (uint64_t c = threadIdx.x; c < chunks; c += kThreads)
+    if ((c & k.hmask) == k.hval) acc += src[c];
+  acc = block_sum(acc);
+  if (threadIdx.x == 0) rec->p = acc;
+}
+
+size_t measure_scratch_bytes(uint32_t n_local) {
+  const uint64_t chunks = 1ull << (n_local - sample_chunk_log2(n_local));
+  return sample_scratch_bytes(n_local, 1) + 8 * chunks;
+}
+
+cudaError_t launch_measure(qip_prec prec, const void *psi, uint32_t n_local, const double *d_draw,
+                           const SampleBits &bits, void *d_scratch, MeasureRecord *d_rec, int sm_count, cudaStream_t s,
+                           uint64_t *launches) {
+  const uint32_t chunk_log2 = sample_chunk_log2(n_local);
+  const uint64_t len = 1ull << n_local, chunks = len >> chunk_log2;
+  const size_t sbytes = sample_scratch_bytes(n_local, 1);
+  const SampleScratch sc((char *)d_scratch, chunks, 1);  // launch_sample leaves the chunk sums in sc.sums
+  double *parts = (double *)((char *)d_scratch + sbytes);
+  cudaError_t e;
+  if (d_draw)
+    e = launch_sample(prec, psi, n_local, d_draw, 1, bits, d_scratch, &d_rec->m, sm_count, s, launches);
+  else
+    e = launch_chunk_sums(prec, psi, len, chunk_log2, sc.sums, s, launches);
+  if (e != cudaSuccess) return e;
+  const uint64_t cap = (uint64_t)(sm_count > 0 ? sm_count : 132) * 8;
+  const unsigned grid = (unsigned)(chunks < cap ? chunks : cap);
+  if (prec == QIP_F32)
+    k_measure_parts<float><<<grid, kThreads, 0, s>>>((const float *)psi, chunk_log2, chunks, d_rec, bits, parts);
+  else
+    k_measure_parts<double><<<grid, kThreads, 0, s>>>((const double *)psi, chunk_log2, chunks, d_rec, bits, parts);
+  k_measure_reduce<<<1, kThreads, 0, s>>>(sc.sums, parts, chunk_log2, chunks, d_rec, bits);
+  *launches += 2;
+  return cudaGetLastError();
+}
+
 template <typename R>
 __global__ void __launch_bounds__(kThreads)
     k_collapse(R *__restrict__ psi, uint64_t len, uint64_t index_base, uint64_t row_mask,

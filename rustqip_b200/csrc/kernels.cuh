@@ -75,6 +75,19 @@ size_t sample_scratch_bytes(uint32_t n_local, uint64_t n_draws);
 cudaError_t launch_sample(qip_prec prec, const void *psi, uint32_t n_local, const double *d_draws, uint64_t n_draws,
                           const SampleBits &bits, void *d_scratch, uint64_t *d_out, int sm_count, cudaStream_t s,
                           uint64_t *launches);
+// measure (qipb200_state_measure): the outcome m of one draw and its probability p, as one device record.
+// d_draw != nullptr: m is launch_sample's result for that draw; else m must already be in d_rec (a forced outcome)
+// and one read sweep computes the chunk sums.  p is summed in a fixed order from the chunk sums of the chunks whose
+// high bits match m, re-reading those chunks only when some measured bit lies below sample_chunk_log2.  The number
+// of kernels depends on nothing but d_draw.
+struct MeasureRecord {
+  uint64_t m;
+  double p;
+};
+size_t measure_scratch_bytes(uint32_t n_local);
+cudaError_t launch_measure(qip_prec prec, const void *psi, uint32_t n_local, const double *d_draw,
+                           const SampleBits &bits, void *d_scratch, MeasureRecord *d_rec, int sm_count, cudaStream_t s,
+                           uint64_t *launches);
 // measure_state: zero where (index & row_mask) != measured_mask, else scale by p_mult.
 cudaError_t launch_collapse(qip_prec prec, void *psi, uint64_t len, uint64_t index_base,
                             uint64_t row_mask, uint64_t measured_mask, double p_mult, cudaStream_t s,

@@ -3,6 +3,7 @@
 
 #include <algorithm>
 #include <cstdio>
+#include <cstring>
 
 namespace qipb200 {
 
@@ -319,3 +320,31 @@ void restrict_flat_op(const FlatOp &f_in, uint32_t n_local, int rank, FlatOp *ou
 }
 
 }  // namespace qipb200
+
+extern "C" void qipb200_collapse_ops(qip_prec prec, const uint64_t *qubits, uint32_t n_qubits, uint64_t measured,
+                                     double p_mult, qip_op *ops, void *dense) {
+  for (uint32_t i = 0; i < n_qubits; ++i) {
+    const uint64_t bit = (measured >> i) & 1ull;
+    const double keep = i == 0 ? p_mult : 1.0;
+    const double re[4] = {bit ? 0.0 : keep, 0.0, 0.0, bit ? keep : 0.0};  // row-major 2x2
+    for (int j = 0; j < 4; ++j) {
+      if (prec == QIP_F32) {
+        float *d = static_cast<float *>(dense) + 8 * i + 2 * j;
+        d[0] = (float)re[j];
+        d[1] = 0.0f;
+      } else {
+        double *d = static_cast<double *>(dense) + 8 * i + 2 * j;
+        d[0] = re[j];
+        d[1] = 0.0;
+      }
+    }
+    qip_op &op = ops[i];
+    memset(&op, 0, sizeof(op));
+    op.kind = QIP_OP_MATRIX;
+    op.n_indices = 1;
+    op.n_entries = 4;
+    op.indices = qubits + i;
+    op.dense = prec == QIP_F32 ? (const void *)(static_cast<float *>(dense) + 8 * i)
+                               : (const void *)(static_cast<double *>(dense) + 8 * i);
+  }
+}

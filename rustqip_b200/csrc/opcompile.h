@@ -71,3 +71,12 @@ void restrict_flat_op(const FlatOp &f_in, uint32_t n_local, int rank, FlatOp *ou
 int validate_op(const qip_op *op, qip_prec prec, uint32_t n_qubits, std::string *err);
 
 }  // namespace qipb200
+
+// The collapse of measure_state (measurement_ops.rs:220-269) as ordinary gates: one one-qubit diagonal QIP_OP_MATRIX
+// per measured qubit, diag(1, 0) where bit i of `measured` is 0 and diag(0, 1) where it is 1, the first op carrying
+// p_mult in place of its 1.  Their product zeroes the contradicting amplitudes and scales the others by p_mult, so a
+// fused schedule can apply a collapse inside its first tile pass.  ops[i] borrows qubits[i] and 4 complex<prec> of
+// `dense` (4 * n_qubits entries, written here); both must outlive the ops.  extern "C": the CPU planner tests call
+// this construction itself.
+extern "C" void qipb200_collapse_ops(qip_prec prec, const uint64_t *qubits, uint32_t n_qubits, uint64_t measured,
+                                     double p_mult, qip_op *ops, void *dense);

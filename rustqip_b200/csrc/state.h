@@ -81,6 +81,13 @@ struct qipb200_state {
   uint32_t epoch = 0;
   uint64_t exchange_bytes = 0;
   bool ipc_ready = false;
+  // Collapse left pending by qipb200_state_measure (unsharded single-device states only): measure_state over the
+  // logical qubits pend_qubits with outcome pend_measured and multiplier pend_p_mult.  The next fused schedule runs
+  // it as diagonal gates in its first tile pass; every other access to the amplitudes applies it first (api.cu).
+  bool collapse_pending = false;
+  std::vector<uint64_t> pend_qubits;
+  uint64_t pend_measured = 0;
+  double pend_p_mult = 1.0;
 };
 
 namespace qipb200 {

@@ -242,6 +242,31 @@ class State:
         idx = np.ascontiguousarray(np.asarray(list(indices), dtype=np.uint64))
         self._chk(_lib.lib().qipb200_state_collapse(self._h, _ptr(idx), len(idx), int(measured), float(prob)))
 
+    def measure(self, indices: Sequence[int], r: Optional[float] = None, measured: Optional[int] = None,
+                prob: Optional[float] = None, rng=None):
+        """measure (measurement_ops.rs:190-214): draw an outcome, take its probability, collapse; returns (m, p).
+
+        ``measured`` forces the outcome and ``prob`` (with ``measured`` only) its probability, as the reference's
+        MeasuredCondition does.  Otherwise the outcome is drawn with ``r`` in [0, 1), or with ``rng.random()`` (a
+        fresh ``np.random.default_rng()`` when None).  On an unsharded state the collapse costs no sweep of its own
+        when the next call is a fused apply_schedule."""
+        idx = np.ascontiguousarray(np.asarray(list(indices), dtype=np.uint64))
+        flags = 0
+        m, p = C.c_uint64(0), C.c_double(0.0)
+        if measured is not None:
+            flags |= _lib.MEASURE_FORCED
+            m.value = int(measured)
+            if prob is not None:
+                flags |= _lib.MEASURE_FORCED_PROB
+                p.value = float(prob)
+        elif prob is not None:
+            raise ValueError("measure: prob is only taken with measured")
+        elif r is None:
+            r = (rng if rng is not None else np.random.default_rng()).random()
+        self._chk(_lib.lib().qipb200_state_measure(self._h, _ptr(idx), len(idx), float(r or 0.0), flags, C.byref(m),
+                                                   C.byref(p)))
+        return int(m.value), float(p.value)
+
     # -- multi-GPU --------------------------------------------------------------
     def ipc_export(self):
         a = (C.c_ubyte * _lib.IPC_HANDLE_BYTES)()
