@@ -84,6 +84,26 @@ uint64_t qipb200_kernel_launches(const qipb200_ctx *ctx);
 /* out4 = { all kernels, fused tile passes, NVLink exchange kernels, reference ops folded into tile passes }. */
 int qipb200_launch_stats(const qipb200_ctx *ctx, uint64_t *out4);
 
+/* Per-gate kernels launched through `ctx` so far (qipb200_state_apply_op and unfused schedules), by kernel:
+ * out[QIPB200_KC_*] for the first min(n, QIPB200_KC_COUNT) entries.  Lets a caller see which kernel an op took,
+ * e.g. that it ran in place rather than on the out-of-place row kernel. */
+enum {
+  QIPB200_KC_DENSE = 0,      /* k_dense, k <= 4 in registers */
+  QIPB200_KC_DIAG = 1,       /* k_diag */
+  QIPB200_KC_DIAG_WIDE = 2,  /* k_diag_wide */
+  QIPB200_KC_EXCHANGE = 3,   /* k_exchange (X / CNOT / Toffoli-X / Swap pairs) */
+  QIPB200_KC_DENSE5 = 4,     /* k_dense5 */
+  QIPB200_KC_DENSE_DMMA = 5, /* k_dense_dmma (f64, k = 5, 6) */
+  QIPB200_KC_DENSE_BIG = 6,  /* k_dense_big */
+  QIPB200_KC_GATHER = 7,     /* k_gather, the out-of-place row kernel */
+  QIPB200_KC_COUNT = 8
+};
+int qipb200_kernel_counts(const qipb200_ctx *ctx, uint64_t *out, size_t n);
+
+/* Free the one state buffer the context keeps after a state is freed (for the next state of the same size), so
+ * that the device memory of freed states is returned at once.  The next state allocates afresh. */
+int qipb200_release_pool(qipb200_ctx *ctx);
+
 /* Generated kernels (absent in the reference): fused tile passes of big states are compiled by NVRTC into
  * kernels specialised to the pass (rustqip_b200/csrc/jit_codegen.cpp); a pass whose kernel is still being compiled
  * in the background runs the generic kernel meanwhile.  With wait != 0 this call blocks until the background

@@ -25,7 +25,7 @@ _lib = None
 # every symbol include/qipb200.h declares
 EXPORTS = [
     "qipb200_abi_version", "qipb200_init", "qipb200_init_multi", "qipb200_shutdown", "qipb200_last_error",
-    "qipb200_kernel_launches", "qipb200_launch_stats", "qipb200_stream_handle", "qipb200_jit_stats", "qipb200_jit_precompile", "qipb200_profile_enable", "qipb200_profile_read", "qipb200_validate_op", "qipb200_apply_op",
+    "qipb200_kernel_launches", "qipb200_launch_stats", "qipb200_kernel_counts", "qipb200_release_pool", "qipb200_stream_handle", "qipb200_jit_stats", "qipb200_jit_precompile", "qipb200_profile_enable", "qipb200_profile_read", "qipb200_validate_op", "qipb200_apply_op",
     "qipb200_apply_op_overwrite", "qipb200_apply_ops", "qipb200_state_new", "qipb200_state_free",
     "qipb200_state_set_basis", "qipb200_state_upload", "qipb200_state_download",
     "qipb200_state_apply_op", "qipb200_state_apply_schedule", "qipb200_state_norm2",
@@ -64,6 +64,8 @@ def lib():
     L.qipb200_profile_enable.restype, L.qipb200_profile_enable.argtypes = i32, [vp, i32]
     L.qipb200_profile_read.restype, L.qipb200_profile_read.argtypes = i32, [vp, vp]
     L.qipb200_kernel_launches.restype, L.qipb200_kernel_launches.argtypes = u64, [vp]
+    L.qipb200_kernel_counts.restype, L.qipb200_kernel_counts.argtypes = i32, [vp, vp, C.c_size_t]
+    L.qipb200_release_pool.restype, L.qipb200_release_pool.argtypes = i32, [vp]
     L.qipb200_validate_op.restype, L.qipb200_validate_op.argtypes = i32, [vp, i32, u32, opp]
     for name in ("qipb200_apply_op", "qipb200_apply_op_overwrite"):
         f = getattr(L, name)

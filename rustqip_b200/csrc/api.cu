@@ -282,6 +282,27 @@ extern "C" int qipb200_launch_stats(const qipb200_ctx *ctx, uint64_t *out4) {
   return QIPB200_OK;
 }
 
+extern "C" int qipb200_kernel_counts(const qipb200_ctx *ctx, uint64_t *out, size_t n) {
+  if (!ctx || (!out && n)) return set_err(ctx, QIPB200_ERR_INVALID_ARG, "kernel_counts: NULL argument");
+  for (size_t k = 0; k < n && k < (size_t)QIPB200_KC_COUNT; ++k) {
+    out[k] = ctx->kernel_counts[k];
+    for (size_t i = 0; i < ctx->children.size(); ++i) out[k] += ctx->children[i]->kernel_counts[k];
+  }
+  return QIPB200_OK;
+}
+
+extern "C" int qipb200_release_pool(qipb200_ctx *ctx) {
+  if (!ctx) return set_err(ctx, QIPB200_ERR_INVALID_ARG, "release_pool: NULL context");
+  for (size_t i = 0; i < ctx->children.size(); ++i) qipb200_release_pool(ctx->children[i]);
+  if (ctx->pool_buf) {
+    CU(ctx, cudaSetDevice(ctx->device));
+    CU(ctx, cudaFree(ctx->pool_buf));
+    ctx->pool_buf = nullptr;
+    ctx->pool_bytes = 0;
+  }
+  return QIPB200_OK;
+}
+
 // Host-only (no GPU, no context): plan `ops` for an n-qubit single-device state (sharded states plan with their own
 // geometry, f64 L = 5 instead of 4, so their passes are not among these programs), generate the specialised source
 // of every fused pass and compile it with NVRTC for sm_90a.  out[0] = passes planned, out[1] = passes the
@@ -724,25 +745,31 @@ int launch_local_op(qipb200_state *s, const FlatOp &f) {
       if (__builtin_popcountll(cm) > kMaxIns) break;
       if (f.diag_bits.size() <= (size_t)kMaxDiagParamK) {
         CU(ctx, launch_diag(s->prec, s->buf, nl, cm, f.diag_bits, f.diag, ctx->stream, &ctx->launches));
+        ++ctx->kernel_counts[QIPB200_KC_DIAG];
         return QIPB200_OK;
       }
       if (f.diag_bits.size() <= 10) {
         CU(ctx, launch_diag_wide(s->prec, s->buf, nl, cm, f.diag_bits, f.diag, ctx->stream, &ctx->launches));
+        ++ctx->kernel_counts[QIPB200_KC_DIAG_WIDE];
         return QIPB200_OK;
       }
       break;
     case CLASS_FLIP:
       CU(ctx, launch_flip(s->prec, s->buf, nl, cm, f.tgt_sorted[0], ctx->stream, &ctx->launches));
+      ++ctx->kernel_counts[QIPB200_KC_EXCHANGE];
       return QIPB200_OK;
     case CLASS_BITSWAP:
-      for (size_t i = 0; i < f.swaps.size(); ++i)
+      for (size_t i = 0; i < f.swaps.size(); ++i) {
         CU(ctx, launch_bitswap(s->prec, s->buf, nl, cm, f.swaps[i].first, f.swaps[i].second, ctx->stream,
                                &ctx->launches));
+        ++ctx->kernel_counts[QIPB200_KC_EXCHANGE];
+      }
       return QIPB200_OK;
     case CLASS_DENSE:
       if (f.tgt_sorted.size() <= (size_t)kMaxRegK &&
           __builtin_popcountll(cm) + f.tgt_sorted.size() <= (size_t)kMaxIns) {
         CU(ctx, launch_dense(s->prec, s->buf, nl, f, ctx->stream, &ctx->launches));
+        ++ctx->kernel_counts[QIPB200_KC_DENSE];
         return QIPB200_OK;
       }
       // k = 5..10 in place (the reference applies any k through the same row loop, qubit_iterators.rs:23-55)
@@ -750,6 +777,10 @@ int launch_local_op(qipb200_state *s, const FlatOp &f) {
           __builtin_popcountll(cm) + f.tgt_sorted.size() <= (size_t)kMaxIns && nl >= f.tgt_sorted.size() + __builtin_popcountll(cm) &&
           (f.tgt_sorted.size() == 5 || nl - (uint32_t)__builtin_popcountll(cm) >= 8)) {
         CU(ctx, launch_dense_wide(s->prec, s->buf, nl, f, ctx->stream, &ctx->launches));
+        const DenseWideKind kind = dense_wide_kind(s->prec, nl, f);
+        ++ctx->kernel_counts[kind == DENSE_WIDE_DMMA ? QIPB200_KC_DENSE_DMMA
+                             : kind == DENSE_WIDE_5  ? QIPB200_KC_DENSE5
+                                                     : QIPB200_KC_DENSE_BIG];
         return QIPB200_OK;
       }
       break;
@@ -766,6 +797,7 @@ int launch_local_op(qipb200_state *s, const FlatOp &f) {
   }
   const uint64_t len = 1ull << nl;
   CU(ctx, launch_gather(s->prec, f, s->n, s->buf, len, 0, s->scratch, len, 0, false, ctx->stream, &ctx->launches));
+  ++ctx->kernel_counts[QIPB200_KC_GATHER];
   std::swap(s->buf, s->scratch);  // `Ok((arena, state, ..))`, builder.rs:514
   return QIPB200_OK;
 }

@@ -454,6 +454,13 @@ static bool dense_dmma_enabled() {
   return on;
 }
 
+DenseWideKind dense_wide_kind(qip_prec prec, uint32_t n_local, const FlatOp &f) {
+  const uint32_t K = (uint32_t)f.tgt_sorted.size();
+  const uint32_t n_ins = K + (uint32_t)__builtin_popcountll(f.ctrl_mask);
+  if (prec == QIP_F64 && (K == 5 || K == 6) && n_local >= n_ins + 4 && dense_dmma_enabled()) return DENSE_WIDE_DMMA;
+  return K == 5 ? DENSE_WIDE_5 : DENSE_WIDE_BIG;
+}
+
 template <typename R>
 static cudaError_t launch_dense_wide_t(R *psi, uint32_t n_local, const FlatOp &f, cudaStream_t s, uint64_t *launches) {
   const uint32_t K = (uint32_t)f.tgt_sorted.size();
@@ -474,7 +481,7 @@ static cudaError_t launch_dense_wide_t(R *psi, uint32_t n_local, const FlatOp &f
     return e;
   }
   const uint32_t n_ins = K + (uint32_t)__builtin_popcountll(f.ctrl_mask);
-  if (sizeof(R) == 8 && (K == 5 || K == 6) && n_local >= n_ins + 4 && dense_dmma_enabled()) {
+  if (dense_wide_kind(sizeof(R) == 8 ? QIP_F64 : QIP_F32, n_local, f) == DENSE_WIDE_DMMA) {
     e = K == 5 ? launch_dense_dmma<5, 2>((double *)psi, n_local, f, (const double *)d_mat, s)
                : launch_dense_dmma<6, 1>((double *)psi, n_local, f, (const double *)d_mat, s);
     ++*launches;

@@ -25,6 +25,10 @@ cudaError_t launch_diag(qip_prec prec, void *psi, uint32_t n_local, uint64_t ctr
 // through shared memory, matrix through L1/L2), and diagonals on 5..10 bits (table in shared memory).
 cudaError_t launch_dense_wide(qip_prec prec, void *psi, uint32_t n_local, const FlatOp &f, cudaStream_t s,
                               uint64_t *launches);
+// The kernel launch_dense_wide runs for `f`: DENSE_WIDE_DMMA (k_dense_dmma), DENSE_WIDE_5 (k_dense5) or
+// DENSE_WIDE_BIG (k_dense_big).
+enum DenseWideKind { DENSE_WIDE_DMMA, DENSE_WIDE_5, DENSE_WIDE_BIG };
+DenseWideKind dense_wide_kind(qip_prec prec, uint32_t n_local, const FlatOp &f);
 cudaError_t launch_diag_wide(qip_prec prec, void *psi, uint32_t n_local, uint64_t ctrl_mask,
                              const std::vector<uint32_t> &bits, const std::vector<cplx> &d, cudaStream_t s,
                              uint64_t *launches);

@@ -8,6 +8,7 @@
 #include <utility>
 #include <vector>
 
+#include "../../include/qipb200.h"
 #include "jit_runtime.h"
 #include "opcompile.h"
 
@@ -35,6 +36,8 @@ struct qipb200_ctx {
   // 2^n amplitudes per call otherwise)
   void *pool_buf = nullptr;
   size_t pool_bytes = 0;
+  // per-gate kernel launches by kernel (qipb200_kernel_counts; index = QIPB200_KC_*)
+  uint64_t kernel_counts[QIPB200_KC_COUNT] = {};
   bool tile_configured = false;    // the tile kernels' > 48 KiB shared-memory opt-in was done on this device
   // optional per-category device timing (qipb200_profile_enable): CUDA-event pairs recorded on `stream`
   // around every fused tile pass [0] and every NVLink exchange incl. its two flag barriers [1]

@@ -75,6 +75,18 @@ class Context:
     def kernel_launches(self) -> int:
         return int(_lib.lib().qipb200_kernel_launches(self._h))
 
+    KERNELS = ("k_dense", "k_diag", "k_diag_wide", "k_exchange", "k_dense5", "k_dense_dmma", "k_dense_big", "k_gather")
+
+    def kernel_counts(self):
+        """dict kernel name -> per-gate launches of that kernel so far (apply_op and unfused schedules)."""
+        out = (C.c_uint64 * len(self.KERNELS))()
+        _lib.check(_lib.lib().qipb200_kernel_counts(self._h, out, len(self.KERNELS)), self._h)
+        return {k: int(v) for k, v in zip(self.KERNELS, out)}
+
+    def release_pool(self):
+        """Return the buffer kept from the last freed state to the device (the next state allocates afresh)."""
+        _lib.check(_lib.lib().qipb200_release_pool(self._h), self._h)
+
     def close(self):
         if self._h:
             _lib.lib().qipb200_shutdown(self._h)

@@ -50,7 +50,8 @@ def test_wide_dense_and_diagonal_in_place(ctx, dtype):
 
 def test_wide_dense_f64_smallest_states(ctx):
     """The f64 5/6-qubit blocks go to the tensor pipe (k_dense_dmma) from 16 groups per shard on; below that the FMA
-    kernels take over.  Both sides of the switch, and the env override, against the oracle."""
+    kernels take over.  Both sides of the switch against the oracle.  The QIPB200_DENSE_DMMA=0 override is read once
+    per process; tests/test_gpu_full_size.py::test_dense_f64_fma_kernels_with_dmma_off runs it in a child process."""
     rng = np.random.default_rng(78)
     for n, k in [(9, 5), (8, 5), (7, 5), (10, 6), (9, 6), (11, 6), (12, 5)]:
         psi = rand_state(n, np.complex128, 16 + n)
