@@ -261,6 +261,23 @@ enum {
 int qipb200_state_measure(qipb200_state *state, const uint64_t *indices, uint32_t n_indices, double r,
                           uint32_t flags, uint64_t *measured, double *prob);
 
+/* <psi|P_t|psi> for n_terms Pauli strings on the state AS IT IS (not renormalised, like measure_probs); absent in the
+ * reference.  Term t is the term_len[t] pairs (qubits[k], paulis[k]) that follow term t-1 in the flat arrays.  The
+ * letters are 'X', 'Y' and 'Z' (else QIPB200_ERR_INVALID_ARG), a qubit >= n or repeated inside one term gives
+ * QIPB200_ERR_BAD_INDEX, NULL arrays with n_terms > 0 give QIPB200_ERR_INVALID_ARG, n_terms == 0 is a no-op, and an
+ * empty term is the identity (= norm2).  out[t] (HOST, n_terms doubles) is real: P_t is Hermitian, and the imaginary
+ * part is rounding and is not returned.  Deterministic (same state and terms -> bit-identical out), accumulated in
+ * double for both precisions, synchronises.  A read sweep carries up to 16384 terms: terms with equal X/Y masks share
+ * one sweep (a mask with more than 16384 terms takes one per 16384), Z-only terms fill the room of the other sweeps and
+ * take one sweep per 16384 of what is left, and distinct masks share a sweep when their bits fit one tile
+ * (qipb200_expect_plan reports the count); one kernel per sweep plus one reduction kernel per batch of sweeps of at
+ * most 16384 terms, so the device scratch stays below 35 MB for any number of terms.  A pending collapse is applied first; a permuted
+ * layout is read as it is.  Sharded and multi-device states: QIPB200_ERR_UNSUPPORTED. */
+int qipb200_state_expect_paulis(qipb200_state *state, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms, double *out);
+/* Host-only (no GPU, ctx-free), like qipb200_plan_exchanges: the number of read sweeps the call above makes for these
+ * terms on an unsharded n-qubit state in canonical layout (0 for n_terms == 0).  Validates as the call above does. */
+int qipb200_expect_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms, uint32_t *sweeps);
+
 /* ---- multi-GPU: the 2^n state sharded by its top log2(world) index bits,
  *      one process per GPU (absent in the reference; its only hook is the
  *      input_offset/output_offset slice model, matrix_ops.rs:74-89) -------------- */

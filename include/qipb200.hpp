@@ -251,6 +251,28 @@ class B200State {
     ctx_.check(qipb200_state_measure_probs(st_, indices.data(), (uint32_t)indices.size(), out.data()));
     return out;
   }
+  // <psi|P_t|psi> for Pauli strings, each a list of (letter, qubit) pairs, e.g. {{'Z', 0}, {'Z', 1}} (absent in the
+  // reference); weighted sums are the caller's dot product
+  std::vector<double> expect_paulis(const std::vector<std::vector<std::pair<char, uint64_t>>> &terms) {
+    std::vector<uint64_t> qubits;
+    std::vector<char> letters;
+    std::vector<uint32_t> lens;
+    for (const auto &t : terms) {
+      lens.push_back((uint32_t)t.size());
+      for (const auto &lq : t) {
+        letters.push_back(lq.first);
+        qubits.push_back(lq.second);
+      }
+    }
+    std::vector<double> out(terms.size());
+    // a list of identities has no letters: pass non-NULL (unread) arrays, the C entry refuses NULL ones
+    const uint64_t no_qubit = 0;
+    const char no_letter = 'Z';
+    ctx_.check(qipb200_state_expect_paulis(st_, qubits.empty() ? &no_qubit : qubits.data(),
+                                           letters.empty() ? &no_letter : letters.data(), lens.data(), terms.size(),
+                                           out.data()));
+    return out;
+  }
   // a schedule parsed from the QIPS wire format (owned by the library): builder.rs:423-514 on foreign circuits
   void apply_parsed(const qip_op *ops, size_t n_ops, bool fusion = true) {
     ctx_.check(qipb200_state_apply_schedule(st_, ops, n_ops, fusion ? QIPB200_SCHED_DEFAULT : QIPB200_SCHED_NO_FUSION));

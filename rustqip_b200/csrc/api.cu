@@ -19,6 +19,7 @@
 
 #include "../../include/qipb200.h"
 #include "dist.cuh"
+#include "expect.h"
 #include "kernels.cuh"
 #include "opcompile.h"
 #include "schedule.h"
@@ -1878,6 +1879,63 @@ extern "C" int qipb200_state_collapse(qipb200_state *s, const uint64_t *indices,
     if (!s->shards.empty())
       return each_shard(s, [&](qipb200_state *sh, int) { return collapse_impl(sh, indices, n_indices, measured, measured_prob); });
     return collapse_impl(s, indices, n_indices, measured, measured_prob);
+  });
+}
+
+// ===================================================================================
+// Pauli-string expectation values (expect.cu)
+// ===================================================================================
+
+namespace {
+
+int expect_impl(qipb200_state *s, const std::vector<PauliTerm> &terms, double *out) {
+  qipb200_ctx *ctx = s->ctx;
+  CU(ctx, cudaSetDevice(ctx->device));
+  int st = materialise_collapse(s);
+  if (st != QIPB200_OK) return st;
+  // A state left permuted (QIPB200_ROTATE) needs no restore_layout sweep: Pauli masks permute with the bits.
+  std::vector<PauliTerm> phys(terms.size());
+  for (size_t t = 0; t < terms.size(); ++t) {
+    phys[t].n_y = terms[t].n_y;
+    for (uint32_t b = 0; b < s->n; ++b) {
+      const uint64_t p = 1ull << s->phys_of_logical[b];
+      if ((terms[t].x >> b) & 1) phys[t].x |= p;
+      if ((terms[t].z >> b) & 1) phys[t].z |= p;
+    }
+  }
+  CU(ctx, run_expect(s->prec, s->buf, s->n_local, phys, out, ctx->stream, &ctx->launches));
+  return QIPB200_OK;
+}
+
+}  // namespace
+
+extern "C" int qipb200_state_expect_paulis(qipb200_state *s, const uint64_t *qubits, const char *paulis,
+                                           const uint32_t *term_len, size_t n_terms, double *out) {
+  if (!s) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, "expect_paulis: NULL state");
+  return guarded(s->ctx, [&]() -> int {
+    std::vector<PauliTerm> terms;
+    std::string err;
+    int st = parse_pauli_terms(s->n, qubits, paulis, term_len, n_terms, &terms, &err);
+    if (st != QIPB200_OK) return set_err(s->ctx, st, err);
+    if (s->world > 1 || !s->shards.empty())
+      return set_err(s->ctx, QIPB200_ERR_UNSUPPORTED, "expect_paulis: sharded states are not supported");
+    if (n_terms == 0) return (int)QIPB200_OK;
+    if (!out) return set_err(s->ctx, QIPB200_ERR_INVALID_ARG, "expect_paulis: NULL out");
+    return expect_impl(s, terms, out);
+  });
+}
+
+extern "C" int qipb200_expect_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, const char *paulis,
+                                   const uint32_t *term_len, size_t n_terms, uint32_t *sweeps) {
+  if (!sweeps || (prec != QIP_F32 && prec != QIP_F64) || n_qubits == 0 || n_qubits > 40)
+    return set_err(nullptr, QIPB200_ERR_INVALID_ARG, "expect_plan: NULL sweeps, bad precision or n_qubits not in 1..40");
+  return guarded(nullptr, [&]() -> int {
+    std::vector<PauliTerm> terms;
+    std::string err;
+    int st = parse_pauli_terms(n_qubits, qubits, paulis, term_len, n_terms, &terms, &err);
+    if (st != QIPB200_OK) return set_err(nullptr, st, err);
+    *sweeps = expect_sweep_count(n_qubits, terms);
+    return (int)QIPB200_OK;
   });
 }
 

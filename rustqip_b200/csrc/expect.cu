@@ -1,0 +1,584 @@
+// expect.cu -- <psi|P|psi> for many Pauli strings P per read sweep of the state (qipb200_state_expect_paulis).
+//
+// Write P = i^nY X^x Z^z (x: index-bit mask of the X/Y letters, z: of the Z/Y letters).  Then
+//   <P> = i^nY * sum_j (-1)^popc(j & z) * c_j,   c_j = conj(a_{j^x}) a_j,
+// so terms with the same x share the products c_j and differ only in the sign pattern.
+//
+// Sweep = tile geometry + x_out.  A tile is the kExpL lowest index bits plus up to kExpM chosen high bits (2^11
+// amplitudes, read as runs of 16 contiguous amplitudes).  Each mask splits as x = x_in ^ x_out with x_in on tile bits;
+// the masks of one sweep share x_out.  With x_out == 0 a CTA holds one tile; otherwise it holds the pair of tiles
+// (B, B ^ x_out), visited once from the side whose lowest x_out bit is clear: the partner's half of the sum is
+// (-1)^popc(x & z) * conj(sum over B), so every amplitude is still read exactly once per sweep.
+//
+// Per mask group the CTA forms c over its tile in registers, then either
+//   - "direct": each of at most kExpMaxDirect terms of the sweep is a signed sum per thread, kept in a register
+//     accumulator across the tiles the CTA walks (groups of few terms, e.g. the single X_i of an Ising field), or
+//   - "WHT": an in-place Walsh-Hadamard transform of c over the 11 tile bits (3 stages in registers, 5 through warp
+//     shuffles, 3 through shared memory); every term is then one shared-memory read at its tile-local z pattern,
+//     added by the thread that owns the term into a shared-memory accumulator.
+// z bits outside the tile give a CTA-uniform sign, popc(tile_base & z_out).  Only the real part of i^nY * sum is
+// kept (P is Hermitian): each term accumulates one real component with a coefficient in {0, +-1, +-2}.
+//
+// Determinism: a fixed grid of kExpGrid CTAs with a static tile assignment, per-thread accumulation in tile order,
+// shuffle/shared-memory block sums in a fixed order, per-CTA partials [CTA][term] summed by one reduction kernel in
+// CTA order.  No floating-point atomics.
+//
+// Terms per sweep: up to kExpBatchTerms.  The first kExpSmemTerms accumulators of a sweep live in shared memory, the
+// rest in the CTA's own column of the partials (each owned by one thread, so still no atomics).  A mask group of more
+// than kExpBatchTerms terms takes one sweep per kExpBatchTerms of them; Z-only terms fill the room the other sweeps
+// leave before opening sweeps of their own.
+//
+// Scratch: at most kExpBatchTerms rows per batch, 8 B per row and CTA (34.6 MB for kExpGrid = 264) plus the term
+// tables; a longer term list runs in several batches, each with its own reduction kernel.  Shared memory: at most
+// 111.4 KiB per CTA (f64 tile pair), so two CTAs fit on an SM.
+#include "expect.h"
+
+#include <algorithm>
+#include <cstdio>
+#include <map>
+
+#include "../../include/qipb200.h"
+
+namespace qipb200 {
+
+namespace {
+
+const uint32_t kExpL = 4;               // low index bits of a tile (runs of 16 amplitudes)
+const uint32_t kExpM = 7;               // chosen high bits of a tile
+const uint32_t kExpTileLog2 = kExpL + kExpM;
+const uint32_t kExpTile = 1u << kExpTileLog2;
+const int kExpThreads = 256;
+const int kExpPer = kExpTile / kExpThreads;  // tile amplitudes per thread (8: three in-register WHT stages)
+const uint32_t kExpMaxDirect = 16;      // register accumulators per thread
+const uint32_t kExpDirectGroupTerms = 4;  // groups of at most this many terms are evaluated directly
+const uint32_t kExpBatchTerms = 16384;  // terms per reduction batch, and so per sweep
+const uint32_t kExpSmemTerms = 1024;    // accumulators in shared memory; a sweep's later terms accumulate in global
+const uint32_t kExpSmemGroups = 256;    // group descriptors staged in shared memory; later ones are read from global
+const int kExpGrid = 264;               // CTAs per sweep: two per SM of a 132-SM H100
+static_assert(kExpPer == 8, "the WHT below assumes 8 amplitudes per thread");
+
+struct ExpGroupDev {
+  uint32_t x_in;          // tile-local X/Y mask
+  uint32_t diag;          // x == 0: c_j = |a_j|^2
+  uint32_t first, end;    // the group's terms (sweep-local)
+  uint32_t dfirst, dend;  // its direct slots (empty: WHT)
+};
+
+struct ExpTermDev {
+  uint64_t z_out;  // Z/Y bits outside the tile
+  uint32_t z_in;   // tile-local Z/Y pattern
+  uint32_t comp;   // 0: real part, 1: imaginary part of the sum
+  double coef;     // sign of i^nY on that component, times (1 +- eta) on the tile-pair path
+};
+
+struct ExpArgs {
+  uint64_t x_out;     // 0, or the out-of-tile X/Y mask shared by the sweep
+  uint64_t n_visits;  // tiles (x_out == 0) or tile pairs
+  uint32_t L, tb;     // low bits, tile bits
+  uint32_t n_out;     // bits of the visit index, spread over out_pos
+  uint32_t n_groups, n_terms, n_direct;
+  uint32_t row_off;   // partial row of the sweep's first term in the batch
+  uint32_t rows;      // rows of the batch (length of a CTA's column of partials)
+  uint8_t hi_pos[kExpM];
+  uint8_t out_pos[64];
+  uint16_t direct_term[kExpMaxDirect];
+  ExpTermDev direct[kExpMaxDirect];  // the direct slots' terms (staged in shared memory by every CTA)
+};
+
+template <typename R>
+struct ExpV;
+template <>
+struct ExpV<float> {
+  typedef float2 type;
+};
+template <>
+struct ExpV<double> {
+  typedef double2 type;
+};
+
+__device__ __forceinline__ double parity_sign(uint64_t v) { return (__popcll(v) & 1) ? -1.0 : 1.0; }
+
+template <int NC>
+__device__ __forceinline__ void butterflies8(double (&c)[kExpPer][2]) {
+#pragma unroll
+  for (int s = 1; s < kExpPer; s <<= 1)
+#pragma unroll
+    for (int k = 0; k < kExpPer; ++k)
+      if (!(k & s))
+#pragma unroll
+        for (int q = 0; q < NC; ++q) {
+          const double u = c[k][q], v = c[k | s][q];
+          c[k][q] = u + v;
+          c[k | s][q] = u - v;
+        }
+}
+
+// Walsh-Hadamard transform over the 11 tile-local bits of c (thread t holds elements t + 256 k) into cbuf[e*NC+q]:
+// bits 8-10 in registers, bits 0-4 through shuffles, bits 5-7 after a transpose through cbuf.
+template <int NC>
+__device__ __forceinline__ void wht_tile(double (&c)[kExpPer][2], double *cbuf) {
+  const int t = threadIdx.x, lane = t & 31;
+  butterflies8<NC>(c);
+#pragma unroll
+  for (int b = 1; b < 32; b <<= 1)
+#pragma unroll
+    for (int k = 0; k < kExpPer; ++k)
+#pragma unroll
+      for (int q = 0; q < NC; ++q) {
+        const double p = __shfl_xor_sync(0xffffffffu, c[k][q], b);
+        c[k][q] = (lane & b) ? p - c[k][q] : c[k][q] + p;
+      }
+  __syncthreads();  // the previous group's readers of cbuf are done
+#pragma unroll
+  for (int k = 0; k < kExpPer; ++k)
+#pragma unroll
+    for (int q = 0; q < NC; ++q) cbuf[(t + kExpThreads * k) * NC + q] = c[k][q];
+  __syncthreads();
+  const int e0 = lane | ((t >> 5) << 8);
+#pragma unroll
+  for (int k = 0; k < kExpPer; ++k)
+#pragma unroll
+    for (int q = 0; q < NC; ++q) c[k][q] = cbuf[(e0 | (k << 5)) * NC + q];
+  butterflies8<NC>(c);
+#pragma unroll
+  for (int k = 0; k < kExpPer; ++k)
+#pragma unroll
+    for (int q = 0; q < NC; ++q) cbuf[(e0 | (k << 5)) * NC + q] = c[k][q];
+  __syncthreads();
+}
+
+template <typename R>
+__global__ void __launch_bounds__(kExpThreads, 2)
+    k_expect(const R *__restrict__ psi, const __grid_constant__ ExpArgs a, const ExpGroupDev *__restrict__ groups,
+             const ExpTermDev *__restrict__ terms, double *__restrict__ partials) {
+  typedef typename ExpV<R>::type V;
+  extern __shared__ __align__(16) unsigned char smem[];
+  const bool pair = a.x_out != 0;
+  V *sA = reinterpret_cast<V *>(smem);
+  V *sP = sA + kExpTile;
+  double *cbuf = reinterpret_cast<double *>(smem + (pair ? 2 : 1) * kExpTile * sizeof(V));
+  double *red = cbuf + 2 * kExpTile;                          // [warp][direct slot]
+  const uint32_t n_smem_terms = min(a.n_terms, kExpSmemTerms), n_smem_groups = min(a.n_groups, kExpSmemGroups);
+  double *acc_s = red + (kExpThreads / 32) * kExpMaxDirect;                  // [sweep term < kExpSmemTerms]
+  ExpTermDev *sd = reinterpret_cast<ExpTermDev *>(acc_s + n_smem_terms);     // the direct slots' terms
+  ExpGroupDev *sg = reinterpret_cast<ExpGroupDev *>(sd + kExpMaxDirect);   // the first groups
+  // this CTA's column of the batch's partials [CTA][row]; the accumulators of terms >= kExpSmemTerms live there
+  double *gcol = partials + (uint64_t)blockIdx.x * a.rows + a.row_off;
+  const int t = threadIdx.x;
+  if ((uint32_t)t < kExpMaxDirect) sd[t] = a.direct[t];
+  for (uint32_t i = t; i < n_smem_terms; i += kExpThreads) acc_s[i] = 0.0;
+  for (uint32_t i = kExpSmemTerms + t; i < a.n_terms; i += kExpThreads) gcol[i] = 0.0;
+  for (uint32_t i = t; i < n_smem_groups; i += kExpThreads) sg[i] = groups[i];
+  double acc[kExpMaxDirect];
+#pragma unroll
+  for (uint32_t d = 0; d < kExpMaxDirect; ++d) acc[d] = 0.0;
+  const uint32_t tsize = 1u << a.tb;
+  uint64_t off[kExpPer];
+#pragma unroll
+  for (int k = 0; k < kExpPer; ++k) {
+    const uint32_t e = t + kExpThreads * k;
+    uint64_t o = e & ((1u << a.L) - 1);
+    for (uint32_t i = 0; i < a.tb - a.L; ++i) o |= (uint64_t)((e >> (a.L + i)) & 1u) << a.hi_pos[i];
+    off[k] = o;
+  }
+  for (uint64_t v = blockIdx.x; v < a.n_visits; v += gridDim.x) {
+    uint64_t base = 0;
+    for (uint32_t i = 0; i < a.n_out; ++i) base |= ((v >> i) & 1ull) << a.out_pos[i];
+    __syncthreads();  // the previous tile's readers are done
+#pragma unroll
+    for (int k = 0; k < kExpPer; ++k) {
+      const uint32_t e = t + kExpThreads * k;
+      V u, w;
+      u.x = u.y = w.x = w.y = (R)0;
+      if (e < tsize) {
+        u = *reinterpret_cast<const V *>(psi + 2 * (base | off[k]));
+        if (pair) w = *reinterpret_cast<const V *>(psi + 2 * ((base ^ a.x_out) | off[k]));
+      }
+      sA[e] = u;
+      if (pair) sP[e] = w;
+    }
+    __syncthreads();
+    for (uint32_t g = 0; g < a.n_groups; ++g) {
+      const ExpGroupDev G = g < kExpSmemGroups ? sg[g] : groups[g];
+      const int sides = (G.diag && pair) ? 2 : 1;  // the diagonal group sums over both tiles of a pair
+      for (int side = 0; side < sides; ++side) {
+        const uint64_t sbase = side ? base ^ a.x_out : base;
+        double c[kExpPer][2];
+#pragma unroll
+        for (int k = 0; k < kExpPer; ++k) {
+          const uint32_t e = t + kExpThreads * k;
+          if (G.diag) {
+            const V u = (side ? sP : sA)[e];
+            c[k][0] = (double)u.x * (double)u.x + (double)u.y * (double)u.y;
+            c[k][1] = 0.0;
+          } else {
+            const V u = sA[e];
+            const V w = (pair ? sP : sA)[e ^ G.x_in];
+            c[k][0] = (double)w.x * (double)u.x + (double)w.y * (double)u.y;  // conj(w) * u
+            c[k][1] = (double)w.x * (double)u.y - (double)w.y * (double)u.x;
+          }
+        }
+        if (G.dend > G.dfirst) {
+#pragma unroll
+          for (uint32_t d = 0; d < kExpMaxDirect; ++d) {
+            if (d < G.dfirst || d >= G.dend) continue;
+            const uint32_t z_in = sd[d].z_in, comp = sd[d].comp;
+            double s = 0.0;
+#pragma unroll
+            for (int k = 0; k < kExpPer; ++k) {
+              const double cv = comp ? c[k][1] : c[k][0];
+              s += (__popc((t + kExpThreads * k) & z_in) & 1) ? -cv : cv;
+            }
+            acc[d] += sd[d].coef * parity_sign(sbase & sd[d].z_out) * s;
+          }
+        } else {
+          if (G.diag)
+            wht_tile<1>(c, cbuf);
+          else
+            wht_tile<2>(c, cbuf);
+          const uint32_t nc = G.diag ? 1 : 2;
+          for (uint32_t i = G.first + t; i < G.end; i += kExpThreads) {
+            const ExpTermDev T = terms[i];
+            const double v = T.coef * parity_sign(sbase & T.z_out) * cbuf[T.z_in * nc + T.comp];
+            if (i < kExpSmemTerms)
+              acc_s[i] += v;
+            else
+              gcol[i] += v;  // owned by this thread like the shared-memory ones: coalesced, no atomics
+          }
+        }
+      }
+    }
+  }
+  // direct slots: warp sums, then the warps in order
+  const int lane = t & 31, warp = t >> 5;
+#pragma unroll
+  for (uint32_t d = 0; d < kExpMaxDirect; ++d) {
+    double v = acc[d];
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+    if (lane == 0) red[warp * kExpMaxDirect + d] = v;
+  }
+  __syncthreads();
+  if ((uint32_t)t < a.n_direct) {
+    double s = 0.0;
+    for (int w = 0; w < kExpThreads / 32; ++w) s += red[w * kExpMaxDirect + t];
+    acc_s[a.direct_term[t]] = s;  // the direct groups come first in a sweep: their terms are < kExpMaxDirect
+  }
+  __syncthreads();
+  for (uint32_t i = t; i < n_smem_terms; i += kExpThreads) gcol[i] = acc_s[i];
+}
+
+__global__ void __launch_bounds__(256) k_expect_reduce(const double *__restrict__ partials, uint32_t rows, uint32_t grid,
+                                                        double *__restrict__ res) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= rows) return;
+  double s = 0.0;
+  for (uint32_t c = 0; c < grid; ++c) s += partials[(uint64_t)c * rows + r];
+  res[r] = s;
+}
+
+// ---- host: grouping and greedy packing ----------------------------------------------
+
+struct Group {
+  uint64_t x = 0;
+  std::vector<uint32_t> terms;
+  bool direct = false;
+};
+
+struct Sweep {
+  uint64_t hi = 0;     // chosen high tile bits
+  uint64_t x_out = 0;  // out-of-tile X/Y bits shared by every group
+  uint32_t n_terms = 0;
+  std::vector<Group> groups;
+};
+
+int popc64(uint64_t v) { return __builtin_popcountll(v); }
+
+void plan_sweeps(uint32_t n, const std::vector<PauliTerm> &terms, std::vector<Sweep> *out) {
+  const uint32_t L = std::min(kExpL, n), m = std::min(kExpM, n - L);
+  const uint64_t low = (1ull << L) - 1;
+  // groups of equal X/Y mask in order of first appearance, cut into units of at most kExpBatchTerms terms
+  std::vector<Group> all;
+  std::map<uint64_t, size_t> where;
+  for (uint32_t t = 0; t < (uint32_t)terms.size(); ++t) {
+    auto it = where.find(terms[t].x);
+    if (it == where.end()) {
+      it = where.emplace(terms[t].x, all.size()).first;
+      all.push_back(Group());
+      all.back().x = terms[t].x;
+    }
+    all[it->second].terms.push_back(t);
+  }
+  std::vector<Group> units;
+  std::vector<uint32_t> diag;
+  for (const Group &g : all)
+    if (g.x == 0) {
+      diag = g.terms;
+    } else {
+      for (size_t s = 0; s < g.terms.size(); s += kExpBatchTerms) {
+        Group u;
+        u.x = g.x;
+        u.terms.assign(g.terms.begin() + s, g.terms.begin() + std::min(g.terms.size(), s + kExpBatchTerms));
+        units.push_back(u);
+      }
+    }
+  // greedy: a unit joins the sweep when the high bits where it differs from the sweep's x_out fit in the tile
+  std::vector<bool> used(units.size(), false);
+  size_t left = units.size();
+  std::vector<Sweep> &sw = *out;
+  sw.clear();
+  while (left) {
+    Sweep s;
+    bool started = false;
+    for (size_t i = 0; i < units.size(); ++i) {
+      if (used[i] || s.n_terms + units[i].terms.size() > kExpBatchTerms) continue;
+      const uint64_t hx = units[i].x & ~low;
+      if (!started) {
+        s.x_out = hx;
+        started = true;
+      } else {
+        const uint64_t h2 = s.hi | ((hx ^ s.x_out) & ~s.hi);
+        if ((uint32_t)popc64(h2) > m) continue;
+        s.hi = h2;
+        s.x_out &= ~h2;
+      }
+      used[i] = true;
+      --left;
+      s.n_terms += (uint32_t)units[i].terms.size();
+      s.groups.push_back(units[i]);
+    }
+    sw.push_back(s);
+  }
+  // diagonal terms fill the room the sweeps leave, in sweep order; only what is left opens sweeps of its own
+  for (size_t done = 0, k = 0; done < diag.size(); ++k) {
+    if (k == sw.size()) sw.push_back(Sweep());
+    const size_t take = std::min<size_t>(kExpBatchTerms - sw[k].n_terms, diag.size() - done);
+    if (take == 0) continue;
+    Group d;
+    d.terms.assign(diag.begin() + done, diag.begin() + done + take);
+    done += take;
+    sw[k].n_terms += (uint32_t)take;
+    sw[k].groups.push_back(d);
+  }
+  for (Sweep &s : sw) {
+    // free tile bits: first x_out bits (fewer tile pairs), then the lowest free bits (longer contiguous runs)
+    for (uint32_t b = 0; b < n && (uint32_t)popc64(s.hi) < m; ++b)
+      if ((s.x_out >> b) & 1) {
+        s.hi |= 1ull << b;
+        s.x_out &= ~(1ull << b);
+      }
+    for (uint32_t b = L; b < n && (uint32_t)popc64(s.hi) < m; ++b)
+      if (!((s.hi >> b) & 1)) s.hi |= 1ull << b;
+    uint32_t slots = 0;
+    for (Group &g : s.groups)
+      if (g.terms.size() <= kExpDirectGroupTerms && slots + g.terms.size() <= kExpMaxDirect) {
+        g.direct = true;
+        slots += (uint32_t)g.terms.size();
+      }
+    std::stable_partition(s.groups.begin(), s.groups.end(), [](const Group &g) { return g.direct; });
+  }
+}
+
+uint32_t compact(uint64_t v, uint32_t L, const std::vector<uint32_t> &hi_pos) {
+  uint32_t r = (uint32_t)(v & ((1ull << L) - 1));
+  for (size_t i = 0; i < hi_pos.size(); ++i) r |= (uint32_t)((v >> hi_pos[i]) & 1ull) << (L + i);
+  return r;
+}
+
+template <typename R>
+cudaError_t launch_sweep(const void *psi, const ExpArgs &a, const ExpGroupDev *g, const ExpTermDev *t, double *partials,
+                         cudaStream_t s) {
+  const size_t smem = (a.x_out ? 2 : 1) * kExpTile * sizeof(typename ExpV<R>::type) + 2 * kExpTile * sizeof(double) +
+                      (kExpThreads / 32) * kExpMaxDirect * sizeof(double) +
+                      std::min(a.n_terms, kExpSmemTerms) * sizeof(double) + kExpMaxDirect * sizeof(ExpTermDev) +
+                      std::min(a.n_groups, kExpSmemGroups) * sizeof(ExpGroupDev);
+  const size_t smem_max = 2 * kExpTile * sizeof(double2) + 2 * kExpTile * sizeof(double) +
+                          (kExpThreads / 32) * kExpMaxDirect * sizeof(double) +
+                          kExpSmemTerms * sizeof(double) + kExpMaxDirect * sizeof(ExpTermDev) +
+                          kExpSmemGroups * sizeof(ExpGroupDev);
+  static_assert(2 * kExpTile * sizeof(double2) + 2 * kExpTile * sizeof(double) +
+                        (kExpThreads / 32) * kExpMaxDirect * sizeof(double) + kExpSmemTerms * sizeof(double) +
+                        kExpMaxDirect * sizeof(ExpTermDev) + kExpSmemGroups * sizeof(ExpGroupDev) <= 113 * 1024,
+                "two CTAs per SM: at most 113 KiB of shared memory each");
+  cudaError_t e = cudaFuncSetAttribute(k_expect<R>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
+  if (e != cudaSuccess) return e;
+  k_expect<R><<<kExpGrid, kExpThreads, smem, s>>>((const R *)psi, a, g, t, partials);
+  return cudaGetLastError();
+}
+
+}  // namespace
+
+int parse_pauli_terms(uint32_t n, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms,
+                      std::vector<PauliTerm> *out, std::string *err) {
+  out->clear();
+  if (n_terms == 0) return QIPB200_OK;
+  if (!qubits || !paulis || !term_len) {
+    *err = "expect: NULL qubits, paulis or term_len";
+    return QIPB200_ERR_INVALID_ARG;
+  }
+  char msg[160];
+  out->reserve(n_terms);
+  size_t k = 0;
+  for (size_t t = 0; t < n_terms; ++t) {
+    PauliTerm p;
+    uint64_t seen = 0;
+    for (uint32_t j = 0; j < term_len[t]; ++j, ++k) {
+      const char c = paulis[k];
+      const uint64_t q = qubits[k];
+      if (c != 'X' && c != 'Y' && c != 'Z') {
+        snprintf(msg, sizeof(msg), "expect: term %zu: Pauli letter 0x%02x is not 'X', 'Y' or 'Z'", t, (unsigned)(unsigned char)c);
+        *err = msg;
+        return QIPB200_ERR_INVALID_ARG;
+      }
+      if (q >= n) {
+        snprintf(msg, sizeof(msg), "expect: term %zu: qubit %llu out of range for %u qubits", t, (unsigned long long)q, n);
+        *err = msg;
+        return QIPB200_ERR_BAD_INDEX;
+      }
+      const uint64_t bit = 1ull << (n - 1 - q);
+      if (seen & bit) {
+        snprintf(msg, sizeof(msg), "expect: term %zu: qubit %llu repeated", t, (unsigned long long)q);
+        *err = msg;
+        return QIPB200_ERR_BAD_INDEX;
+      }
+      seen |= bit;
+      if (c != 'Z') p.x |= bit;
+      if (c != 'X') p.z |= bit;
+      if (c == 'Y') ++p.n_y;
+    }
+    out->push_back(p);
+  }
+  return QIPB200_OK;
+}
+
+uint32_t expect_sweep_count(uint32_t n, const std::vector<PauliTerm> &terms) {
+  std::vector<Sweep> sw;
+  plan_sweeps(n, terms, &sw);
+  return (uint32_t)sw.size();
+}
+
+cudaError_t run_expect(qip_prec prec, const void *psi, uint32_t n, const std::vector<PauliTerm> &terms, double *out,
+                       cudaStream_t s, uint64_t *launches) {
+  if (terms.empty()) return cudaSuccess;
+  std::vector<Sweep> sw;
+  plan_sweeps(n, terms, &sw);
+  const uint32_t L = std::min(kExpL, n);
+  const uint64_t low = (1ull << L) - 1;
+  // host tables of every sweep, rows in sweep order; batches of whole sweeps of at most kExpBatchTerms rows
+  std::vector<ExpArgs> args(sw.size());
+  std::vector<ExpGroupDev> hg;
+  std::vector<ExpTermDev> ht;
+  std::vector<uint32_t> orig;
+  std::vector<size_t> g_off(sw.size()), t_off(sw.size());
+  for (size_t k = 0; k < sw.size(); ++k) {
+    const Sweep &S = sw[k];
+    ExpArgs &a = args[k];
+    memset(&a, 0, sizeof(a));
+    std::vector<uint32_t> hi_pos;
+    for (uint32_t b = 0; b < n; ++b)
+      if ((S.hi >> b) & 1) hi_pos.push_back(b);
+    const uint64_t tile = low | S.hi;
+    a.x_out = S.x_out;
+    a.L = L;
+    a.tb = L + (uint32_t)hi_pos.size();
+    for (size_t i = 0; i < hi_pos.size(); ++i) a.hi_pos[i] = (uint8_t)hi_pos[i];
+    const int pair_bit = S.x_out ? __builtin_ctzll(S.x_out) : -1;
+    for (uint32_t b = 0; b < n; ++b)
+      if (!((tile >> b) & 1) && (int)b != pair_bit) a.out_pos[a.n_out++] = (uint8_t)b;
+    a.n_visits = 1ull << a.n_out;
+    a.n_groups = (uint32_t)S.groups.size();
+    a.n_terms = S.n_terms;
+    g_off[k] = hg.size();
+    t_off[k] = ht.size();
+    uint32_t first = 0;
+    for (const Group &G : S.groups) {
+      ExpGroupDev gd;
+      gd.x_in = compact(G.x & tile, L, hi_pos);
+      gd.diag = G.x == 0;
+      gd.first = first;
+      gd.end = first + (uint32_t)G.terms.size();
+      gd.dfirst = gd.dend = 0;
+      if (G.direct) {
+        gd.dfirst = a.n_direct;
+        gd.dend = a.n_direct + (uint32_t)G.terms.size();
+      }
+      for (uint32_t j = 0; j < G.terms.size(); ++j) {
+        const PauliTerm &P = terms[G.terms[j]];
+        ExpTermDev td;
+        td.z_out = P.z & ~tile;
+        td.z_in = compact(P.z & tile, L, hi_pos);
+        const uint32_t ph = P.n_y & 3;  // Re(i^ph w): +Re, -Im, -Re, +Im
+        td.comp = ph & 1;
+        td.coef = (ph == 0 || ph == 3) ? 1.0 : -1.0;
+        if (S.x_out && !gd.diag) {  // + the partner tile: w + eta conj(w)
+          const double eta = (popc64(P.x & P.z) & 1) ? -1.0 : 1.0;
+          td.coef *= td.comp ? 1.0 - eta : 1.0 + eta;
+        }
+        if (G.direct) {
+          a.direct[a.n_direct] = td;
+          a.direct_term[a.n_direct++] = (uint16_t)(first + j);
+        }
+        ht.push_back(td);
+        orig.push_back(G.terms[j]);
+      }
+      first = gd.end;
+      hg.push_back(gd);
+    }
+  }
+  std::vector<std::pair<size_t, size_t>> batches;  // [first sweep, end sweep)
+  size_t rows_cap = 0, groups_cap = 0;
+  for (size_t k = 0; k < sw.size();) {
+    size_t e = k, rows = 0;
+    while (e < sw.size() && rows + sw[e].n_terms <= kExpBatchTerms) rows += sw[e++].n_terms;
+    batches.push_back(std::make_pair(k, e));
+    rows_cap = std::max(rows_cap, rows);
+    groups_cap = std::max(groups_cap, (e < sw.size() ? g_off[e] : hg.size()) - g_off[k]);
+    k = e;
+  }
+  const size_t part_bytes = rows_cap * kExpGrid * sizeof(double);
+  const size_t res_bytes = rows_cap * sizeof(double);
+  const size_t term_bytes = rows_cap * sizeof(ExpTermDev);
+  const size_t bytes = part_bytes + res_bytes + term_bytes + groups_cap * sizeof(ExpGroupDev);
+  char *d = nullptr;
+  cudaError_t e = cudaMallocAsync((void **)&d, bytes, s);
+  if (e != cudaSuccess) return e;
+  double *d_part = (double *)d;
+  double *d_res = (double *)(d + part_bytes);
+  ExpTermDev *d_terms = (ExpTermDev *)(d + part_bytes + res_bytes);
+  ExpGroupDev *d_groups = (ExpGroupDev *)(d + part_bytes + res_bytes + term_bytes);
+  std::vector<double> res(ht.size());
+  for (size_t b = 0; b < batches.size() && e == cudaSuccess; ++b) {
+    const size_t k0 = batches[b].first, k1 = batches[b].second;
+    const size_t t_end = k1 < sw.size() ? t_off[k1] : ht.size();
+    const size_t g_end = k1 < sw.size() ? g_off[k1] : hg.size();
+    const uint32_t rows = (uint32_t)(t_end - t_off[k0]);
+    e = cudaMemcpyAsync(d_terms, ht.data() + t_off[k0], rows * sizeof(ExpTermDev), cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess)
+      e = cudaMemcpyAsync(d_groups, hg.data() + g_off[k0], (g_end - g_off[k0]) * sizeof(ExpGroupDev),
+                          cudaMemcpyHostToDevice, s);
+    for (size_t k = k0; k < k1 && e == cudaSuccess; ++k) {
+      ExpArgs a = args[k];
+      a.row_off = (uint32_t)(t_off[k] - t_off[k0]);
+      a.rows = rows;
+      const ExpGroupDev *g = d_groups + (g_off[k] - g_off[k0]);
+      const ExpTermDev *t = d_terms + a.row_off;
+      e = prec == QIP_F32 ? launch_sweep<float>(psi, a, g, t, d_part, s) : launch_sweep<double>(psi, a, g, t, d_part, s);
+      ++*launches;
+    }
+    if (e == cudaSuccess) {
+      k_expect_reduce<<<(rows + 255) / 256, 256, 0, s>>>(d_part, rows, kExpGrid, d_res);
+      ++*launches;
+      e = cudaGetLastError();
+    }
+    if (e == cudaSuccess)
+      e = cudaMemcpyAsync(res.data() + t_off[k0], d_res, rows * sizeof(double), cudaMemcpyDeviceToHost, s);
+  }
+  const cudaError_t ef = cudaFreeAsync(d, s);
+  if (e == cudaSuccess) e = ef;
+  const cudaError_t es = cudaStreamSynchronize(s);
+  if (e == cudaSuccess) e = es;
+  if (e != cudaSuccess) return e;
+  for (size_t r = 0; r < res.size(); ++r) out[orig[r]] = res[r];
+  return cudaSuccess;
+}
+
+}  // namespace qipb200

@@ -279,6 +279,17 @@ class State:
                                                    C.byref(p)))
         return int(m.value), float(p.value)
 
+    def expect_paulis(self, terms) -> np.ndarray:
+        """<psi|P_t|psi> for each Pauli string P_t on the state as it is (not renormalised), computed on the device.
+
+        A term is a sequence of (letter, qubit) pairs with letters "X", "Y", "Z", e.g. ``[("Z", 0), ("Z", 1)]``; an
+        empty term is the identity.  A read sweep of the state carries up to 16384 terms: terms with equal X/Y masks
+        share one, Z-only terms ride along (``expect_plan`` gives the count).  For H = sum_t c_t P_t take ``np.dot(c, st.expect_paulis(P))``."""
+        qs, ls, lens = _marshal_paulis(terms)
+        out = np.zeros(max(1, lens.shape[0]), dtype=np.float64)
+        self._chk(_lib.lib().qipb200_state_expect_paulis(self._h, _ptr(qs), ls, _ptr(lens), lens.shape[0], _ptr(out)))
+        return out[: lens.shape[0]]
+
     # -- multi-GPU --------------------------------------------------------------
     def ipc_export(self):
         a = (C.c_ubyte * _lib.IPC_HANDLE_BYTES)()
@@ -308,6 +319,32 @@ def validate_op(op: MatrixOp, n: int, dtype=np.complex128):
     prec = prec_of(dtype)
     cop, keep = marshal_op(op, prec)
     _lib.check(_lib.lib().qipb200_validate_op(None, prec, int(n), C.byref(cop)), None)
+
+
+def _marshal_paulis(terms):
+    """Flat (qubits u64, letters bytes, term lengths u32) arrays of the C ABI from [[(letter, qubit), ...], ...]."""
+    qs, ls, lens = [], [], []
+    for t in terms:
+        t = list(t)
+        lens.append(len(t))
+        for letter, q in t:
+            b = letter.encode("ascii") if isinstance(letter, str) else bytes(letter)
+            if len(b) != 1:
+                raise ValueError("Pauli letter must be one character, got %r" % (letter,))
+            ls.append(b)
+            qs.append(int(q))
+    qa = np.ascontiguousarray(np.asarray(qs if qs else [0], dtype=np.uint64))
+    la = C.create_string_buffer(b"".join(ls) or b"\0", max(1, len(ls)))
+    return qa, la, np.ascontiguousarray(np.asarray(lens if lens else [0], dtype=np.uint32))[: len(lens)]
+
+
+def expect_plan(n: int, dtype, terms) -> int:
+    """Read sweeps State.expect_paulis makes for these terms on an unsharded n-qubit state (needs no GPU)."""
+    qs, ls, lens = _marshal_paulis(terms)
+    v = C.c_uint32()
+    _lib.check(_lib.lib().qipb200_expect_plan(prec_of(dtype), int(n), _ptr(qs), ls, _ptr(lens), lens.shape[0],
+                                             C.byref(v)), None)
+    return int(v.value)
 
 
 def plan_exchanges(ops: Sequence[MatrixOp], n: int, world_size: int, dtype=np.complex128):
