@@ -1772,6 +1772,10 @@ static int plan_rotating_scaled(const qip_op *ops, size_t n_ops, qip_prec prec, 
       ps.op_index = out->singles.size() - 1;
       out->steps.push_back(ps);
       remaining.erase(remaining.begin() + best.single);
+      // no pass is pending any more: the next tile carries over only the qubits that now sit in the low positions
+      // (not the whole tile of the flushed pass, whose high qubits no later swap brings down)
+      prev = 0;
+      for (uint32_t p = 0; p < L; ++p) prev |= 1ull << logical_at(p);
       continue;
     }
     // the tile of this pass: the selected qubits, padded to T (first from the previous tile: they cost nothing)

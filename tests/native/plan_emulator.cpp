@@ -2,6 +2,7 @@
 // exactly as the tile kernel would (same serialised blob, same micro-op semantics), so the
 // host logic (planner.cpp, opcompile.cpp, serialisation) is validated without a GPU.
 // Built by tests/test_planner_cpu.py into tests/native/_build/; never part of libqipb200.
+#include <algorithm>
 #include <complex>
 #include <cstdio>
 #include <cstdlib>
@@ -704,6 +705,91 @@ extern "C" int emul_jit_plan_stats(int prec, uint32_t n, const qip_op *ops, size
     stats[4] += prog.n_cta_barriers;
     stats[5] += prog.n_warp_syncs;
     stats[6] += prog.n_renamed;
+  }
+  return 0;
+}
+
+// Coverage histogram of a plan (no amplitudes): which shapes the planner and the generator emitted for a circuit, so a
+// test can assert that a circuit family reaches every one of them.
+// hist: [0..39] interpreter case ids (EC_*) of the serialised records; [40..44] JElem kinds of the generated-kernel view
+//       (D1, X, PH, DK, HAD); [45] JElem phases with a thread predicate (pm != 0); [46] JElem phases with thread-term
+//       factors; [47] JElem phases with CTA-uniform factor terms; [48] JElems under a CTA-uniform condition;
+//       [49] / [50] conditional exchanges folded into a load / store address of the generated source;
+//       [51] records on the condition-table overflow path; [52] passes; [53] passes the generator declined;
+//       [54] single steps; [55] CTA-uniform store-time phase terms; [56] MK_DENSE, [57] MK_DIAG, [58] MK_EXCH micro-ops;
+//       [59] most distinct CTA-uniform conditions of the generated-kernel view in one pass; [60] fewest tiles of a pass
+//       (2^(n-T)); [61] passes the generator declined although they hold register-group work and every op fits a group;
+//       [62] passes holding an op wider than a register group; [63] passes with no register-group work at all (only
+//       CTA-uniform store-time phases) -- [62] and [63] run the interpreter kernel by design
+static uint64_t count_substr(const std::string &s, const char *what) {
+  uint64_t n = 0;
+  for (size_t at = s.find(what); at != std::string::npos; at = s.find(what, at + 1)) ++n;
+  return n;
+}
+
+extern "C" int emul_plan_coverage(int prec, uint32_t n, const qip_op *ops, size_t n_ops, uint32_t T, uint32_t L, uint64_t *hist) {
+  std::vector<FlatOp> flat(n_ops);
+  for (size_t i = 0; i < n_ops; ++i) {
+    std::string err;
+    if (compile_op(&ops[i], (qip_prec)prec, n, &flat[i], &err) != QIPB200_OK) return -1;
+  }
+  PlanConfig cfg = default_plan_config((qip_prec)prec, n);
+  if (T) cfg.T = T;
+  if (L) cfg.L = L;
+  std::vector<PlanStep> steps;
+  plan_passes(flat, n, (qip_prec)prec, cfg, &steps);
+  for (int i = 0; i < 64; ++i) hist[i] = 0;
+  const size_t gsz = prec == QIP_F32 ? sizeof(GlobalTerm<float>) : sizeof(GlobalTerm<double>);
+  for (size_t s = 0; s < steps.size(); ++s) {
+    if (!steps[s].is_pass) {
+      ++hist[54];
+      continue;
+    }
+    const HostPass &p = steps[s].pass;
+    ++hist[52];
+    hist[55] += p.gterms.size() / gsz;
+    const uint64_t tiles = 1ull << (n - p.hdr.T);
+    if (hist[60] == 0 || tiles < hist[60]) hist[60] = tiles;
+    if (p.jbits == 0) ++hist[62];
+    if (p.jbits != 0 && p.jgroups.empty()) ++hist[63];
+    std::vector<std::pair<uint64_t, uint64_t>> conds;
+    for (size_t i = 0; i < p.ops.size(); ++i) {
+      const MicroOp &mo = p.ops[i].h;
+      if (mo.kind == MK_DENSE) ++hist[56];
+      if (mo.kind == MK_DIAG) ++hist[57];
+      if (mo.kind == MK_EXCH) ++hist[58];
+      if (mo.kind != MK_SUPER) continue;
+      const unsigned char *ep = p.ops[i].data.data();
+      for (;;) {
+        uint32_t op;
+        memcpy(&op, ep, 4);
+        if (elem_case(op) == EC_END) break;
+        ++hist[elem_case(op)];
+        if ((op & kElemHasCond) && elem_cond_slot(op) == kCondOverflow) ++hist[51];
+        ep += elem_size_bytes(op);
+      }
+    }
+    for (size_t g = 0; g < p.jgroups.size(); ++g)
+      for (size_t e = 0; e < p.jgroups[g].elems.size(); ++e) {
+        const JElem &d = p.jgroups[g].elems[e];
+        ++hist[40 + d.kind];
+        if (d.kind == JElem::PH && d.pm) ++hist[45];
+        if (d.kind == JElem::PH && !d.tterms.empty()) ++hist[46];
+        if (d.kind == JElem::PH && !d.terms.empty()) ++hist[47];
+        if (d.gmask) ++hist[48];
+        if (d.gmask && std::find(conds.begin(), conds.end(), std::make_pair(d.gmask, d.gval)) == conds.end())
+          conds.push_back(std::make_pair(d.gmask, d.gval));
+      }
+    if (conds.size() > hist[59]) hist[59] = conds.size();
+    JitProgram prog;
+    std::string why;
+    if (!jit_generate(p, (qip_prec)prec, &prog, &why)) {
+      ++hist[53];
+      if (p.jbits != 0 && !p.jgroups.empty()) ++hist[61];
+      continue;
+    }
+    hist[49] += count_substr(prog.source, "const unsigned la");
+    hist[50] += count_substr(prog.source, "const unsigned sa");
   }
   return 0;
 }
