@@ -278,6 +278,19 @@ int qipb200_state_expect_paulis(qipb200_state *state, const uint64_t *qubits, co
  * terms on an unsharded n-qubit state in canonical layout (0 for n_terms == 0).  Validates as the call above does. */
 int qipb200_expect_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms, uint32_t *sweeps);
 
+/* Reduced density matrix of the k = n_qubits_kept qubits `qubits` on the state AS IT IS (not renormalised, like
+ * measure_probs); absent in the reference.  out (HOST, 2 * 4^k doubles, interleaved re/im) receives
+ *   rho[a * 2^k + b] = sum_r psi(r, a) conj(psi(r, b))      (partial trace over every other qubit)
+ * where bit i of a and b is the value of qubit qubits[i] (the convention of measure_probs: diag(rho) equals
+ * measure_probs(qubits) up to rounding, and the trace is norm2).  The lower triangle is the conjugate of the upper one
+ * and the diagonal's imaginary part is exactly 0.0.  Double for f32 and f64 states (f32 amplitudes are widened before
+ * they are multiplied), deterministic (same state and qubits -> bit-identical out), synchronises.  NULL qubits, k == 0
+ * or k > n give QIPB200_ERR_INVALID_ARG, a qubit >= n or repeated QIPB200_ERR_BAD_INDEX, NULL out
+ * QIPB200_ERR_INVALID_ARG, k > 10 QIPB200_ERR_UNSUPPORTED.  One read sweep for k <= 6 (2 kernels); for k = 7..10,
+ * nB = 2^(k-6) sweeps in nB (nB + 1) kernels.  A pending collapse is applied first; a permuted layout is read as it is.
+ * Sharded and multi-device states: QIPB200_ERR_UNSUPPORTED. */
+int qipb200_state_reduced_density(qipb200_state *state, const uint64_t *qubits, uint32_t n_qubits_kept, double *out);
+
 /* ---- multi-GPU: the 2^n state sharded by its top log2(world) index bits,
  *      one process per GPU (absent in the reference; its only hook is the
  *      input_offset/output_offset slice model, matrix_ops.rs:74-89) -------------- */

@@ -273,6 +273,15 @@ class B200State {
                                            out.data()));
     return out;
   }
+  // reduced density matrix of up to 10 qubits, row-major 2^k x 2^k; bit i of the row and column index is the value of
+  // qubits[i], as in measure_probs (absent in the reference)
+  std::vector<std::complex<double>> reduced_density(const std::vector<uint64_t> &qubits) {
+    const size_t dim = qubits.size() <= 10 ? (size_t)1 << qubits.size() : 1;
+    std::vector<std::complex<double>> out(dim * dim);
+    ctx_.check(qipb200_state_reduced_density(st_, qubits.data(), (uint32_t)qubits.size(),
+                                             reinterpret_cast<double *>(out.data())));
+    return out;
+  }
   // a schedule parsed from the QIPS wire format (owned by the library): builder.rs:423-514 on foreign circuits
   void apply_parsed(const qip_op *ops, size_t n_ops, bool fusion = true) {
     ctx_.check(qipb200_state_apply_schedule(st_, ops, n_ops, fusion ? QIPB200_SCHED_DEFAULT : QIPB200_SCHED_NO_FUSION));

@@ -22,6 +22,7 @@
 #include "expect.h"
 #include "kernels.cuh"
 #include "opcompile.h"
+#include "rdm.h"
 #include "schedule.h"
 #include "tile.cuh"
 #include "jit_codegen.h"
@@ -1936,6 +1937,42 @@ extern "C" int qipb200_expect_plan(qip_prec prec, uint32_t n_qubits, const uint6
     if (st != QIPB200_OK) return set_err(nullptr, st, err);
     *sweeps = expect_sweep_count(n_qubits, terms);
     return (int)QIPB200_OK;
+  });
+}
+
+// ===================================================================================
+// reduced density matrices (rdm.cu)
+// ===================================================================================
+
+namespace {
+
+int rdm_impl(qipb200_state *s, const uint64_t *qubits, uint32_t k, double *out) {
+  qipb200_ctx *ctx = s->ctx;
+  CU(ctx, cudaSetDevice(ctx->device));
+  int st = materialise_collapse(s);
+  if (st != QIPB200_OK) return st;
+  // A state left permuted (QIPB200_ROTATE) needs no restore_layout sweep: the kept qubits are read where they are.
+  uint32_t pos[kRdmMaxKept];
+  for (uint32_t i = 0; i < k; ++i) pos[i] = s->phys_of_logical[s->n - 1 - (uint32_t)qubits[i]];
+  CU(ctx, run_reduced_density(s->prec, s->buf, s->n_local, pos, k, out, ctx->stream, &ctx->launches));
+  return QIPB200_OK;
+}
+
+}  // namespace
+
+extern "C" int qipb200_state_reduced_density(qipb200_state *s, const uint64_t *qubits, uint32_t n_qubits_kept,
+                                             double *out) {
+  if (!s) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, "reduced_density: NULL state");
+  return guarded(s->ctx, [&]() -> int {
+    int st = check_indices(s, qubits, n_qubits_kept);
+    if (st != QIPB200_OK) return st;
+    if (!out) return set_err(s->ctx, QIPB200_ERR_INVALID_ARG, "reduced_density: NULL out");
+    if (n_qubits_kept > kRdmMaxKept)
+      return set_err(s->ctx, QIPB200_ERR_UNSUPPORTED,
+                     "reduced_density: at most 10 kept qubits (the output at 10 is already 16 MiB)");
+    if (s->world > 1 || !s->shards.empty())
+      return set_err(s->ctx, QIPB200_ERR_UNSUPPORTED, "reduced_density: sharded states are not supported");
+    return rdm_impl(s, qubits, n_qubits_kept, out);
   });
 }
 

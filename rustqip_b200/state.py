@@ -290,6 +290,19 @@ class State:
         self._chk(_lib.lib().qipb200_state_expect_paulis(self._h, _ptr(qs), ls, _ptr(lens), lens.shape[0], _ptr(out)))
         return out[: lens.shape[0]]
 
+    def reduced_density(self, qubits: Sequence[int]) -> np.ndarray:
+        """Reduced density matrix of ``qubits`` (1 to 10 of them) on the state as it is (not renormalised), computed
+        on the device: complex128 of shape (2^k, 2^k) with rho[a, b] = sum_r psi(r, a) conj(psi(r, b)).
+
+        Bit i of the row and column indices a, b is the value of qubit ``qubits[i]`` (the convention of
+        ``measure_probs``, so ``diag(rho)`` is ``measure_probs(qubits)`` up to rounding).  rho is exactly Hermitian
+        and deterministic.  One read sweep of the state for k <= 6, 2^(k-6) sweeps above."""
+        idx = np.ascontiguousarray(np.asarray(list(qubits), dtype=np.uint64))
+        k = len(idx)
+        out = np.zeros((1 << min(k, 10)) ** 2 if k else 1, dtype=np.complex128)
+        self._chk(_lib.lib().qipb200_state_reduced_density(self._h, _ptr(idx) if k else None, k, _ptr(out)))
+        return out.reshape(1 << k, 1 << k)
+
     # -- multi-GPU --------------------------------------------------------------
     def ipc_export(self):
         a = (C.c_ubyte * _lib.IPC_HANDLE_BYTES)()
