@@ -291,6 +291,26 @@ int qipb200_expect_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits
  * Sharded and multi-device states: QIPB200_ERR_UNSUPPORTED. */
 int qipb200_state_reduced_density(qipb200_state *state, const uint64_t *qubits, uint32_t n_qubits_kept, double *out);
 
+/* psi <- exp(-i angles[T-1]/2 P_{T-1}) ... exp(-i angles[0]/2 P_0) psi: Pauli-string rotations, term 0 first; absent in
+ * the reference.  Terms are encoded and validated as for qipb200_state_expect_paulis (same codes and messages), with
+ * P = i^nY X^x Z^z, so a single 'Z' term is rz(q, angle) and a single 'X' term is Rx(angle); an empty term is the
+ * global phase e^{-i angle/2}.  NULL angles with n_terms > 0, or a non-finite angle, give QIPB200_ERR_INVALID_ARG.
+ * Every term and angle is checked before any device work: a refused call leaves the amplitudes (and a pending
+ * collapse) as they were.  n_terms == 0 is a no-op.  Arithmetic (fixed, so that it can be emulated bit for bit): per
+ * term c = cos(angle/2) and s = sin(angle/2) are computed in double on the host and rounded once to the state's
+ * precision; each pair (j, j ^ x) is updated from its old values as
+ *   psi'_j = (RN(RN(c re psi_j) + RN(s re w_j)), RN(RN(c im psi_j) + RN(s im w_j))),   w_j = -i (P psi)_j (exact)
+ * in the state's precision, without FMA, so the result depends neither on how terms share sweeps nor on the layout.
+ * Stream-ordered like apply_schedule (does not synchronise; the host arrays are copied before it returns).  One kernel
+ * per read-write sweep of the state; a sweep carries a run of consecutive terms whose X/Y letters fit one tile (plus
+ * one shared out-of-tile mask); qipb200_pauli_rotation_plan reports the count.  A pending collapse is applied first
+ * (one more kernel); a permuted layout is rotated in place and stays as it is.  Sharded and multi-device states:
+ * QIPB200_ERR_UNSUPPORTED. */
+int qipb200_state_apply_pauli_rotations(qipb200_state *state, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms, const double *angles);
+/* Host-only (no GPU, ctx-free): the number of read-write sweeps the call above makes for these terms on an unsharded
+ * n-qubit state in canonical layout (0 for n_terms == 0).  Validates the terms as the call above does. */
+int qipb200_pauli_rotation_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms, uint32_t *sweeps);
+
 /* ---- multi-GPU: the 2^n state sharded by its top log2(world) index bits,
  *      one process per GPU (absent in the reference; its only hook is the
  *      input_offset/output_offset slice model, matrix_ops.rs:74-89) -------------- */

@@ -273,6 +273,30 @@ class B200State {
                                            out.data()));
     return out;
   }
+  // psi <- exp(-i angles[T-1]/2 P_{T-1}) ... exp(-i angles[0]/2 P_0) psi for Pauli strings encoded as in
+  // expect_paulis, term 0 first (absent in the reference)
+  void apply_pauli_rotations(const std::vector<std::vector<std::pair<char, uint64_t>>> &terms,
+                             const std::vector<double> &angles) {
+    if (angles.size() != terms.size())
+      throw CircuitError("apply_pauli_rotations: " + std::to_string(terms.size()) + " terms but " +
+                         std::to_string(angles.size()) + " angles");
+    std::vector<uint64_t> qubits;
+    std::vector<char> letters;
+    std::vector<uint32_t> lens;
+    for (const auto &t : terms) {
+      lens.push_back((uint32_t)t.size());
+      for (const auto &lq : t) {
+        letters.push_back(lq.first);
+        qubits.push_back(lq.second);
+      }
+    }
+    // a list of identities has no letters: pass non-NULL (unread) arrays, the C entry refuses NULL ones
+    const uint64_t no_qubit = 0;
+    const char no_letter = 'Z';
+    ctx_.check(qipb200_state_apply_pauli_rotations(st_, qubits.empty() ? &no_qubit : qubits.data(),
+                                                   letters.empty() ? &no_letter : letters.data(), lens.data(),
+                                                   terms.size(), angles.data()));
+  }
   // reduced density matrix of up to 10 qubits, row-major 2^k x 2^k; bit i of the row and column index is the value of
   // qubits[i], as in measure_probs (absent in the reference)
   std::vector<std::complex<double>> reduced_density(const std::vector<uint64_t> &qubits) {

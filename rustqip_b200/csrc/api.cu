@@ -22,6 +22,7 @@
 #include "expect.h"
 #include "kernels.cuh"
 #include "opcompile.h"
+#include "pauli_rot.h"
 #include "rdm.h"
 #include "schedule.h"
 #include "tile.cuh"
@@ -1973,6 +1974,71 @@ extern "C" int qipb200_state_reduced_density(qipb200_state *s, const uint64_t *q
     if (s->world > 1 || !s->shards.empty())
       return set_err(s->ctx, QIPB200_ERR_UNSUPPORTED, "reduced_density: sharded states are not supported");
     return rdm_impl(s, qubits, n_qubits_kept, out);
+  });
+}
+
+// ===================================================================================
+// Pauli-string rotations (pauli_rot.cu)
+// ===================================================================================
+
+namespace {
+
+int pauli_rot_impl(qipb200_state *s, const std::vector<PauliTerm> &terms, const double *angles) {
+  qipb200_ctx *ctx = s->ctx;
+  CU(ctx, cudaSetDevice(ctx->device));
+  int st = materialise_collapse(s);
+  if (st != QIPB200_OK) return st;
+  // A state left permuted (QIPB200_ROTATE) is rotated where it is: Pauli masks permute with the bits.
+  std::vector<PauliTerm> phys(terms.size());
+  for (size_t t = 0; t < terms.size(); ++t) {
+    phys[t].n_y = terms[t].n_y;
+    for (uint32_t b = 0; b < s->n; ++b) {
+      const uint64_t p = 1ull << s->phys_of_logical[b];
+      if ((terms[t].x >> b) & 1) phys[t].x |= p;
+      if ((terms[t].z >> b) & 1) phys[t].z |= p;
+    }
+  }
+  CU(ctx, run_pauli_rotations(s->prec, s->buf, s->n_local, phys, angles, 2 * ctx->sm_count, ctx->stream,
+                              &ctx->launches));
+  return QIPB200_OK;
+}
+
+}  // namespace
+
+extern "C" int qipb200_state_apply_pauli_rotations(qipb200_state *s, const uint64_t *qubits, const char *paulis,
+                                                   const uint32_t *term_len, size_t n_terms, const double *angles) {
+  if (!s) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, "apply_pauli_rotations: NULL state");
+  return guarded(s->ctx, [&]() -> int {
+    // every term and angle is checked before any device work: a refused call leaves the state as it was
+    std::vector<PauliTerm> terms;
+    std::string err;
+    int st = parse_pauli_terms(s->n, qubits, paulis, term_len, n_terms, &terms, &err);
+    if (st != QIPB200_OK) return set_err(s->ctx, st, err);
+    if (n_terms && !angles) return set_err(s->ctx, QIPB200_ERR_INVALID_ARG, "apply_pauli_rotations: NULL angles");
+    for (size_t t = 0; t < n_terms; ++t)
+      if (!std::isfinite(angles[t]))
+        return set_err(s->ctx, QIPB200_ERR_INVALID_ARG,
+                       "apply_pauli_rotations: angle " + std::to_string(t) + " is not finite");
+    if (s->world > 1 || !s->shards.empty())
+      return set_err(s->ctx, QIPB200_ERR_UNSUPPORTED, "apply_pauli_rotations: sharded states are not supported");
+    if (n_terms == 0) return (int)QIPB200_OK;
+    return pauli_rot_impl(s, terms, angles);
+  });
+}
+
+extern "C" int qipb200_pauli_rotation_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits,
+                                           const char *paulis, const uint32_t *term_len, size_t n_terms,
+                                           uint32_t *sweeps) {
+  if (!sweeps || (prec != QIP_F32 && prec != QIP_F64) || n_qubits == 0 || n_qubits > 40)
+    return set_err(nullptr, QIPB200_ERR_INVALID_ARG,
+                   "pauli_rotation_plan: NULL sweeps, bad precision or n_qubits not in 1..40");
+  return guarded(nullptr, [&]() -> int {
+    std::vector<PauliTerm> terms;
+    std::string err;
+    int st = parse_pauli_terms(n_qubits, qubits, paulis, term_len, n_terms, &terms, &err);
+    if (st != QIPB200_OK) return set_err(nullptr, st, err);
+    *sweeps = pauli_rotation_sweep_count(n_qubits, terms);
+    return (int)QIPB200_OK;
   });
 }
 

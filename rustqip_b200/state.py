@@ -290,6 +290,21 @@ class State:
         self._chk(_lib.lib().qipb200_state_expect_paulis(self._h, _ptr(qs), ls, _ptr(lens), lens.shape[0], _ptr(out)))
         return out[: lens.shape[0]]
 
+    def apply_pauli_rotations(self, terms, angles):
+        """Apply exp(-i angles[t]/2 P_t) for each Pauli string P_t, term 0 first, on the device.
+
+        Terms are encoded as for ``expect_paulis``; a single ``[("Z", q)]`` term is ``gates.rz(q, angle)`` and a
+        single ``[("X", q)]`` term is Rx(angle).  A read-write sweep of the state carries a run of consecutive terms
+        whose X/Y letters fit one tile (``pauli_rotation_plan`` gives the count).  Stream-ordered like
+        ``apply_schedule``; the result is the same bits however the terms are split over calls."""
+        a = np.ascontiguousarray(np.asarray(angles, dtype=np.float64).reshape(-1))
+        terms = list(terms)
+        if a.shape[0] != len(terms):
+            raise ValueError("apply_pauli_rotations: %d terms but %d angles" % (len(terms), a.shape[0]))
+        qs, ls, lens = _marshal_paulis(terms)
+        self._chk(_lib.lib().qipb200_state_apply_pauli_rotations(self._h, _ptr(qs), ls, _ptr(lens), lens.shape[0],
+                                                                 _ptr(a) if a.shape[0] else None))
+
     def reduced_density(self, qubits: Sequence[int]) -> np.ndarray:
         """Reduced density matrix of ``qubits`` (1 to 10 of them) on the state as it is (not renormalised), computed
         on the device: complex128 of shape (2^k, 2^k) with rho[a, b] = sum_r psi(r, a) conj(psi(r, b)).
@@ -357,6 +372,16 @@ def expect_plan(n: int, dtype, terms) -> int:
     v = C.c_uint32()
     _lib.check(_lib.lib().qipb200_expect_plan(prec_of(dtype), int(n), _ptr(qs), ls, _ptr(lens), lens.shape[0],
                                              C.byref(v)), None)
+    return int(v.value)
+
+
+def pauli_rotation_plan(n: int, dtype, terms) -> int:
+    """Read-write sweeps State.apply_pauli_rotations makes for these terms on an unsharded n-qubit state (needs no
+    GPU)."""
+    qs, ls, lens = _marshal_paulis(terms)
+    v = C.c_uint32()
+    _lib.check(_lib.lib().qipb200_pauli_rotation_plan(prec_of(dtype), int(n), _ptr(qs), ls, _ptr(lens), lens.shape[0],
+                                                      C.byref(v)), None)
     return int(v.value)
 
 
