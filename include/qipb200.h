@@ -311,6 +311,46 @@ int qipb200_state_apply_pauli_rotations(qipb200_state *state, const uint64_t *qu
  * n-qubit state in canonical layout (0 for n_terms == 0).  Validates the terms as the call above does. */
 int qipb200_pauli_rotation_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms, uint32_t *sweeps);
 
+/* dst <- sum_h coeffs[h] P_h src, out of place: H|psi> for a Hamiltonian given as a real Pauli sum (absent in the
+ * reference).  Terms are encoded and validated as for qipb200_state_expect_paulis (same codes and messages); an empty
+ * term is coeffs[h] times the identity.  NULL coeffs with n_terms > 0, a non-finite coefficient or dst == src give
+ * QIPB200_ERR_INVALID_ARG; states of different contexts, precisions or sizes QIPB200_ERR_SIZE_MISMATCH; sharded and
+ * multi-device states QIPB200_ERR_UNSUPPORTED.  Every check runs before any device work: a refused call leaves both
+ * states (and a pending collapse) as they were.  n_terms == 0 sets dst to zero.  A collapse pending on src is applied
+ * first, one pending on dst is dropped (dst is overwritten), and dst takes src's layout.  Arithmetic: per amplitude the
+ * terms of one X/Y mask sum their signed coefficients in double, the products with the partner amplitude (widened to
+ * double) are added in a fixed order, and each read-write sweep stores the sum rounded to the state's precision; the
+ * order and the forward error bound are documented in rustqip_b200/csrc/gradient.cu.  The terms are grouped into
+ * sweeps on physical index bits, so a permuted layout may round differently; the same inputs in the same layout give
+ * the same bits.
+ * Stream-ordered (does not synchronise).  One kernel per sweep; qipb200_pauli_sum_plan reports the count. */
+int qipb200_state_apply_pauli_sum(qipb200_state *dst, const qipb200_state *src, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms, const double *coeffs);
+/* Host-only (no GPU, ctx-free): the number of sweeps qipb200_state_apply_pauli_sum makes for these terms on an
+ * unsharded n-qubit state in canonical layout (0 for n_terms == 0).  Validates the terms as the call does. */
+int qipb200_pauli_sum_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms, uint32_t *sweeps);
+
+/* Energy and gradient of a Pauli-rotation circuit by the adjoint method (absent in the reference).  With
+ * U = R_{T-1} ... R_0, R_t = exp(-i angles[t]/2 P_t) (the convention of qipb200_state_apply_pauli_rotations) and
+ * H = sum_h coeffs[h] Q_h, on entry `state` holds psi0 and the call
+ *   1. state <- U state, exactly qipb200_state_apply_pauli_rotations;
+ *   2. work <- H state, exactly qipb200_state_apply_pauli_sum;
+ *   3. for t = T-1 down to 0: grad[t] = Im <work|P_t|state>, then state <- R_t^dagger state, work <- R_t^dagger work;
+ *      *energy = Re <work|state> before the first undo.
+ * In exact arithmetic grad[t] = dE/dangles[t] for E = <psi0|U^dagger H U|psi0>.  A parameter shared by several terms
+ * (one QAOA angle on many strings) has the sum of their entries as its derivative.  The undo uses the rotation update
+ * with the same host-rounded c and the negated s, so `state` ends bit-identical to that arithmetic run forward and then
+ * backward: psi0 only up to rounding (re-prepare it when it is needed exactly); `work` ends holding U^dagger H U psi0.
+ * Inner products are accumulated in double in a fixed order: the same inputs give the same bits.  Validation as above
+ * for both term lists; NULL or non-finite angles or coeffs (when their list is not empty), NULL energy, NULL grad with
+ * n_terms > 0 or state == work give QIPB200_ERR_INVALID_ARG, mismatched states QIPB200_ERR_SIZE_MISMATCH, sharded
+ * states QIPB200_ERR_UNSUPPORTED, all before any device work.  Pending collapses and layout: `work` plays dst and
+ * `state` src of qipb200_state_apply_pauli_sum.  Synchronises.  Launches f + s + 2 b kernels for the three counts
+ * {f, s, b} of qipb200_pauli_gradient_plan (plus one for a pending collapse on `state`). */
+int qipb200_state_pauli_energy_gradient(qipb200_state *state, qipb200_state *work, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms, const double *angles, const uint64_t *ham_qubits, const char *ham_paulis, const uint32_t *ham_term_len, size_t n_ham, const double *coeffs, double *energy, double *grad);
+/* Host-only (no GPU, ctx-free): out3 = {forward, sum, backward} sweeps of the call above on an unsharded n-qubit state
+ * in canonical layout.  Validates both term lists as the call does. */
+int qipb200_pauli_gradient_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms, const uint64_t *ham_qubits, const char *ham_paulis, const uint32_t *ham_term_len, size_t n_ham, uint32_t *out3);
+
 /* ---- multi-GPU: the 2^n state sharded by its top log2(world) index bits,
  *      one process per GPU (absent in the reference; its only hook is the
  *      input_offset/output_offset slice model, matrix_ops.rs:74-89) -------------- */

@@ -297,6 +297,35 @@ class B200State {
                                                    letters.empty() ? &no_letter : letters.data(), lens.data(),
                                                    terms.size(), angles.data()));
   }
+  // this state <- H src for H = sum_h coeffs[h] P_h, Pauli strings encoded as in expect_paulis; src is another state
+  // of the same context, precision and size, and this state takes its layout (absent in the reference)
+  void apply_pauli_sum(const B200State &src, const std::vector<std::vector<std::pair<char, uint64_t>>> &terms,
+                       const std::vector<double> &coeffs) {
+    if (coeffs.size() != terms.size())
+      throw CircuitError("apply_pauli_sum: " + std::to_string(terms.size()) + " terms but " +
+                         std::to_string(coeffs.size()) + " coefficients");
+    Flat f(terms);
+    ctx_.check(qipb200_state_apply_pauli_sum(st_, src.st_, f.q(), f.l(), f.lens.data(), terms.size(), coeffs.data()));
+  }
+  // energy and gradient of <psi0|U^dagger H U|psi0> by the adjoint method: this state holds psi0 (and ends there up
+  // to rounding), U applies exp(-i angles[t]/2 P_t) for the ansatz strings, term 0 first, H = sum_h coeffs[h] Q_h;
+  // work is scratch of the same size and precision.  A parameter shared by several strings has the sum of their
+  // entries as its derivative (absent in the reference)
+  std::pair<double, std::vector<double>> energy_gradient(
+      B200State &work, const std::vector<std::vector<std::pair<char, uint64_t>>> &ansatz,
+      const std::vector<double> &angles, const std::vector<std::vector<std::pair<char, uint64_t>>> &hamiltonian,
+      const std::vector<double> &coeffs) {
+    if (angles.size() != ansatz.size() || coeffs.size() != hamiltonian.size())
+      throw CircuitError("energy_gradient: " + std::to_string(ansatz.size()) + " terms, " +
+                         std::to_string(angles.size()) + " angles, " + std::to_string(hamiltonian.size()) +
+                         " Hamiltonian terms, " + std::to_string(coeffs.size()) + " coefficients");
+    Flat a(ansatz), h(hamiltonian);
+    std::pair<double, std::vector<double>> out(0.0, std::vector<double>(ansatz.size()));
+    ctx_.check(qipb200_state_pauli_energy_gradient(st_, work.st_, a.q(), a.l(), a.lens.data(), ansatz.size(),
+                                                   angles.data(), h.q(), h.l(), h.lens.data(), hamiltonian.size(),
+                                                   coeffs.data(), &out.first, out.second.data()));
+    return out;
+  }
   // reduced density matrix of up to 10 qubits, row-major 2^k x 2^k; bit i of the row and column index is the value of
   // qubits[i], as in measure_probs (absent in the reference)
   std::vector<std::complex<double>> reduced_density(const std::vector<uint64_t> &qubits) {
@@ -313,6 +342,26 @@ class B200State {
   qipb200_state *get() const { return st_; }
 
  private:
+  // Pauli strings as the flat arrays of the C ABI; a list of identities has no letters, so q() and l() point at
+  // non-NULL (unread) values then, since the C entries refuse NULL arrays
+  struct Flat {
+    std::vector<uint64_t> qubits;
+    std::vector<char> letters;
+    std::vector<uint32_t> lens;
+    uint64_t no_qubit = 0;
+    char no_letter = 'Z';
+    explicit Flat(const std::vector<std::vector<std::pair<char, uint64_t>>> &terms) {
+      for (const auto &t : terms) {
+        lens.push_back((uint32_t)t.size());
+        for (const auto &lq : t) {
+          letters.push_back(lq.first);
+          qubits.push_back(lq.second);
+        }
+      }
+    }
+    const uint64_t *q() const { return qubits.empty() ? &no_qubit : qubits.data(); }
+    const char *l() const { return letters.empty() ? &no_letter : letters.data(); }
+  };
   Context &ctx_;
   size_t n_;
   qipb200_state *st_ = nullptr;

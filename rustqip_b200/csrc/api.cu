@@ -22,6 +22,7 @@
 #include "expect.h"
 #include "kernels.cuh"
 #include "opcompile.h"
+#include "gradient.h"
 #include "pauli_rot.h"
 #include "rdm.h"
 #include "schedule.h"
@@ -1890,12 +1891,8 @@ extern "C" int qipb200_state_collapse(qipb200_state *s, const uint64_t *indices,
 
 namespace {
 
-int expect_impl(qipb200_state *s, const std::vector<PauliTerm> &terms, double *out) {
-  qipb200_ctx *ctx = s->ctx;
-  CU(ctx, cudaSetDevice(ctx->device));
-  int st = materialise_collapse(s);
-  if (st != QIPB200_OK) return st;
-  // A state left permuted (QIPB200_ROTATE) needs no restore_layout sweep: Pauli masks permute with the bits.
+// Logical masks -> physical index bits of s (a permuted layout needs no restore sweep: Pauli masks permute with bits).
+std::vector<PauliTerm> phys_terms(const qipb200_state *s, const std::vector<PauliTerm> &terms) {
   std::vector<PauliTerm> phys(terms.size());
   for (size_t t = 0; t < terms.size(); ++t) {
     phys[t].n_y = terms[t].n_y;
@@ -1905,6 +1902,16 @@ int expect_impl(qipb200_state *s, const std::vector<PauliTerm> &terms, double *o
       if ((terms[t].z >> b) & 1) phys[t].z |= p;
     }
   }
+  return phys;
+}
+
+int expect_impl(qipb200_state *s, const std::vector<PauliTerm> &terms, double *out) {
+  qipb200_ctx *ctx = s->ctx;
+  CU(ctx, cudaSetDevice(ctx->device));
+  int st = materialise_collapse(s);
+  if (st != QIPB200_OK) return st;
+  // A state left permuted (QIPB200_ROTATE) needs no restore_layout sweep: Pauli masks permute with the bits.
+  const std::vector<PauliTerm> phys = phys_terms(s, terms);
   CU(ctx, run_expect(s->prec, s->buf, s->n_local, phys, out, ctx->stream, &ctx->launches));
   return QIPB200_OK;
 }
@@ -1989,15 +1996,7 @@ int pauli_rot_impl(qipb200_state *s, const std::vector<PauliTerm> &terms, const 
   int st = materialise_collapse(s);
   if (st != QIPB200_OK) return st;
   // A state left permuted (QIPB200_ROTATE) is rotated where it is: Pauli masks permute with the bits.
-  std::vector<PauliTerm> phys(terms.size());
-  for (size_t t = 0; t < terms.size(); ++t) {
-    phys[t].n_y = terms[t].n_y;
-    for (uint32_t b = 0; b < s->n; ++b) {
-      const uint64_t p = 1ull << s->phys_of_logical[b];
-      if ((terms[t].x >> b) & 1) phys[t].x |= p;
-      if ((terms[t].z >> b) & 1) phys[t].z |= p;
-    }
-  }
+  const std::vector<PauliTerm> phys = phys_terms(s, terms);
   CU(ctx, run_pauli_rotations(s->prec, s->buf, s->n_local, phys, angles, 2 * ctx->sm_count, ctx->stream,
                               &ctx->launches));
   return QIPB200_OK;
@@ -2038,6 +2037,131 @@ extern "C" int qipb200_pauli_rotation_plan(qip_prec prec, uint32_t n_qubits, con
     int st = parse_pauli_terms(n_qubits, qubits, paulis, term_len, n_terms, &terms, &err);
     if (st != QIPB200_OK) return set_err(nullptr, st, err);
     *sweeps = pauli_rotation_sweep_count(n_qubits, terms);
+    return (int)QIPB200_OK;
+  });
+}
+
+// ===================================================================================
+// Pauli sums and the adjoint energy gradient (gradient.cu)
+// ===================================================================================
+
+namespace {
+
+// dst == src, then context, precision and size, then sharding: the checks the two-state calls share.
+int check_state_pair(const qipb200_state *dst, const qipb200_state *src, const std::string &who) {
+  if (dst == src) return set_err(dst->ctx, QIPB200_ERR_INVALID_ARG, who + ": the two states must differ");
+  if (dst->ctx != src->ctx || dst->prec != src->prec || dst->n != src->n)
+    return set_err(dst->ctx, QIPB200_ERR_SIZE_MISMATCH, who + ": the states differ in context, precision or size");
+  if (dst->world > 1 || !dst->shards.empty() || src->world > 1 || !src->shards.empty())
+    return set_err(dst->ctx, QIPB200_ERR_UNSUPPORTED, who + ": sharded states are not supported");
+  return QIPB200_OK;
+}
+
+int check_finite(qipb200_ctx *ctx, const double *v, size_t n, const std::string &who, const char *what) {
+  if (n && !v) return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL " + what + "s");
+  for (size_t t = 0; t < n; ++t)
+    if (!std::isfinite(v[t]))
+      return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": " + what + " " + std::to_string(t) + " is not finite");
+  return QIPB200_OK;
+}
+
+// src's pending collapse runs, dst's is dropped (dst is overwritten), and dst takes src's layout.
+int prepare_out_of_place(qipb200_state *dst, qipb200_state *src) {
+  int st = materialise_collapse(src);
+  if (st != QIPB200_OK) return st;
+  dst->collapse_pending = false;
+  dst->phys_of_logical = src->phys_of_logical;
+  return QIPB200_OK;
+}
+
+}  // namespace
+
+extern "C" int qipb200_state_apply_pauli_sum(qipb200_state *dst, const qipb200_state *src, const uint64_t *qubits,
+                                             const char *paulis, const uint32_t *term_len, size_t n_terms,
+                                             const double *coeffs) {
+  if (!dst || !src) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, "apply_pauli_sum: NULL state");
+  return guarded(dst->ctx, [&]() -> int {
+    // every check runs before any device work: a refused call leaves both states as they were
+    int st = check_state_pair(dst, src, "apply_pauli_sum");
+    if (st != QIPB200_OK) return st;
+    std::vector<PauliTerm> terms;
+    std::string err;
+    st = parse_pauli_terms(src->n, qubits, paulis, term_len, n_terms, &terms, &err);
+    if (st != QIPB200_OK) return set_err(dst->ctx, st, err);
+    if ((st = check_finite(dst->ctx, coeffs, n_terms, "apply_pauli_sum", "coefficient")) != QIPB200_OK) return st;
+    qipb200_state *s = const_cast<qipb200_state *>(src);  // a pending collapse is applied: the state it stands for
+    qipb200_ctx *ctx = dst->ctx;
+    CU(ctx, cudaSetDevice(ctx->device));
+    if ((st = prepare_out_of_place(dst, s)) != QIPB200_OK) return st;
+    CU(ctx, run_pauli_sum(src->prec, dst->buf, src->buf, src->n_local, phys_terms(src, terms), coeffs, ctx->stream,
+                          &ctx->launches));
+    return (int)QIPB200_OK;
+  });
+}
+
+extern "C" int qipb200_pauli_sum_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, const char *paulis,
+                                      const uint32_t *term_len, size_t n_terms, uint32_t *sweeps) {
+  if (!sweeps || (prec != QIP_F32 && prec != QIP_F64) || n_qubits == 0 || n_qubits > 40)
+    return set_err(nullptr, QIPB200_ERR_INVALID_ARG,
+                   "pauli_sum_plan: NULL sweeps, bad precision or n_qubits not in 1..40");
+  return guarded(nullptr, [&]() -> int {
+    std::vector<PauliTerm> terms;
+    std::string err;
+    int st = parse_pauli_terms(n_qubits, qubits, paulis, term_len, n_terms, &terms, &err);
+    if (st != QIPB200_OK) return set_err(nullptr, st, err);
+    *sweeps = pauli_sum_sweep_count(n_qubits, terms);
+    return (int)QIPB200_OK;
+  });
+}
+
+extern "C" int qipb200_state_pauli_energy_gradient(qipb200_state *state, qipb200_state *work, const uint64_t *qubits,
+                                                   const char *paulis, const uint32_t *term_len, size_t n_terms,
+                                                   const double *angles, const uint64_t *ham_qubits,
+                                                   const char *ham_paulis, const uint32_t *ham_term_len, size_t n_ham,
+                                                   const double *coeffs, double *energy, double *grad) {
+  const char *who = "pauli_energy_gradient";
+  if (!state || !work) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, std::string(who) + ": NULL state");
+  return guarded(state->ctx, [&]() -> int {
+    // every check runs before any device work: a refused call leaves both states as they were
+    int st = check_state_pair(work, state, who);
+    if (st != QIPB200_OK) return st;
+    std::vector<PauliTerm> ansatz, ham;
+    std::string err;
+    st = parse_pauli_terms(state->n, qubits, paulis, term_len, n_terms, &ansatz, &err);
+    if (st != QIPB200_OK) return set_err(state->ctx, st, err);
+    st = parse_pauli_terms(state->n, ham_qubits, ham_paulis, ham_term_len, n_ham, &ham, &err);
+    if (st != QIPB200_OK) return set_err(state->ctx, st, err);
+    if ((st = check_finite(state->ctx, angles, n_terms, who, "angle")) != QIPB200_OK) return st;
+    if ((st = check_finite(state->ctx, coeffs, n_ham, who, "coefficient")) != QIPB200_OK) return st;
+    if (!energy) return set_err(state->ctx, QIPB200_ERR_INVALID_ARG, std::string(who) + ": NULL energy");
+    if (n_terms && !grad) return set_err(state->ctx, QIPB200_ERR_INVALID_ARG, std::string(who) + ": NULL grad");
+    qipb200_ctx *ctx = state->ctx;
+    CU(ctx, cudaSetDevice(ctx->device));
+    if ((st = prepare_out_of_place(work, state)) != QIPB200_OK) return st;
+    CU(ctx, run_pauli_gradient(state->prec, state->buf, work->buf, state->n_local, phys_terms(state, ansatz), angles,
+                               phys_terms(state, ham), coeffs, 2 * ctx->sm_count, ctx->stream, &ctx->launches, energy,
+                               grad));
+    return (int)QIPB200_OK;
+  });
+}
+
+extern "C" int qipb200_pauli_gradient_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits,
+                                           const char *paulis, const uint32_t *term_len, size_t n_terms,
+                                           const uint64_t *ham_qubits, const char *ham_paulis,
+                                           const uint32_t *ham_term_len, size_t n_ham, uint32_t *out3) {
+  if (!out3 || (prec != QIP_F32 && prec != QIP_F64) || n_qubits == 0 || n_qubits > 40)
+    return set_err(nullptr, QIPB200_ERR_INVALID_ARG,
+                   "pauli_gradient_plan: NULL out3, bad precision or n_qubits not in 1..40");
+  return guarded(nullptr, [&]() -> int {
+    std::vector<PauliTerm> ansatz, ham;
+    std::string err;
+    int st = parse_pauli_terms(n_qubits, qubits, paulis, term_len, n_terms, &ansatz, &err);
+    if (st != QIPB200_OK) return set_err(nullptr, st, err);
+    st = parse_pauli_terms(n_qubits, ham_qubits, ham_paulis, ham_term_len, n_ham, &ham, &err);
+    if (st != QIPB200_OK) return set_err(nullptr, st, err);
+    out3[0] = pauli_rotation_sweep_count(n_qubits, ansatz);
+    out3[1] = pauli_sum_sweep_count(n_qubits, ham);
+    out3[2] = pauli_adjoint_sweep_count(n_qubits, ansatz);
     return (int)QIPB200_OK;
   });
 }

@@ -1,0 +1,657 @@
+// gradient.cu -- dst <- H src for a real Pauli sum H = sum_h c_h P_h (qipb200_state_apply_pauli_sum), and the
+// adjoint-method gradient of E = <psi0|U^dagger H U|psi0> for U = R_{T-1} ... R_0, R_t = exp(-i theta_t/2 P_t)
+// (qipb200_state_pauli_energy_gradient).  Planner policies: gradient.h.
+//
+// Geometry.  Both kernels stage two states per CTA, so their tile is the kRotL = 4 lowest index bits plus up to
+// kGradM = 6 chosen high bits: 2^10 amplitudes, four per thread of 256.  One tile or tile pair of each of two states is
+// 64 KiB at f64 (four 16 KiB tiles), which keeps two CTAs per SM at under 113 KiB each.
+//
+// k_pauli_sum.  (P src)_j = i^nY (-1)^popc(k & z) src_k with k = j ^ x, so the terms of one X/Y mask x (a group) share
+// src_k and differ by a real or imaginary sign: the group's coefficient at j is a + i b with
+//   a = sum of +-c_h over the group's terms with nY even, b = the same over nY odd, in list order, in double,
+// (the sign is Re / Im of i^nY times (-1)^popc(k & z_h); the first addition is to +0.0).  Per amplitude, in double and
+// with no FMA contraction:
+//   re = RN(RN(a p.x) - RN(b p.y)), im = RN(RN(a p.y) + RN(b p.x)), acc = (RN(acc.x + re), RN(acc.y + im)),
+// p = src_k widened to double, groups in the sweep's order (gradient.h), sweeps in plan order.  acc starts at +0.0 in
+// the first sweep, which writes dst without reading it, and at the stored dst in later ones; each sweep stores acc
+// rounded to the state's precision (exact at f64).  So dst is a fixed function of the inputs and the plan (made on
+// physical index bits, so it follows the layout), emulated bit for bit in tests/gradient_ref.py.  Forward error, per
+// amplitude j with A_j = sum_h |c_h| |src_(j^x_h)|:
+//   |dst_j - (H src)_j| <= 2 (gamma_(T+G+2)(2^-53) + gamma_S(u)) A_j     (T terms, G groups, S sweeps, u the state's
+// unit roundoff: each component is a sum of at most T + G + 2 rounded double operations on terms bounded by
+// |c_h| (|p.x| + |p.y|), plus one rounding to the state's precision per sweep).  A thread owns its four amplitudes of
+// each tile: src is read from shared memory only, so no barrier separates groups.
+//
+// k_pauli_adjoint.  The backward pass runs over the sweeps of the reversed term list (gradient.h) with the descriptors
+// of pauli_rot.cu for c and -s: R_t^dagger = exp(+i theta_t/2 P_t) is exactly the rotation update of pauli_rot.cu with
+// s negated, so phi (= state) and lambda (= work) go back bit for bit as the emulator says.  Per term, on the pairs
+// (or the diagonal elements) the thread owns by the rules of pauli_rot.cu, barriers included, it first adds
+// Im<lambda|P_t|phi> = sum_j Re(conj(lambda_j) w_j), w_j = -i (P phi)_j, in a double register (f32 amplitudes widened,
+// fma), then undoes R_t on both states.  The first backward sweep adds Re<lambda|phi> (the energy) from the staged tiles
+// before any term, then waits at a CTA barrier: the first term of a sweep carries no barrier of its own (the loop
+// otherwise starts right after the staging barrier), and its pairs may belong to threads of other warps.  Per term the
+// 32 lanes of a warp reduce by butterfly shuffles and lane 0 adds into the warp's slot in shared memory (one slot per warp and row, visits in order); when the CTA has done its tiles it sums its 8 warp slots
+// in warp order into scratch[row][CTA], and k_adjoint_reduce sums each row over the CTAs in CTA order.  The grid is a
+// fixed kAdjGrid CTAs (or the visit count, when smaller): the same inputs give the same bits on any device.
+// A sweep holds at most kAdjMaxTerms terms so the slots fit shared memory: 64 KiB of tiles, 8 x 257 slots and the
+// staged descriptors, at most 91 KiB per CTA.
+#include "gradient.h"
+
+#include <algorithm>
+#include <cmath>
+#include <cstring>
+#include <map>
+
+#include "../../include/qipb200.h"
+#include "pauli_rot.h"
+#include "pauli_rot_dev.cuh"
+
+namespace qipb200 {
+
+namespace {
+
+const uint32_t kGradM = 6;
+const uint32_t kGradTile = 1u << (kRotL + kGradM);
+const int kGradThreads = 256;
+const int kGradPer = kGradTile / kGradThreads;  // tile amplitudes per thread
+const int kGradWarps = kGradThreads / 32;
+const uint32_t kAdjMaxTerms = 256;       // terms of one backward sweep
+const uint32_t kAdjRows = kAdjMaxTerms + 1;  // + the energy
+const int kAdjGrid = 264;
+
+struct SumGroupDev {
+  uint32_t x_in;   // tile-local X/Y mask
+  uint32_t pair;   // the group's partner amplitudes are in the other tile of the pair
+  uint32_t first, end;  // its terms
+};
+
+struct SumTermDev {
+  uint64_t z_out;  // Z/Y bits outside the tile
+  uint32_t z_in;   // tile-local Z/Y mask
+  uint32_t odd;    // nY odd: the term adds to b, else to a
+  double c;        // c_h times the sign of Re / Im of i^nY
+};
+
+__device__ __forceinline__ double2 widen(float2 v) { return make_double2(v.x, v.y); }
+__device__ __forceinline__ double2 widen(double2 v) { return v; }
+__device__ __forceinline__ void narrow(double2 a, float2 *o) { *o = make_float2((float)a.x, (float)a.y); }
+__device__ __forceinline__ void narrow(double2 a, double2 *o) { *o = a; }
+
+template <typename R, bool PAIR>
+__global__ void __launch_bounds__(kGradThreads, 2)
+    k_pauli_sum(R *__restrict__ dst, const R *__restrict__ src, const __grid_constant__ RotArgs a,
+                const SumGroupDev *__restrict__ groups, const SumTermDev *__restrict__ terms, uint32_t accumulate) {
+  typedef typename RotV<R>::type V;
+  extern __shared__ __align__(16) unsigned char smem[];
+  // single tiles: [buffer][src, dst] double-buffered; pairs: src A, src B, dst A, dst B
+  V *tiles = reinterpret_cast<V *>(smem);
+  const int t = threadIdx.x;
+  const uint32_t tsize = 1u << a.tb;
+  uint64_t off[kGradPer];
+#pragma unroll
+  for (int k = 0; k < kGradPer; ++k) {
+    const uint32_t e = t + kGradThreads * k;
+    uint64_t o = e & ((1u << a.L) - 1);
+    for (uint32_t i = 0; i < a.tb - a.L; ++i) o |= (uint64_t)((e >> (a.L + i)) & 1u) << a.hi_pos[i];
+    off[k] = o;
+  }
+  auto base_of = [&](uint64_t v) {
+    uint64_t b = 0;
+    for (uint32_t i = 0; i < a.n_out; ++i) b |= ((v >> i) & 1ull) << a.out_pos[i];
+    return b;
+  };
+  auto issue = [&](uint64_t v, V *S, V *D, V *S2, V *D2) {  // S2, D2: the pair's B tiles
+    const uint64_t b = base_of(v);
+#pragma unroll
+    for (int k = 0; k < kGradPer; ++k) {
+      const uint32_t e = t + kGradThreads * k;
+      if (e >= tsize) continue;
+      cp_async<sizeof(V)>(S + e, src + 2 * (b | off[k]));
+      if (accumulate) cp_async<sizeof(V)>(D + e, dst + 2 * (b | off[k]));
+      if (PAIR) {
+        cp_async<sizeof(V)>(S2 + e, src + 2 * ((b ^ a.x_out) | off[k]));
+        if (accumulate) cp_async<sizeof(V)>(D2 + e, dst + 2 * ((b ^ a.x_out) | off[k]));
+      }
+    }
+  };
+  uint64_t v = blockIdx.x;
+  if (!PAIR) {
+    if (v < a.n_visits) issue(v, tiles, tiles + kGradTile, nullptr, nullptr);
+    cp_async_commit();
+  }
+  int cur = 0;
+  for (; v < a.n_visits; v += gridDim.x) {
+    V *sA, *sB, *dA, *dB;
+    if (PAIR) {
+      sA = tiles;
+      sB = tiles + kGradTile;
+      dA = tiles + 2 * kGradTile;
+      dB = tiles + 3 * kGradTile;
+      issue(v, sA, dA, sB, dB);
+      cp_async_commit();
+      cp_async_wait<0>();
+    } else {
+      sA = tiles + cur * 2 * kGradTile;
+      dA = sA + kGradTile;
+      sB = dB = nullptr;
+      const uint64_t nv = v + gridDim.x;
+      V *nS = tiles + (cur ^ 1) * 2 * kGradTile;
+      if (nv < a.n_visits) issue(nv, nS, nS + kGradTile, nullptr, nullptr);
+      cp_async_commit();
+      cp_async_wait<1>();
+    }
+    __syncthreads();
+    const uint64_t bA = base_of(v), bB = bA ^ a.x_out;
+#pragma unroll 1
+    for (int side = 0; side < (PAIR ? 2 : 1); ++side) {
+      const V *own = side ? sB : sA, *other = side ? sA : sB;
+      const V *D = side ? dB : dA;
+      const uint64_t b = side ? bB : bA, bo = side ? bA : bB;
+      double2 acc[kGradPer];
+#pragma unroll
+      for (int k = 0; k < kGradPer; ++k) {
+        const uint32_t e = t + kGradThreads * k;
+        acc[k] = make_double2(0.0, 0.0);
+        if (accumulate && e < tsize) acc[k] = widen(D[e]);
+      }
+      for (uint32_t g = 0; g < a.n_terms; ++g) {
+        const SumGroupDev G = groups[g];
+        const V *S = (PAIR && G.pair) ? other : own;
+        const uint64_t bk = (PAIR && G.pair) ? bo : b;  // base of the tile that holds k = j ^ x
+        double ca[kGradPer], cb[kGradPer];
+#pragma unroll
+        for (int k = 0; k < kGradPer; ++k) ca[k] = cb[k] = 0.0;
+        for (uint32_t h = G.first; h < G.end; ++h) {
+          const SumTermDev T = terms[h];
+          const uint32_t so = (uint32_t)parity(bk & T.z_out);
+#pragma unroll
+          for (int k = 0; k < kGradPer; ++k) {
+            const uint32_t e = t + kGradThreads * k;
+            const double cv = flip_sign(T.c, so ^ (__popc((e ^ G.x_in) & T.z_in) & 1));
+            if (T.odd)
+              cb[k] = __dadd_rn(cb[k], cv);
+            else
+              ca[k] = __dadd_rn(ca[k], cv);
+          }
+        }
+#pragma unroll
+        for (int k = 0; k < kGradPer; ++k) {
+          const uint32_t e = t + kGradThreads * k;
+          if (e >= tsize) continue;
+          const double2 p = widen(S[e ^ G.x_in]);
+          const double re = __dadd_rn(__dmul_rn(ca[k], p.x), -__dmul_rn(cb[k], p.y));
+          const double im = __dadd_rn(__dmul_rn(ca[k], p.y), __dmul_rn(cb[k], p.x));
+          acc[k].x = __dadd_rn(acc[k].x, re);
+          acc[k].y = __dadd_rn(acc[k].y, im);
+        }
+      }
+#pragma unroll
+      for (int k = 0; k < kGradPer; ++k) {
+        const uint32_t e = t + kGradThreads * k;
+        if (e >= tsize) continue;
+        narrow(acc[k], reinterpret_cast<V *>(dst + 2 * (b | off[k])));
+      }
+    }
+    __syncthreads();  // every thread has read this buffer before the next cp.async writes it
+    if (!PAIR) cur ^= 1;
+  }
+  cp_async_wait<0>();
+}
+
+// Re(conj(l) w) for w = i^ph (+-1) p as rot1 forms it: swap: w = (-p.y, p.x), else (p.x, p.y), times (-1)^neg.
+__device__ __forceinline__ double dot_w(double2 l, double2 p, bool swap, uint32_t neg) {
+  const double d = swap ? fma(l.y, p.x, -l.x * p.y) : fma(l.x, p.x, l.y * p.y);
+  return neg ? -d : d;
+}
+
+__device__ __forceinline__ void slot_add(double *red, uint32_t row, double g) {
+#pragma unroll
+  for (int o = 16; o; o >>= 1) g += __shfl_xor_sync(0xffffffffu, g, o);
+  if ((threadIdx.x & 31) == 0) red[(threadIdx.x >> 5) * kAdjRows + row] += g;
+}
+
+template <typename R, bool PAIR>
+__global__ void __launch_bounds__(kGradThreads, 2)
+    k_pauli_adjoint(R *__restrict__ phi, R *__restrict__ lam, const __grid_constant__ RotArgs a,
+                    const RotTermDev *__restrict__ terms, uint32_t energy, double *__restrict__ scratch) {
+  typedef typename RotV<R>::type V;
+  extern __shared__ __align__(16) unsigned char smem[];
+  // single tiles: [buffer][phi, lambda] double-buffered; pairs: phi A, phi B, lambda A, lambda B
+  V *tiles = reinterpret_cast<V *>(smem);
+  double *red = reinterpret_cast<double *>(smem + 4 * kGradTile * sizeof(V));  // [warp][row]
+  RotTermDev *sT = reinterpret_cast<RotTermDev *>(red + kGradWarps * kAdjRows);
+  const int t = threadIdx.x;
+  const uint32_t rows = a.n_terms + (energy ? 1u : 0u);  // the energy is row n_terms
+  for (uint32_t i = t; i < a.n_terms; i += kGradThreads) sT[i] = terms[i];
+  for (uint32_t i = t; i < kGradWarps * kAdjRows; i += kGradThreads) red[i] = 0.0;  // ordered by the loop's barrier
+  const uint32_t tsize = 1u << a.tb;
+  uint64_t off[kGradPer];
+#pragma unroll
+  for (int k = 0; k < kGradPer; ++k) {
+    const uint32_t e = t + kGradThreads * k;
+    uint64_t o = e & ((1u << a.L) - 1);
+    for (uint32_t i = 0; i < a.tb - a.L; ++i) o |= (uint64_t)((e >> (a.L + i)) & 1u) << a.hi_pos[i];
+    off[k] = o;
+  }
+  auto base_of = [&](uint64_t v) {
+    uint64_t b = 0;
+    for (uint32_t i = 0; i < a.n_out; ++i) b |= ((v >> i) & 1ull) << a.out_pos[i];
+    return b;
+  };
+  auto issue = [&](uint64_t v, V *P, V *Lm, V *P2, V *L2) {  // P2, L2: the pair's B tiles
+    const uint64_t b = base_of(v);
+#pragma unroll
+    for (int k = 0; k < kGradPer; ++k) {
+      const uint32_t e = t + kGradThreads * k;
+      if (e >= tsize) continue;
+      cp_async<sizeof(V)>(P + e, phi + 2 * (b | off[k]));
+      cp_async<sizeof(V)>(Lm + e, lam + 2 * (b | off[k]));
+      if (PAIR) {
+        cp_async<sizeof(V)>(P2 + e, phi + 2 * ((b ^ a.x_out) | off[k]));
+        cp_async<sizeof(V)>(L2 + e, lam + 2 * ((b ^ a.x_out) | off[k]));
+      }
+    }
+  };
+  uint64_t v = blockIdx.x;
+  if (!PAIR) {
+    if (v < a.n_visits) issue(v, tiles, tiles + kGradTile, nullptr, nullptr);
+    cp_async_commit();
+  }
+  int cur = 0;
+  for (; v < a.n_visits; v += gridDim.x) {
+    V *pA, *pB, *lA, *lB;
+    if (PAIR) {
+      pA = tiles;
+      pB = tiles + kGradTile;
+      lA = tiles + 2 * kGradTile;
+      lB = tiles + 3 * kGradTile;
+      issue(v, pA, lA, pB, lB);
+      cp_async_commit();
+      cp_async_wait<0>();
+    } else {
+      pA = tiles + cur * 2 * kGradTile;
+      lA = pA + kGradTile;
+      pB = lB = nullptr;
+      const uint64_t nv = v + gridDim.x;
+      V *nP = tiles + (cur ^ 1) * 2 * kGradTile;
+      if (nv < a.n_visits) issue(nv, nP, nP + kGradTile, nullptr, nullptr);
+      cp_async_commit();
+      cp_async_wait<1>();
+    }
+    __syncthreads();
+    const uint64_t bA = base_of(v), bB = bA ^ a.x_out;
+    if (energy) {  // Re<lambda|phi> on the thread's own elements, before any term is undone
+      double g = 0.0;
+      for (int side = 0; side < (PAIR ? 2 : 1); ++side) {
+        const V *P = side ? pB : pA, *Lm = side ? lB : lA;
+#pragma unroll
+        for (int k = 0; k < kGradPer; ++k) {
+          const uint32_t e = t + kGradThreads * k;
+          if (e < tsize) g += dot_w(widen(Lm[e]), widen(P[e]), false, 0);
+        }
+      }
+      slot_add(red, a.n_terms, g);
+      // the first term of a sweep carries no barrier and may update elements other warps have yet to read here
+      __syncthreads();
+    }
+    for (uint32_t i = 0; i < a.n_terms;) {
+      const RotTermDev T = sT[i];
+      if (T.flags & kRotBarrier) __syncthreads();
+      if (T.flags & kRotDiag) {  // a run of diagonal terms on the thread's own elements, in registers, tile by tile
+        const uint32_t end = i + T.aux;
+#pragma unroll 1
+        for (int side = 0; side < (PAIR ? 2 : 1); ++side) {
+          V *P = side ? pB : pA, *Lm = side ? lB : lA;
+          const uint64_t b = side ? bB : bA;
+          V r[kGradPer], q[kGradPer];
+#pragma unroll
+          for (int k = 0; k < kGradPer; ++k) {
+            const uint32_t e = t + kGradThreads * k;
+            r[k].x = r[k].y = q[k].x = q[k].y = (R)0;  // elements past a small tile add 0 and are never stored
+            if (e < tsize) {
+              r[k] = P[e];
+              q[k] = Lm[e];
+            }
+          }
+          for (uint32_t j = i; j < end; ++j) {
+            const RotTermDev D = sT[j];
+            const uint32_t ph = D.flags & kRotPhase;
+            const bool swap = ph & 1;
+            const R c = (R)D.c, s = flip_sign((R)D.s, ph >> 1);
+            // sign of element k (e = t + 256 k): parity(t & z_in) ^ parity(k & z_in >> 8) ^ parity(base & z_out)
+            const uint32_t zk = D.z_in >> 8;
+            const uint32_t par4 = ((zk & 1) ? 0xAu : 0u) ^ ((zk & 2) ? 0xCu : 0u);
+            const uint32_t f = par4 ^ (((__popc((uint32_t)t & D.z_in) & 1) ^ (uint32_t)parity(b & D.z_out)) ? 0xFu : 0u);
+            double g = 0.0;
+#pragma unroll
+            for (int k = 0; k < kGradPer; ++k) {
+              const uint32_t nk = (f >> k) & 1;
+              g += dot_w(widen(q[k]), widen(r[k]), swap, nk ^ (ph >> 1));
+              r[k] = rot1<R, V>(r[k], r[k], c, flip_sign(s, nk), swap);
+              q[k] = rot1<R, V>(q[k], q[k], c, flip_sign(s, nk), swap);
+            }
+            slot_add(red, j, g);
+          }
+#pragma unroll
+          for (int k = 0; k < kGradPer; ++k) {
+            const uint32_t e = t + kGradThreads * k;
+            if (e < tsize) {
+              P[e] = r[k];
+              Lm[e] = q[k];
+            }
+          }
+        }
+        i = end;
+        continue;
+      }
+      const uint32_t ph = T.flags & kRotPhase;
+      const bool swap = ph & 1;
+      const R c = (R)T.c, s = flip_sign((R)T.s, ph >> 1);
+      double g = 0.0;
+      if (PAIR && (T.flags & kRotPair)) {  // (A[e], B[e ^ x_in]) for the thread's own e
+        const uint32_t nA = parity(bA & T.z_out), nB = parity(bB & T.z_out);
+#pragma unroll
+        for (int k = 0; k < kGradPer; ++k) {
+          const uint32_t e = t + kGradThreads * k;
+          if (e >= tsize) continue;
+          const uint32_t f = e ^ T.x_in;
+          const uint32_t sa = nB ^ (__popc(f & T.z_in) & 1), sb = nA ^ (__popc(e & T.z_in) & 1);
+          const V u = pA[e], w = pB[f], lu = lA[e], lw = lB[f];
+          g += dot_w(widen(lu), widen(w), swap, sa ^ (ph >> 1)) + dot_w(widen(lw), widen(u), swap, sb ^ (ph >> 1));
+          pA[e] = rot1<R, V>(u, w, c, flip_sign(s, sa), swap);
+          pB[f] = rot1<R, V>(w, u, c, flip_sign(s, sb), swap);
+          lA[e] = rot1<R, V>(lu, lw, c, flip_sign(s, sa), swap);
+          lB[f] = rot1<R, V>(lw, lu, c, flip_sign(s, sb), swap);
+        }
+      } else {  // the thread's pairs (e, e ^ x_in) with bit aux of e clear, on each tile
+        const uint32_t h = T.aux;
+#pragma unroll 1
+        for (int side = 0; side < (PAIR ? 2 : 1); ++side) {
+          V *P = side ? pB : pA, *Lm = side ? lB : lA;
+          const uint32_t no = parity((side ? bB : bA) & T.z_out);
+#pragma unroll
+          for (int k = 0; k < kGradPer / 2; ++k) {
+            const uint32_t p = t + kGradThreads * k;
+            if (2 * p >= tsize) continue;
+            const uint32_t e = ((p >> h) << (h + 1)) | (p & ((1u << h) - 1)), f = e ^ T.x_in;
+            const uint32_t se = no ^ (__popc(f & T.z_in) & 1), sf = no ^ (__popc(e & T.z_in) & 1);
+            const V u = P[e], w = P[f], lu = Lm[e], lw = Lm[f];
+            g += dot_w(widen(lu), widen(w), swap, se ^ (ph >> 1)) + dot_w(widen(lw), widen(u), swap, sf ^ (ph >> 1));
+            P[e] = rot1<R, V>(u, w, c, flip_sign(s, se), swap);
+            P[f] = rot1<R, V>(w, u, c, flip_sign(s, sf), swap);
+            Lm[e] = rot1<R, V>(lu, lw, c, flip_sign(s, se), swap);
+            Lm[f] = rot1<R, V>(lw, lu, c, flip_sign(s, sf), swap);
+          }
+        }
+      }
+      slot_add(red, i, g);
+      ++i;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < kGradPer; ++k) {
+      const uint32_t e = t + kGradThreads * k;
+      if (e >= tsize) continue;
+      *reinterpret_cast<V *>(phi + 2 * (bA | off[k])) = pA[e];
+      *reinterpret_cast<V *>(lam + 2 * (bA | off[k])) = lA[e];
+      if (PAIR) {
+        *reinterpret_cast<V *>(phi + 2 * (bB | off[k])) = pB[e];
+        *reinterpret_cast<V *>(lam + 2 * (bB | off[k])) = lB[e];
+      }
+    }
+    __syncthreads();  // the stores have read this buffer before the next cp.async writes it
+    if (!PAIR) cur ^= 1;
+  }
+  cp_async_wait<0>();
+  __syncthreads();
+  for (uint32_t r = t; r < rows; r += kGradThreads) {
+    double s = 0.0;
+    for (int w = 0; w < kGradWarps; ++w) s += red[w * kAdjRows + r];
+    scratch[(uint64_t)r * gridDim.x + blockIdx.x] = s;
+  }
+}
+
+// res[idx] = sum over CTAs in order of scratch[row][CTA]; row i < n_terms is reversed position first + i, that is term
+// T - 1 - first - i, at res[1 + that term]; row n_terms (energy sweeps) is the energy at res[0].
+__global__ void __launch_bounds__(256) k_adjoint_reduce(const double *__restrict__ scratch, uint32_t rows,
+                                                         uint32_t grid, uint32_t n_terms, uint32_t T, uint32_t first,
+                                                         double *__restrict__ res) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= rows) return;
+  double s = 0.0;
+  for (uint32_t c = 0; c < grid; ++c) s += scratch[(uint64_t)r * grid + c];
+  res[r == n_terms ? 0 : T - first - r] = s;
+}
+
+// ---- host ----------------------------------------------------------------------------------------------------------
+
+struct SumGroup {
+  uint64_t x = 0;
+  std::vector<uint32_t> terms;
+};
+
+struct SumSweep {
+  RotSweep geo;
+  std::vector<uint32_t> groups;  // indices into the group list, in order
+};
+
+void plan_sum(uint32_t n, const std::vector<PauliTerm> &terms, std::vector<SumGroup> *groups_out,
+              std::vector<SumSweep> *out) {
+  const uint32_t L = std::min(kRotL, n), m = std::min(kGradM, n - L);
+  const uint64_t low = (1ull << L) - 1;
+  std::vector<SumGroup> &gr = *groups_out;
+  gr.clear();
+  std::map<uint64_t, size_t> where;
+  for (uint32_t t = 0; t < (uint32_t)terms.size(); ++t) {
+    auto it = where.find(terms[t].x);
+    if (it == where.end()) {
+      it = where.emplace(terms[t].x, gr.size()).first;
+      gr.push_back(SumGroup());
+      gr.back().x = terms[t].x;
+    }
+    gr[it->second].terms.push_back(t);
+  }
+  std::vector<SumSweep> &sw = *out;
+  sw.clear();
+  std::vector<bool> used(gr.size(), false);
+  size_t left = gr.size();
+  while (left) {
+    SumSweep S;
+    for (size_t g = 0; g < gr.size(); ++g)
+      if (!used[g] && rot_sweep_join(&S.geo, gr[g].x, low, m)) {
+        used[g] = true;
+        --left;
+        S.groups.push_back((uint32_t)g);
+      }
+    sw.push_back(S);
+  }
+  for (SumSweep &S : sw) rot_sweep_fill(&S.geo, n, L, m);
+}
+
+void plan_adjoint(uint32_t n, const std::vector<PauliTerm> &rev, std::vector<RotSweep> *out) {
+  std::vector<RotSweep> sw;
+  plan_rot_sweeps(n, kGradM, rev, &sw);
+  out->clear();
+  if (sw.empty()) {  // no terms: one sweep for the energy, on the tile of the lowest bits
+    const uint32_t L = std::min(kRotL, n), m = std::min(kGradM, n - L);
+    RotSweep S;
+    rot_sweep_fill(&S, n, L, m);
+    out->push_back(S);
+    return;
+  }
+  for (const RotSweep &S : sw)
+    for (uint32_t f = S.first; f < S.end; f += kAdjMaxTerms) {
+      RotSweep P = S;
+      P.first = f;
+      P.end = std::min(S.end, f + kAdjMaxTerms);
+      out->push_back(P);
+    }
+}
+
+template <typename R, bool PAIR>
+cudaError_t launch_sum(void *dst, const void *src, const RotArgs &a, const SumGroupDev *g, const SumTermDev *t,
+                       uint32_t accumulate, cudaStream_t s) {
+  typedef typename RotV<R>::type V;
+  static_assert(4 * kGradTile * sizeof(double2) <= 113 * 1024, "two CTAs per SM: at most 113 KiB of shared memory each");
+  const size_t smem = 4 * kGradTile * sizeof(V);
+  cudaError_t e = cudaFuncSetAttribute(k_pauli_sum<R, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  const int grid = (int)std::min<uint64_t>(a.n_visits, (uint64_t)kAdjGrid);
+  k_pauli_sum<R, PAIR><<<grid, kGradThreads, smem, s>>>((R *)dst, (const R *)src, a, g, t, accumulate);
+  return cudaGetLastError();
+}
+
+template <typename R, bool PAIR>
+cudaError_t launch_adjoint(void *phi, void *lam, const RotArgs &a, const RotTermDev *terms, uint32_t energy,
+                           double *scratch, int grid, cudaStream_t s) {
+  typedef typename RotV<R>::type V;
+  static_assert(kGradThreads == 256 && kGradPer == 4, "the diagonal path's sign table assumes e = t + 256 k, k < 4");
+  const size_t fixed = 4 * kGradTile * sizeof(V) + kGradWarps * kAdjRows * sizeof(double);
+  static_assert(4 * kGradTile * sizeof(double2) + kGradWarps * kAdjRows * sizeof(double) +
+                        kAdjMaxTerms * sizeof(RotTermDev) <= 113 * 1024,
+                "two CTAs per SM: at most 113 KiB of shared memory each");
+  const size_t smem = fixed + a.n_terms * sizeof(RotTermDev);
+  cudaError_t e = cudaFuncSetAttribute(k_pauli_adjoint<R, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)(fixed + kAdjMaxTerms * sizeof(RotTermDev)));
+  if (e != cudaSuccess) return e;
+  k_pauli_adjoint<R, PAIR><<<grid, kGradThreads, smem, s>>>((R *)phi, (R *)lam, a, terms, energy, scratch);
+  return cudaGetLastError();
+}
+
+}  // namespace
+
+uint32_t pauli_sum_sweep_count(uint32_t n, const std::vector<PauliTerm> &terms) {
+  std::vector<SumGroup> gr;
+  std::vector<SumSweep> sw;
+  plan_sum(n, terms, &gr, &sw);
+  return (uint32_t)sw.size();
+}
+
+uint32_t pauli_adjoint_sweep_count(uint32_t n, const std::vector<PauliTerm> &ansatz) {
+  std::vector<PauliTerm> rev(ansatz.rbegin(), ansatz.rend());
+  std::vector<RotSweep> sw;
+  plan_adjoint(n, rev, &sw);
+  return (uint32_t)sw.size();
+}
+
+cudaError_t run_pauli_sum(qip_prec prec, void *dst, const void *src, uint32_t n, const std::vector<PauliTerm> &terms,
+                          const double *coeffs, cudaStream_t s, uint64_t *launches) {
+  const size_t amp_bytes = (prec == QIP_F32 ? 2 * sizeof(float) : 2 * sizeof(double)) << n;
+  if (terms.empty()) return cudaMemsetAsync(dst, 0, amp_bytes, s);  // the empty sum
+  std::vector<SumGroup> gr;
+  std::vector<SumSweep> sw;
+  plan_sum(n, terms, &gr, &sw);
+  const uint32_t L = std::min(kRotL, n);
+  const uint64_t low = (1ull << L) - 1;
+  std::vector<RotArgs> args(sw.size());
+  std::vector<SumGroupDev> hg;
+  std::vector<SumTermDev> ht;
+  std::vector<size_t> g_off(sw.size());
+  for (size_t k = 0; k < sw.size(); ++k) {
+    const SumSweep &S = sw[k];
+    RotArgs &a = args[k];
+    memset(&a, 0, sizeof(a));
+    std::vector<uint32_t> hi_pos;
+    rot_geometry(n, L, S.geo.hi, S.geo.x_out, &a, &hi_pos);
+    const uint64_t tile = low | S.geo.hi;
+    a.n_terms = (uint32_t)S.groups.size();  // groups, for this kernel
+    g_off[k] = hg.size();
+    for (uint32_t gi : S.groups) {
+      const SumGroup &G = gr[gi];
+      const uint64_t xo = G.x & ~tile;
+      if (xo != 0 && xo != S.geo.x_out) return cudaErrorInvalidValue;  // the planner's invariant
+      SumGroupDev gd;
+      gd.x_in = compact_tile_bits(G.x & tile, L, hi_pos);
+      gd.pair = xo ? 1u : 0u;
+      gd.first = (uint32_t)ht.size();
+      for (uint32_t t : G.terms) {
+        const PauliTerm &P = terms[t];
+        SumTermDev td;
+        td.z_out = P.z & ~tile;
+        td.z_in = compact_tile_bits(P.z & tile, L, hi_pos);
+        td.odd = P.n_y & 1;
+        td.c = ((P.n_y & 3) >= 2) ? -coeffs[t] : coeffs[t];  // i^nY = 1, i, -1, -i
+        ht.push_back(td);
+      }
+      gd.end = (uint32_t)ht.size();
+      hg.push_back(gd);
+    }
+  }
+  const size_t gbytes = hg.size() * sizeof(SumGroupDev), tbytes = ht.size() * sizeof(SumTermDev);
+  char *d = nullptr;
+  cudaError_t e = cudaMallocAsync((void **)&d, tbytes + gbytes, s);
+  if (e != cudaSuccess) return e;
+  SumTermDev *dt = (SumTermDev *)d;
+  SumGroupDev *dg = (SumGroupDev *)(d + tbytes);
+  // pageable sources: the copies are staged before cudaMemcpyAsync returns
+  e = cudaMemcpyAsync(dt, ht.data(), tbytes, cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(dg, hg.data(), gbytes, cudaMemcpyHostToDevice, s);
+  for (size_t k = 0; k < sw.size() && e == cudaSuccess; ++k) {
+    const uint32_t acc = k > 0;
+    const SumGroupDev *g = dg + g_off[k];
+    if (prec == QIP_F32)
+      e = args[k].x_out ? launch_sum<float, true>(dst, src, args[k], g, dt, acc, s)
+                        : launch_sum<float, false>(dst, src, args[k], g, dt, acc, s);
+    else
+      e = args[k].x_out ? launch_sum<double, true>(dst, src, args[k], g, dt, acc, s)
+                        : launch_sum<double, false>(dst, src, args[k], g, dt, acc, s);
+    ++*launches;
+  }
+  const cudaError_t ef = cudaFreeAsync(d, s);
+  return e != cudaSuccess ? e : ef;
+}
+
+cudaError_t run_pauli_gradient(qip_prec prec, void *state, void *work, uint32_t n, const std::vector<PauliTerm> &ansatz,
+                               const double *angles, const std::vector<PauliTerm> &ham, const double *coeffs, int grid,
+                               cudaStream_t s, uint64_t *launches, double *energy, double *grad) {
+  const uint32_t T = (uint32_t)ansatz.size();
+  cudaError_t e = run_pauli_rotations(prec, state, n, ansatz, angles, grid, s, launches);
+  if (e == cudaSuccess) e = run_pauli_sum(prec, work, state, n, ham, coeffs, s, launches);
+  if (e != cudaSuccess) return e;
+  std::vector<PauliTerm> rev(ansatz.rbegin(), ansatz.rend());
+  std::vector<double> rev_angles(angles ? std::vector<double>(angles, angles + T) : std::vector<double>());
+  std::reverse(rev_angles.begin(), rev_angles.end());
+  std::vector<RotSweep> sw;
+  plan_adjoint(n, rev, &sw);
+  std::vector<RotArgs> args;
+  std::vector<RotTermDev> ht;
+  if (!build_rot_tables(prec, n, rev, rev_angles.data(), true, sw, &args, &ht)) return cudaErrorInvalidValue;
+  const size_t tbytes = std::max<size_t>(1, ht.size()) * sizeof(RotTermDev);
+  const size_t sbytes = (size_t)kAdjRows * kAdjGrid * sizeof(double), rbytes = (T + 1) * sizeof(double);
+  char *d = nullptr;
+  e = cudaMallocAsync((void **)&d, tbytes + sbytes + rbytes, s);
+  if (e != cudaSuccess) return e;
+  RotTermDev *dt = (RotTermDev *)d;
+  double *scratch = (double *)(d + tbytes);
+  double *res = (double *)(d + tbytes + sbytes);
+  if (!ht.empty()) e = cudaMemcpyAsync(dt, ht.data(), ht.size() * sizeof(RotTermDev), cudaMemcpyHostToDevice, s);
+  for (size_t k = 0; k < sw.size() && e == cudaSuccess; ++k) {
+    RotArgs &a = args[k];
+    const uint32_t en = k == 0, g = (uint32_t)std::min<uint64_t>(a.n_visits, (uint64_t)kAdjGrid);
+    const RotTermDev *td = dt + sw[k].first;
+    if (prec == QIP_F32)
+      e = a.x_out ? launch_adjoint<float, true>(state, work, a, td, en, scratch, g, s)
+                  : launch_adjoint<float, false>(state, work, a, td, en, scratch, g, s);
+    else
+      e = a.x_out ? launch_adjoint<double, true>(state, work, a, td, en, scratch, g, s)
+                  : launch_adjoint<double, false>(state, work, a, td, en, scratch, g, s);
+    ++*launches;
+    if (e != cudaSuccess) break;
+    const uint32_t rows = a.n_terms + en;
+    k_adjoint_reduce<<<(rows + 255) / 256, 256, 0, s>>>(scratch, rows, g, a.n_terms, T, sw[k].first, res);
+    e = cudaGetLastError();
+    ++*launches;
+  }
+  std::vector<double> host(T + 1);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(host.data(), res, rbytes, cudaMemcpyDeviceToHost, s);
+  const cudaError_t ef = cudaFreeAsync(d, s);
+  const cudaError_t es = cudaStreamSynchronize(s);
+  if (e != cudaSuccess) return e;
+  if (ef != cudaSuccess) return ef;
+  if (es != cudaSuccess) return es;
+  *energy = host[0];
+  for (uint32_t t = 0; t < T; ++t) grad[t] = host[1 + t];
+  return cudaSuccess;
+}
+
+}  // namespace qipb200

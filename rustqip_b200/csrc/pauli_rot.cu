@@ -25,6 +25,7 @@
 // memory, later ones are read from global memory, so a run of any length fits one sweep if its geometry does.
 // Shared memory: two tiles plus the staged descriptors, at most 74 KiB per CTA (two CTAs per SM).
 #include "pauli_rot.h"
+#include "pauli_rot_dev.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -37,92 +38,11 @@ namespace qipb200 {
 
 namespace {
 
-const uint32_t kRotL = 4;   // low index bits of a tile (runs of 16 amplitudes)
 const uint32_t kRotM = 7;   // chosen high bits of a tile
 const uint32_t kRotTile = 1u << (kRotL + kRotM);
 const int kRotThreads = 256;
 const int kRotPer = kRotTile / kRotThreads;  // tile amplitudes per thread
 const uint32_t kRotSmemTerms = 256;          // descriptors staged in shared memory; later ones are read from global
-
-enum : uint32_t {
-  kRotPhase = 3u,     // w = i^phase (+-1) psi_partner
-  kRotPair = 4u,      // the term's partner is in the other tile of the pair
-  kRotBarrier = 8u,   // ownership differs from the previous term's: __syncthreads first
-  kRotDiag = 16u,     // x == 0
-};
-
-struct RotTermDev {
-  uint64_t z_out;  // Z/Y bits outside the tile
-  uint32_t x_in;   // tile-local X/Y mask
-  uint32_t z_in;   // tile-local Z/Y mask
-  double c, s;     // cos and sin of theta/2, rounded to the state's precision
-  uint32_t flags;
-  uint32_t aux;    // kRotDiag: length of the diagonal run this term starts; one-tile terms: lowest bit of x_in
-};
-
-struct RotArgs {
-  uint64_t x_out;     // 0, or the out-of-tile X/Y mask shared by the sweep
-  uint64_t n_visits;  // tiles (x_out == 0) or tile pairs
-  uint32_t L, tb;     // low bits, tile bits
-  uint32_t n_out;     // bits of the visit index, spread over out_pos
-  uint32_t n_terms;
-  uint8_t hi_pos[kRotM];
-  uint8_t out_pos[64];
-};
-
-template <typename R>
-struct RotV;
-template <>
-struct RotV<float> {
-  typedef float2 type;
-};
-template <>
-struct RotV<double> {
-  typedef double2 type;
-};
-
-__device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
-__device__ __forceinline__ double mul_rn(double a, double b) { return __dmul_rn(a, b); }
-__device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }
-__device__ __forceinline__ double add_rn(double a, double b) { return __dadd_rn(a, b); }
-
-__device__ __forceinline__ bool parity(uint64_t v) { return __popcll(v) & 1; }
-
-__device__ __forceinline__ float flip_sign(float v, uint32_t bit) {
-  return __int_as_float(__float_as_int(v) ^ (int)(bit << 31));
-}
-__device__ __forceinline__ double flip_sign(double v, uint32_t bit) {
-  return __hiloint2double(__double2hiint(v) ^ (int)(bit << 31), __double2loint(v));
-}
-
-// c a + s w with w = i^ph (+-1) p, for s that already carries the sign (-1)^(ph >> 1) (+-1) and swap = ph & 1:
-// w = (-p.y, p.x) or (p.x, p.y) up to that sign.  RN(s (-v)) = -RN(s v), so these are the bits of the definition.
-template <typename R, typename V>
-__device__ __forceinline__ V rot1(V a, V p, R c, R s, bool swap) {
-  V o;
-  if (swap) {
-    o.x = add_rn(mul_rn(c, a.x), -mul_rn(s, p.y));
-    o.y = add_rn(mul_rn(c, a.y), mul_rn(s, p.x));
-  } else {
-    o.x = add_rn(mul_rn(c, a.x), mul_rn(s, p.x));
-    o.y = add_rn(mul_rn(c, a.y), mul_rn(s, p.y));
-  }
-  return o;
-}
-
-template <int B>
-__device__ __forceinline__ void cp_async(void *sdst, const void *gsrc) {
-  const uint32_t d = (uint32_t)__cvta_generic_to_shared(sdst);
-  if (B == 16)
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(d), "l"(gsrc) : "memory");
-  else
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;\n" ::"r"(d), "l"(gsrc) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-  asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory");
-}
 
 // One one-tile term with x_in != 0 on tile X (base b): the thread's pairs (e, e ^ x_in), e with bit h clear.
 template <typename R, typename V>
@@ -271,61 +191,6 @@ __global__ void __launch_bounds__(kRotThreads, 2)
   cp_async_wait<0>();
 }
 
-// ---- host: the sweep planner (policy in pauli_rot.h) --------------------------------------------------------------
-
-struct RotSweep {
-  uint64_t hi = 0;     // chosen high tile bits
-  uint64_t x_out = 0;  // out-of-tile X/Y mask shared by the sweep
-  uint32_t first = 0, end = 0;
-};
-
-int popc64(uint64_t v) { return __builtin_popcountll(v); }
-
-void plan_rot_sweeps(uint32_t n, const std::vector<PauliTerm> &terms, std::vector<RotSweep> *out) {
-  const uint32_t L = std::min(kRotL, n), m = std::min(kRotM, n - L);
-  const uint64_t low = (1ull << L) - 1;
-  auto join = [&](RotSweep &S, uint64_t x) {
-    const uint64_t r = x & ~(low | S.hi);
-    if (r == 0 || r == S.x_out) return true;
-    if (!(r & S.x_out) && (uint32_t)(popc64(S.hi) + popc64(r)) <= m) {
-      S.hi |= r;
-      return true;
-    }
-    if (S.x_out == 0) {
-      S.x_out = r;
-      return true;
-    }
-    return false;
-  };
-  std::vector<RotSweep> &sw = *out;
-  sw.clear();
-  if (terms.empty()) return;
-  sw.push_back(RotSweep());
-  for (uint32_t t = 0; t < (uint32_t)terms.size(); ++t) {
-    if (join(sw.back(), terms[t].x)) continue;
-    sw.back().end = t;
-    sw.push_back(RotSweep());
-    sw.back().first = t;
-    join(sw.back(), terms[t].x);  // always joins an empty sweep
-  }
-  sw.back().end = (uint32_t)terms.size();
-  for (RotSweep &S : sw) {
-    // free tile bits: first x_out bits (fewer tile pairs), then the lowest free bits (longer contiguous runs)
-    for (uint32_t b = 0; b < n && (uint32_t)popc64(S.hi) < m; ++b)
-      if ((S.x_out >> b) & 1) {
-        S.hi |= 1ull << b;
-        S.x_out &= ~(1ull << b);
-      }
-    for (uint32_t b = L; b < n && (uint32_t)popc64(S.hi) < m; ++b) S.hi |= 1ull << b;
-  }
-}
-
-uint32_t compact(uint64_t v, uint32_t L, const std::vector<uint32_t> &hi_pos) {
-  uint32_t r = (uint32_t)(v & ((1ull << L) - 1));
-  for (size_t i = 0; i < hi_pos.size(); ++i) r |= (uint32_t)((v >> hi_pos[i]) & 1ull) << (L + i);
-  return r;
-}
-
 template <typename R, bool PAIR>
 cudaError_t launch_rot(void *psi, const RotArgs &a, const RotTermDev *terms, int grid, cudaStream_t s) {
   typedef typename RotV<R>::type V;
@@ -342,37 +207,87 @@ cudaError_t launch_rot(void *psi, const RotArgs &a, const RotTermDev *terms, int
 
 }  // namespace
 
-uint32_t pauli_rotation_sweep_count(uint32_t n, const std::vector<PauliTerm> &terms) {
-  std::vector<RotSweep> sw;
-  plan_rot_sweeps(n, terms, &sw);
-  return (uint32_t)sw.size();
+// ---- host: the sweep planner (policy in pauli_rot.h) and the descriptor tables --------------------------------------
+
+bool rot_sweep_join(RotSweep *S, uint64_t x, uint64_t low, uint32_t m) {
+  const uint64_t r = x & ~(low | S->hi);
+  if (r == 0 || r == S->x_out) return true;
+  if (!(r & S->x_out) && (uint32_t)(__builtin_popcountll(S->hi) + __builtin_popcountll(r)) <= m) {
+    S->hi |= r;
+    return true;
+  }
+  if (S->x_out == 0) {
+    S->x_out = r;
+    return true;
+  }
+  return false;
 }
 
-cudaError_t run_pauli_rotations(qip_prec prec, void *psi, uint32_t n, const std::vector<PauliTerm> &terms,
-                                const double *angles, int grid, cudaStream_t s, uint64_t *launches) {
-  if (terms.empty()) return cudaSuccess;
-  std::vector<RotSweep> sw;
-  plan_rot_sweeps(n, terms, &sw);
+void rot_sweep_fill(RotSweep *S, uint32_t n, uint32_t L, uint32_t m) {
+  for (uint32_t b = 0; b < n && (uint32_t)__builtin_popcountll(S->hi) < m; ++b)
+    if ((S->x_out >> b) & 1) {
+      S->hi |= 1ull << b;
+      S->x_out &= ~(1ull << b);
+    }
+  for (uint32_t b = L; b < n && (uint32_t)__builtin_popcountll(S->hi) < m; ++b) S->hi |= 1ull << b;
+}
+
+void plan_rot_sweeps(uint32_t n, uint32_t m_max, const std::vector<PauliTerm> &terms, std::vector<RotSweep> *out) {
+  const uint32_t L = std::min(kRotL, n), m = std::min(m_max, n - L);
+  const uint64_t low = (1ull << L) - 1;
+  std::vector<RotSweep> &sw = *out;
+  sw.clear();
+  if (terms.empty()) return;
+  sw.push_back(RotSweep());
+  for (uint32_t t = 0; t < (uint32_t)terms.size(); ++t) {
+    if (rot_sweep_join(&sw.back(), terms[t].x, low, m)) continue;
+    sw.back().end = t;
+    sw.push_back(RotSweep());
+    sw.back().first = t;
+    rot_sweep_join(&sw.back(), terms[t].x, low, m);  // always joins an empty sweep
+  }
+  sw.back().end = (uint32_t)terms.size();
+  for (RotSweep &S : sw) rot_sweep_fill(&S, n, L, m);
+}
+
+uint32_t compact_tile_bits(uint64_t v, uint32_t L, const std::vector<uint32_t> &hi_pos) {
+  uint32_t r = (uint32_t)(v & ((1ull << L) - 1));
+  for (size_t i = 0; i < hi_pos.size(); ++i) r |= (uint32_t)((v >> hi_pos[i]) & 1ull) << (L + i);
+  return r;
+}
+
+void rot_geometry(uint32_t n, uint32_t L, uint64_t hi, uint64_t x_out, RotArgs *a, std::vector<uint32_t> *hi_pos) {
+  hi_pos->clear();
+  for (uint32_t b = 0; b < n; ++b)
+    if ((hi >> b) & 1) hi_pos->push_back(b);
+  const uint64_t tile = ((1ull << L) - 1) | hi;
+  a->x_out = x_out;
+  a->L = L;
+  a->tb = L + (uint32_t)hi_pos->size();
+  for (size_t i = 0; i < hi_pos->size(); ++i) a->hi_pos[i] = (uint8_t)(*hi_pos)[i];
+  const int pair_bit = x_out ? __builtin_ctzll(x_out) : -1;
+  a->n_out = 0;
+  for (uint32_t b = 0; b < n; ++b)
+    if (!((tile >> b) & 1) && (int)b != pair_bit) a->out_pos[a->n_out++] = (uint8_t)b;
+  a->n_visits = 1ull << a->n_out;
+}
+
+bool build_rot_tables(qip_prec prec, uint32_t n, const std::vector<PauliTerm> &terms, const double *angles,
+                      bool negate_s, const std::vector<RotSweep> &sw, std::vector<RotArgs> *args_out,
+                      std::vector<RotTermDev> *ht_out) {
   const uint32_t L = std::min(kRotL, n);
   const uint64_t low = (1ull << L) - 1;
-  std::vector<RotArgs> args(sw.size());
-  std::vector<RotTermDev> ht(terms.size());
+  std::vector<RotArgs> &args = *args_out;
+  std::vector<RotTermDev> &ht = *ht_out;
+  args.assign(sw.size(), RotArgs());
+  ht.assign(terms.size(), RotTermDev());
   for (size_t k = 0; k < sw.size(); ++k) {
     const RotSweep &S = sw[k];
     RotArgs &a = args[k];
     memset(&a, 0, sizeof(a));
     std::vector<uint32_t> hi_pos;
-    for (uint32_t b = 0; b < n; ++b)
-      if ((S.hi >> b) & 1) hi_pos.push_back(b);
+    rot_geometry(n, L, S.hi, S.x_out, &a, &hi_pos);
     const uint64_t tile = low | S.hi;
-    a.x_out = S.x_out;
-    a.L = L;
-    a.tb = L + (uint32_t)hi_pos.size();
-    for (size_t i = 0; i < hi_pos.size(); ++i) a.hi_pos[i] = (uint8_t)hi_pos[i];
-    const int pair_bit = S.x_out ? __builtin_ctzll(S.x_out) : -1;
-    for (uint32_t b = 0; b < n; ++b)
-      if (!((tile >> b) & 1) && (int)b != pair_bit) a.out_pos[a.n_out++] = (uint8_t)b;
-    a.n_visits = 1ull << a.n_out;
     a.n_terms = S.end - S.first;
     uint64_t prev_key = ~0ull;  // ownership of the previous term: (x_in, pair), diagonal terms (0, 0)
     for (uint32_t t = S.first; t < S.end; ++t) {
@@ -380,17 +295,17 @@ cudaError_t run_pauli_rotations(qip_prec prec, void *psi, uint32_t n, const std:
       RotTermDev &d = ht[t];
       memset(&d, 0, sizeof(d));
       const uint64_t xo = P.x & ~tile;
-      if (xo != 0 && xo != S.x_out) return cudaErrorInvalidValue;  // the planner's invariant
+      if (xo != 0 && xo != S.x_out) return false;  // the planner's invariant
       d.z_out = P.z & ~tile;
-      d.x_in = compact(P.x & tile, L, hi_pos);
-      d.z_in = compact(P.z & tile, L, hi_pos);
+      d.x_in = compact_tile_bits(P.x & tile, L, hi_pos);
+      d.z_in = compact_tile_bits(P.z & tile, L, hi_pos);
       double c = cos(angles[t] / 2), sn = sin(angles[t] / 2);
       if (prec == QIP_F32) {
         c = (double)(float)c;
         sn = (double)(float)sn;
       }
       d.c = c;
-      d.s = sn;
+      d.s = negate_s ? -sn : sn;
       d.flags = (P.n_y + 3) & kRotPhase;  // w = -i * i^nY * sign * psi_partner
       if (P.x == 0) {
         d.flags |= kRotDiag;
@@ -415,6 +330,23 @@ cudaError_t run_pauli_rotations(qip_prec prec, void *psi, uint32_t n, const std:
       t = e;
     }
   }
+  return true;
+}
+
+uint32_t pauli_rotation_sweep_count(uint32_t n, const std::vector<PauliTerm> &terms) {
+  std::vector<RotSweep> sw;
+  plan_rot_sweeps(n, kRotM, terms, &sw);
+  return (uint32_t)sw.size();
+}
+
+cudaError_t run_pauli_rotations(qip_prec prec, void *psi, uint32_t n, const std::vector<PauliTerm> &terms,
+                                const double *angles, int grid, cudaStream_t s, uint64_t *launches) {
+  if (terms.empty()) return cudaSuccess;
+  std::vector<RotSweep> sw;
+  plan_rot_sweeps(n, kRotM, terms, &sw);
+  std::vector<RotArgs> args;
+  std::vector<RotTermDev> ht;
+  if (!build_rot_tables(prec, n, terms, angles, false, sw, &args, &ht)) return cudaErrorInvalidValue;
   RotTermDev *d = nullptr;
   cudaError_t e = cudaMallocAsync((void **)&d, ht.size() * sizeof(RotTermDev), s);
   if (e != cudaSuccess) return e;

@@ -305,6 +305,47 @@ class State:
         self._chk(_lib.lib().qipb200_state_apply_pauli_rotations(self._h, _ptr(qs), ls, _ptr(lens), lens.shape[0],
                                                                  _ptr(a) if a.shape[0] else None))
 
+    def apply_pauli_sum(self, src: "State", terms, coeffs):
+        """Set this state to H|src> for H = sum_h coeffs[h] P_h, a real Pauli sum, on the device (out of place).
+
+        Terms are encoded as for ``expect_paulis``; an empty term is the identity, and no terms give zero.  ``src``
+        must be another state of the same context, precision and size; its pending collapse is applied first and
+        this state takes its qubit layout.  Deterministic; stream-ordered like ``apply_schedule``
+        (``pauli_sum_plan`` gives the sweep count).  For example ``w.apply_pauli_sum(st, H, c)`` then ``w.norm2()``
+        is <psi|H^2|psi>."""
+        c = np.ascontiguousarray(np.asarray(coeffs, dtype=np.float64).reshape(-1))
+        terms = list(terms)
+        if c.shape[0] != len(terms):
+            raise ValueError("apply_pauli_sum: %d terms but %d coefficients" % (len(terms), c.shape[0]))
+        qs, ls, lens = _marshal_paulis(terms)
+        self._chk(_lib.lib().qipb200_state_apply_pauli_sum(self._h, src._h, _ptr(qs), ls, _ptr(lens), lens.shape[0],
+                                                           _ptr(c) if c.shape[0] else None))
+
+    def energy_gradient(self, work: "State", ansatz, angles, hamiltonian, coeffs):
+        """Energy and gradient of E(angles) = <psi0|U^dagger H U|psi0> by the adjoint method, on the device.
+
+        This state holds psi0 on entry; U applies exp(-i angles[t]/2 P_t) for the ``ansatz`` strings, term 0 first
+        (as ``apply_pauli_rotations``), and H = sum_h coeffs[h] Q_h (as ``apply_pauli_sum``).  Returns (E, g) with
+        g[t] = dE/dangles[t]; a parameter shared by several strings has the sum of their entries as its derivative.
+        ``work`` is scratch of the same size and precision: it ends holding U^dagger H U psi0.  This state ends at
+        psi0 up to rounding (run forward and back); re-prepare psi0 when it is needed exactly.  Deterministic;
+        synchronises (``pauli_gradient_plan`` gives the sweep counts)."""
+        a = np.ascontiguousarray(np.asarray(angles, dtype=np.float64).reshape(-1))
+        c = np.ascontiguousarray(np.asarray(coeffs, dtype=np.float64).reshape(-1))
+        ansatz, hamiltonian = list(ansatz), list(hamiltonian)
+        if a.shape[0] != len(ansatz):
+            raise ValueError("energy_gradient: %d terms but %d angles" % (len(ansatz), a.shape[0]))
+        if c.shape[0] != len(hamiltonian):
+            raise ValueError("energy_gradient: %d Hamiltonian terms but %d coefficients" % (len(hamiltonian), c.shape[0]))
+        qs, ls, lens = _marshal_paulis(ansatz)
+        hq, hl, hlen = _marshal_paulis(hamiltonian)
+        energy = np.zeros(1, dtype=np.float64)
+        grad = np.zeros(max(1, len(ansatz)), dtype=np.float64)
+        self._chk(_lib.lib().qipb200_state_pauli_energy_gradient(
+            self._h, work._h, _ptr(qs), ls, _ptr(lens), lens.shape[0], _ptr(a) if a.shape[0] else None,
+            _ptr(hq), hl, _ptr(hlen), hlen.shape[0], _ptr(c) if c.shape[0] else None, _ptr(energy), _ptr(grad)))
+        return float(energy[0]), grad[: len(ansatz)]
+
     def reduced_density(self, qubits: Sequence[int]) -> np.ndarray:
         """Reduced density matrix of ``qubits`` (1 to 10 of them) on the state as it is (not renormalised), computed
         on the device: complex128 of shape (2^k, 2^k) with rho[a, b] = sum_r psi(r, a) conj(psi(r, b)).
@@ -383,6 +424,26 @@ def pauli_rotation_plan(n: int, dtype, terms) -> int:
     _lib.check(_lib.lib().qipb200_pauli_rotation_plan(prec_of(dtype), int(n), _ptr(qs), ls, _ptr(lens), lens.shape[0],
                                                       C.byref(v)), None)
     return int(v.value)
+
+
+def pauli_sum_plan(n: int, dtype, terms) -> int:
+    """Read-write sweeps State.apply_pauli_sum makes for these terms on an unsharded n-qubit state (needs no GPU)."""
+    qs, ls, lens = _marshal_paulis(terms)
+    v = C.c_uint32()
+    _lib.check(_lib.lib().qipb200_pauli_sum_plan(prec_of(dtype), int(n), _ptr(qs), ls, _ptr(lens), lens.shape[0],
+                                                 C.byref(v)), None)
+    return int(v.value)
+
+
+def pauli_gradient_plan(n: int, dtype, ansatz, hamiltonian):
+    """(forward, sum, backward) sweeps State.energy_gradient makes on an unsharded n-qubit state (needs no GPU); the
+    call launches forward + sum + 2 * backward kernels."""
+    qs, ls, lens = _marshal_paulis(ansatz)
+    hq, hl, hlen = _marshal_paulis(hamiltonian)
+    v = (C.c_uint32 * 3)()
+    _lib.check(_lib.lib().qipb200_pauli_gradient_plan(prec_of(dtype), int(n), _ptr(qs), ls, _ptr(lens), lens.shape[0],
+                                                      _ptr(hq), hl, _ptr(hlen), hlen.shape[0], v), None)
+    return int(v[0]), int(v[1]), int(v[2])
 
 
 def plan_exchanges(ops: Sequence[MatrixOp], n: int, world_size: int, dtype=np.complex128):
