@@ -351,6 +351,31 @@ int qipb200_state_pauli_energy_gradient(qipb200_state *state, qipb200_state *wor
  * in canonical layout.  Validates both term lists as the call does. */
 int qipb200_pauli_gradient_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms, const uint64_t *ham_qubits, const char *ham_paulis, const uint32_t *ham_term_len, size_t n_ham, uint32_t *out3);
 
+/* state <- exp(-i time H) state for a real Pauli sum H = sum_h coeffs[h] P_h, by a Chebyshev expansion (absent in the
+ * reference).  Terms are encoded and validated as for qipb200_state_apply_pauli_sum (same codes and messages).  The
+ * identity terms sum to a; the others give the half-width b = sum |coeffs[h]| >= |H - a|; with H~ = (H - a) / b,
+ *   exp(-iHt) = e^{-iat} sum_k (2 - delta_k0) (-i)^k J_k(bt) T_k(H~),
+ * cut at the smallest degree K >= 2 whose tail bound tau_K = 2 sum_(j > K) |J_j(bt)| is <= tol, so in exact arithmetic
+ * |result - exp(-iHt) state| <= tau_K |state|.  *degree = K and *tail = tau_K.  The recurrence T_(k+1) = 2 H~ T_k -
+ * T_(k-1) runs in work_a and work_b (scratch: their contents afterwards are unspecified) with one read-write sweep of
+ * the sum plan per kernel, and state accumulates the series; the arithmetic is fixed and its forward error bound is
+ * documented in rustqip_b200/csrc/gradient.cu, the coefficients in rustqip_b200/csrc/evolve.h.  time == 0 or
+ * n_terms == 0: a no-op (K = 0, no kernel).  b == 0 (identity terms only): the global phase e^{-iat}, exactly
+ * qipb200_state_apply_pauli_rotations of one empty term by the angle 2 RN(a time) (K = 0, one kernel).
+ * Errors, all before any device work (a refused call leaves the three states and a pending collapse as they were):
+ * a state passed twice, NULL or non-finite coeffs (n_terms > 0), a non-finite time, tol not in (0, 1) or NULL
+ * degree / tail give QIPB200_ERR_INVALID_ARG; states of different contexts, precisions or sizes
+ * QIPB200_ERR_SIZE_MISMATCH; sharded or multi-device states, and K > 65536 (split the time over several calls),
+ * QIPB200_ERR_UNSUPPORTED.  A collapse pending on state is applied first; ones pending on the work states are dropped,
+ * and they take the state's layout.  Stream-ordered (the host arrays are copied before it returns); launches
+ * K x sweeps kernels (qipb200_pauli_evolution_plan), plus one for a pending collapse. */
+int qipb200_state_evolve_pauli_sum(qipb200_state *state, qipb200_state *work_a, qipb200_state *work_b, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms, const double *coeffs, double time, double tol, uint32_t *degree, double *tail);
+/* Host-only (no GPU, ctx-free): the plan of the call above on an unsharded n-qubit state in canonical layout.
+ * out3 = {degree K, sweeps per step, kernels}, *tail = tau_K, and when coeffs_out is not NULL and coeffs_cap (in
+ * doubles) is at least 2 (K + 1), coeffs_out = C_0..C_K as (re, im) pairs, the series coefficients including
+ * e^{-iat} (C_0 = 1 for a no-op, e^{-iat} alone for identity-only H).  Validates as the call does. */
+int qipb200_pauli_evolution_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms, const double *coeffs, double time, double tol, uint32_t *out3, double *tail, double *coeffs_out, size_t coeffs_cap);
+
 /* ---- multi-GPU: the 2^n state sharded by its top log2(world) index bits,
  *      one process per GPU (absent in the reference; its only hook is the
  *      input_offset/output_offset slice model, matrix_ops.rs:74-89) -------------- */

@@ -326,6 +326,21 @@ class B200State {
                                                    coeffs.data(), &out.first, out.second.data()));
     return out;
   }
+  // this state <- exp(-i time H) this state for H = sum_h coeffs[h] P_h, by a Chebyshev series cut at the smallest
+  // degree K >= 2 whose tail bound is <= tol; work_a and work_b are scratch of the same context, precision and size.
+  // Returns (K, tail bound) (absent in the reference)
+  std::pair<uint32_t, double> evolve_pauli_sum(B200State &work_a, B200State &work_b,
+                                               const std::vector<std::vector<std::pair<char, uint64_t>>> &terms,
+                                               const std::vector<double> &coeffs, double time, double tol) {
+    if (coeffs.size() != terms.size())
+      throw CircuitError("evolve_pauli_sum: " + std::to_string(terms.size()) + " terms but " +
+                         std::to_string(coeffs.size()) + " coefficients");
+    Flat f(terms);
+    std::pair<uint32_t, double> out(0, 0.0);
+    ctx_.check(qipb200_state_evolve_pauli_sum(st_, work_a.st_, work_b.st_, f.q(), f.l(), f.lens.data(), terms.size(),
+                                              coeffs.data(), time, tol, &out.first, &out.second));
+    return out;
+  }
   // reduced density matrix of up to 10 qubits, row-major 2^k x 2^k; bit i of the row and column index is the value of
   // qubits[i], as in measure_probs (absent in the reference)
   std::vector<std::complex<double>> reduced_density(const std::vector<uint64_t> &qubits) {

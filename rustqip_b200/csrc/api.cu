@@ -22,6 +22,7 @@
 #include "expect.h"
 #include "kernels.cuh"
 #include "opcompile.h"
+#include "evolve.h"
 #include "gradient.h"
 #include "pauli_rot.h"
 #include "rdm.h"
@@ -2162,6 +2163,92 @@ extern "C" int qipb200_pauli_gradient_plan(qip_prec prec, uint32_t n_qubits, con
     out3[0] = pauli_rotation_sweep_count(n_qubits, ansatz);
     out3[1] = pauli_sum_sweep_count(n_qubits, ham);
     out3[2] = pauli_adjoint_sweep_count(n_qubits, ansatz);
+    return (int)QIPB200_OK;
+  });
+}
+
+// ===================================================================================
+// exp(-iHt) for a real Pauli sum by a Chebyshev expansion (evolve.h, gradient.cu)
+// ===================================================================================
+
+namespace {
+
+// The checks the evolution call and its plan share once the terms are parsed.
+int check_evolution_args(qipb200_ctx *ctx, const std::string &who, const double *coeffs, size_t n_terms, double time,
+                         double tol) {
+  int st = check_finite(ctx, coeffs, n_terms, who, "coefficient");
+  if (st != QIPB200_OK) return st;
+  if (!std::isfinite(time)) return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": time is not finite");
+  if (!(tol > 0.0 && tol < 1.0)) return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": tol must be in (0, 1)");
+  return QIPB200_OK;
+}
+
+}  // namespace
+
+extern "C" int qipb200_state_evolve_pauli_sum(qipb200_state *state, qipb200_state *work_a, qipb200_state *work_b,
+                                              const uint64_t *qubits, const char *paulis, const uint32_t *term_len,
+                                              size_t n_terms, const double *coeffs, double time, double tol,
+                                              uint32_t *degree, double *tail) {
+  const std::string who = "evolve_pauli_sum";
+  if (!state || !work_a || !work_b) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, who + ": NULL state");
+  return guarded(state->ctx, [&]() -> int {
+    // every check runs before any device work: a refused call leaves the three states (and a pending collapse) as
+    // they were
+    if (state == work_a || state == work_b || work_a == work_b)
+      return set_err(state->ctx, QIPB200_ERR_INVALID_ARG, who + ": the three states must differ");
+    int st = check_state_pair(work_a, state, who);
+    if (st == QIPB200_OK) st = check_state_pair(work_b, state, who);
+    if (st != QIPB200_OK) return st;
+    std::vector<PauliTerm> terms;
+    std::string err;
+    st = parse_pauli_terms(state->n, qubits, paulis, term_len, n_terms, &terms, &err);
+    if (st != QIPB200_OK) return set_err(state->ctx, st, err);
+    if ((st = check_evolution_args(state->ctx, who, coeffs, n_terms, time, tol)) != QIPB200_OK) return st;
+    if (!degree || !tail) return set_err(state->ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL degree or tail");
+    EvolutionPlan p;
+    if ((st = plan_evolution(terms, coeffs, time, tol, &p, &err)) != QIPB200_OK) return set_err(state->ctx, st, err);
+    *degree = p.degree;
+    *tail = p.tail;
+    if (p.kind == EvolutionPlan::kNoop) return (int)QIPB200_OK;
+    qipb200_ctx *ctx = state->ctx;
+    CU(ctx, cudaSetDevice(ctx->device));
+    if (p.kind == EvolutionPlan::kPhase) {  // e^{-iat}: the empty-term rotation by 2 RN(a t)
+      if ((st = materialise_collapse(state)) != QIPB200_OK) return st;
+      const double angle = 2.0 * (p.a * time);
+      CU(ctx, run_pauli_rotations(state->prec, state->buf, state->n_local, std::vector<PauliTerm>(1), &angle,
+                                  2 * ctx->sm_count, ctx->stream, &ctx->launches));
+      return (int)QIPB200_OK;
+    }
+    if ((st = prepare_out_of_place(work_a, state)) != QIPB200_OK) return st;
+    if ((st = prepare_out_of_place(work_b, state)) != QIPB200_OK) return st;
+    CU(ctx, run_pauli_evolution(state->prec, state->buf, work_a->buf, work_b->buf, state->n_local,
+                                phys_terms(state, p.terms), p.coeffs.data(), p.b, p.C, ctx->stream, &ctx->launches));
+    return (int)QIPB200_OK;
+  });
+}
+
+extern "C" int qipb200_pauli_evolution_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits,
+                                            const char *paulis, const uint32_t *term_len, size_t n_terms,
+                                            const double *coeffs, double time, double tol, uint32_t *out3,
+                                            double *tail, double *coeffs_out, size_t coeffs_cap) {
+  const std::string who = "pauli_evolution_plan";
+  if (!out3 || !tail || (prec != QIP_F32 && prec != QIP_F64) || n_qubits == 0 || n_qubits > 40)
+    return set_err(nullptr, QIPB200_ERR_INVALID_ARG,
+                   who + ": NULL out3 or tail, bad precision or n_qubits not in 1..40");
+  return guarded(nullptr, [&]() -> int {
+    std::vector<PauliTerm> terms;
+    std::string err;
+    int st = parse_pauli_terms(n_qubits, qubits, paulis, term_len, n_terms, &terms, &err);
+    if (st != QIPB200_OK) return set_err(nullptr, st, err);
+    if ((st = check_evolution_args(nullptr, who, coeffs, n_terms, time, tol)) != QIPB200_OK) return st;
+    EvolutionPlan p;
+    if ((st = plan_evolution(terms, coeffs, time, tol, &p, &err)) != QIPB200_OK) return set_err(nullptr, st, err);
+    const uint64_t s = p.kind == EvolutionPlan::kSeries ? pauli_sum_sweep_count(n_qubits, p.terms) : 0;
+    out3[0] = p.degree;
+    out3[1] = (uint32_t)s;
+    out3[2] = p.kind == EvolutionPlan::kPhase ? 1u : (uint32_t)std::min<uint64_t>(p.degree * s, UINT32_MAX);
+    *tail = p.tail;
+    if (coeffs_out && coeffs_cap >= p.C.size()) std::copy(p.C.begin(), p.C.end(), coeffs_out);
     return (int)QIPB200_OK;
   });
 }

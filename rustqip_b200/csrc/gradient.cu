@@ -22,6 +22,30 @@
 // |c_h| (|p.x| + |p.y|), plus one rounding to the state's precision per sweep).  A thread owns its four amplitudes of
 // each tile: src is read from shared memory only, so no barrier separates groups.
 //
+// k_pauli_sum, evolution mode (EVO = true; qipb200_state_evolve_pauli_sum, host plan in evolve.h).  Step k of the
+// Chebyshev recurrence T_1 = H~ S, T_k = 2 H~ T_(k-1) - T_(k-2) runs the s sweeps of plan_sum over the non-identity
+// terms with the coefficients RN(c_h / b) (step 1) or RN(c_h (2 / b)) (later steps) in place of c_h.  T_k is in
+// work_a for odd k, work_b for even k; src = T_(k-1) (S for k = 1) is the only operand read at partner indices and is
+// never written in the step, so no sweep has a read-after-write hazard.  Per amplitude, in double, no FMA:
+//   - the first sweep's acc starts at +0.0 (k = 1), at -S (k = 2) or at -T_(k-2) (k >= 3, read from dst, which it
+//     overwrites in place), an exact negation of the value widened to double; later sweeps start at the stored dst;
+//   - the groups add as above, and each sweep stores acc rounded to the state's precision;
+//   - the last sweep of step k >= 2 then updates S at the own index from the stored (rounded) t = T_k, with
+//     cmul(c, v) = (RN(RN(c.x v.x) - RN(c.y v.y)), RN(RN(c.x v.y) + RN(c.y v.x))) and RN additions:
+//       k = 2: S <- RN_prec((cmul(C_0, S) + cmul(C_1, T_1)) + cmul(C_2, t))   (T_1 = src at the own index)
+//       k > 2: S <- RN_prec(S + cmul(C_k, t)).
+// S and T_(k-2) are read before they are written, by the thread that owns the amplitude; T_(k-2) (the accumulator
+// start) is staged in the dst tiles, S is loaded straight into registers before the groups.  Emulated bit for bit in
+// tests/evolve_ref.py.  Forward error in 2-norm, to first order, for |psi| = |S| on entry: with
+//   delta = 2 (gamma_(T+G+4)(2^-53) + gamma_s(u))   (T non-identity terms, G groups, s sweeps; the extra operations are
+// the start value and the rounding of RN(c_h / b)), step k adds a local error e_k with |e_1| <= delta |psi| and
+// |e_k| <= 3 delta |psi| (|A| <= sum_h |2 c_h / b| |T| = 2 |T|, plus |T_(k-2)|).  The error of T_k is
+// sum_(m <= k) U_(k-m)(H~) e_m, and |U_j(H~)| <= j + 1 (Chebyshev polynomials of the second kind), so it is at most
+// 3 delta k (k + 1) / 2 |psi|: quadratic in k.  With C = sum_k |C_k| (|S| <= C |psi| after any step),
+//   |S_device - sum_k C_k T_k(H~) psi| <= [3 delta sum_k |C_k| k (k + 1) / 2 + sqrt(2) (2 gamma_4(2^-53) + u) K C]
+//                                        x (1 + 3 delta K (K + 1) / 2) |psi|,
+// the second term for the K accumulations into S.  tests/evolve_ref.py: bound().
+//
 // k_pauli_adjoint.  The backward pass runs over the sweeps of the reversed term list (gradient.h) with the descriptors
 // of pauli_rot.cu for c and -s: R_t^dagger = exp(+i theta_t/2 P_t) is exactly the rotation update of pauli_rot.cu with
 // s negated, so phi (= state) and lambda (= work) go back bit for bit as the emulator says.  Per term, on the pairs
@@ -72,21 +96,43 @@ struct SumTermDev {
   double c;        // c_h times the sign of Re / Im of i^nY
 };
 
+// One sweep of a Chebyshev step (k_pauli_sum<R, PAIR, true>), see "k_pauli_sum, evolution mode" above.
+struct EvoSweep {
+  const void *from;  // the accumulator starts at -from (negate) or +from at the own index; NULL: at +0.0
+  void *state;       // S, updated at the own index after the store when update != 0
+  uint32_t negate;
+  uint32_t update;   // 0: none; 1: S <- c0 S + c1 src + c2 dst (step 2); 2: S <- S + c2 dst (steps >= 3)
+  double2 c0, c1, c2;
+};
+
 __device__ __forceinline__ double2 widen(float2 v) { return make_double2(v.x, v.y); }
 __device__ __forceinline__ double2 widen(double2 v) { return v; }
 __device__ __forceinline__ void narrow(double2 a, float2 *o) { *o = make_float2((float)a.x, (float)a.y); }
 __device__ __forceinline__ void narrow(double2 a, double2 *o) { *o = a; }
 
-template <typename R, bool PAIR>
+// c v and a + v, complex, in double with every product and sum rounded (no FMA)
+__device__ __forceinline__ double2 cmul_rn(double2 c, double2 v) {
+  return make_double2(__dadd_rn(__dmul_rn(c.x, v.x), -__dmul_rn(c.y, v.y)),
+                      __dadd_rn(__dmul_rn(c.x, v.y), __dmul_rn(c.y, v.x)));
+}
+__device__ __forceinline__ double2 cadd_rn(double2 a, double2 v) {
+  return make_double2(__dadd_rn(a.x, v.x), __dadd_rn(a.y, v.y));
+}
+
+template <typename R, bool PAIR, bool EVO>
 __global__ void __launch_bounds__(kGradThreads, 2)
     k_pauli_sum(R *__restrict__ dst, const R *__restrict__ src, const __grid_constant__ RotArgs a,
-                const SumGroupDev *__restrict__ groups, const SumTermDev *__restrict__ terms, uint32_t accumulate) {
+                const SumGroupDev *__restrict__ groups, const SumTermDev *__restrict__ terms, uint32_t accumulate,
+                const __grid_constant__ EvoSweep ev) {
   typedef typename RotV<R>::type V;
   extern __shared__ __align__(16) unsigned char smem[];
-  // single tiles: [buffer][src, dst] double-buffered; pairs: src A, src B, dst A, dst B
+  // single tiles: [buffer][src, from] double-buffered; pairs: src A, src B, from A, from B
   V *tiles = reinterpret_cast<V *>(smem);
   const int t = threadIdx.x;
   const uint32_t tsize = 1u << a.tb;
+  // where the accumulator starts: the stored partial (dst) or, in the first sweep of a Chebyshev step, T_(k-1)
+  const R *from = EVO ? (const R *)ev.from : dst;
+  const bool load = EVO ? ev.from != nullptr : accumulate != 0;
   uint64_t off[kGradPer];
 #pragma unroll
   for (int k = 0; k < kGradPer; ++k) {
@@ -107,10 +153,10 @@ __global__ void __launch_bounds__(kGradThreads, 2)
       const uint32_t e = t + kGradThreads * k;
       if (e >= tsize) continue;
       cp_async<sizeof(V)>(S + e, src + 2 * (b | off[k]));
-      if (accumulate) cp_async<sizeof(V)>(D + e, dst + 2 * (b | off[k]));
+      if (load) cp_async<sizeof(V)>(D + e, from + 2 * (b | off[k]));
       if (PAIR) {
         cp_async<sizeof(V)>(S2 + e, src + 2 * ((b ^ a.x_out) | off[k]));
-        if (accumulate) cp_async<sizeof(V)>(D2 + e, dst + 2 * ((b ^ a.x_out) | off[k]));
+        if (load) cp_async<sizeof(V)>(D2 + e, from + 2 * ((b ^ a.x_out) | off[k]));
       }
     }
   };
@@ -148,11 +194,15 @@ __global__ void __launch_bounds__(kGradThreads, 2)
       const V *D = side ? dB : dA;
       const uint64_t b = side ? bB : bA, bo = side ? bA : bB;
       double2 acc[kGradPer];
+      V sv[kGradPer];  // S at the own index, loaded before the groups for the update after the store
 #pragma unroll
       for (int k = 0; k < kGradPer; ++k) {
         const uint32_t e = t + kGradThreads * k;
         acc[k] = make_double2(0.0, 0.0);
-        if (accumulate && e < tsize) acc[k] = widen(D[e]);
+        if (load && e < tsize) acc[k] = widen(D[e]);
+        if (EVO && ev.negate) acc[k] = make_double2(-acc[k].x, -acc[k].y);
+        if (EVO && ev.update && e < tsize)
+          sv[k] = *reinterpret_cast<const V *>((const R *)ev.state + 2 * (b | off[k]));
       }
       for (uint32_t g = 0; g < a.n_terms; ++g) {
         const SumGroupDev G = groups[g];
@@ -190,6 +240,15 @@ __global__ void __launch_bounds__(kGradThreads, 2)
         const uint32_t e = t + kGradThreads * k;
         if (e >= tsize) continue;
         narrow(acc[k], reinterpret_cast<V *>(dst + 2 * (b | off[k])));
+        if (EVO && ev.update) {
+          V o;
+          narrow(acc[k], &o);
+          const double2 sk = widen(sv[k]), tk = widen(o);
+          const double2 r = ev.update == 1 ? cadd_rn(cadd_rn(cmul_rn(ev.c0, sk), cmul_rn(ev.c1, widen(own[e]))),
+                                                     cmul_rn(ev.c2, tk))
+                                           : cadd_rn(sk, cmul_rn(ev.c2, tk));
+          narrow(r, reinterpret_cast<V *>((R *)ev.state + 2 * (b | off[k])));
+        }
       }
     }
     __syncthreads();  // every thread has read this buffer before the next cp.async writes it
@@ -488,17 +547,77 @@ void plan_adjoint(uint32_t n, const std::vector<PauliTerm> &rev, std::vector<Rot
     }
 }
 
-template <typename R, bool PAIR>
+template <typename R, bool PAIR, bool EVO>
 cudaError_t launch_sum(void *dst, const void *src, const RotArgs &a, const SumGroupDev *g, const SumTermDev *t,
-                       uint32_t accumulate, cudaStream_t s) {
+                       uint32_t accumulate, const EvoSweep &ev, cudaStream_t s) {
   typedef typename RotV<R>::type V;
   static_assert(4 * kGradTile * sizeof(double2) <= 113 * 1024, "two CTAs per SM: at most 113 KiB of shared memory each");
   const size_t smem = 4 * kGradTile * sizeof(V);
-  cudaError_t e = cudaFuncSetAttribute(k_pauli_sum<R, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  cudaError_t e =
+      cudaFuncSetAttribute(k_pauli_sum<R, PAIR, EVO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
   const int grid = (int)std::min<uint64_t>(a.n_visits, (uint64_t)kAdjGrid);
-  k_pauli_sum<R, PAIR><<<grid, kGradThreads, smem, s>>>((R *)dst, (const R *)src, a, g, t, accumulate);
+  k_pauli_sum<R, PAIR, EVO><<<grid, kGradThreads, smem, s>>>((R *)dst, (const R *)src, a, g, t, accumulate, ev);
   return cudaGetLastError();
+}
+
+template <bool EVO>
+cudaError_t launch_sum_any(qip_prec prec, void *dst, const void *src, const RotArgs &a, const SumGroupDev *g,
+                           const SumTermDev *t, uint32_t accumulate, const EvoSweep &ev, cudaStream_t s) {
+  if (prec == QIP_F32)
+    return a.x_out ? launch_sum<float, true, EVO>(dst, src, a, g, t, accumulate, ev, s)
+                   : launch_sum<float, false, EVO>(dst, src, a, g, t, accumulate, ev, s);
+  return a.x_out ? launch_sum<double, true, EVO>(dst, src, a, g, t, accumulate, ev, s)
+                 : launch_sum<double, false, EVO>(dst, src, a, g, t, accumulate, ev, s);
+}
+
+// The device tables of plan_sum: args[k] (n_terms = its group count) and the groups of sweep k from (*hg)[(*g_off)[k]]
+// for every sweep, and the terms they index, with c = RN(scale coeffs[h]) times the sign of Re / Im of i^nY.  False
+// when a group breaks the planner's invariant (a different out-of-tile mask).
+bool build_sum_tables(uint32_t n, const std::vector<PauliTerm> &terms, const double *coeffs, double scale,
+                      std::vector<RotArgs> *args, std::vector<SumGroupDev> *hg, std::vector<SumTermDev> *ht,
+                      std::vector<size_t> *g_off) {
+  std::vector<SumGroup> gr;
+  std::vector<SumSweep> sw;
+  plan_sum(n, terms, &gr, &sw);
+  const uint32_t L = std::min(kRotL, n);
+  const uint64_t low = (1ull << L) - 1;
+  args->assign(sw.size(), RotArgs());
+  g_off->assign(sw.size(), 0);
+  hg->clear();
+  ht->clear();
+  for (size_t k = 0; k < sw.size(); ++k) {
+    const SumSweep &S = sw[k];
+    RotArgs &a = (*args)[k];
+    memset(&a, 0, sizeof(a));
+    std::vector<uint32_t> hi_pos;
+    rot_geometry(n, L, S.geo.hi, S.geo.x_out, &a, &hi_pos);
+    const uint64_t tile = low | S.geo.hi;
+    a.n_terms = (uint32_t)S.groups.size();  // groups, for this kernel
+    (*g_off)[k] = hg->size();
+    for (uint32_t gi : S.groups) {
+      const SumGroup &G = gr[gi];
+      const uint64_t xo = G.x & ~tile;
+      if (xo != 0 && xo != S.geo.x_out) return false;
+      SumGroupDev gd;
+      gd.x_in = compact_tile_bits(G.x & tile, L, hi_pos);
+      gd.pair = xo ? 1u : 0u;
+      gd.first = (uint32_t)ht->size();
+      for (uint32_t t : G.terms) {
+        const PauliTerm &P = terms[t];
+        SumTermDev td;
+        td.z_out = P.z & ~tile;
+        td.z_in = compact_tile_bits(P.z & tile, L, hi_pos);
+        td.odd = P.n_y & 1;
+        const double c = scale * coeffs[t];
+        td.c = ((P.n_y & 3) >= 2) ? -c : c;  // i^nY = 1, i, -1, -i
+        ht->push_back(td);
+      }
+      gd.end = (uint32_t)ht->size();
+      hg->push_back(gd);
+    }
+  }
+  return true;
 }
 
 template <typename R, bool PAIR>
@@ -538,45 +657,11 @@ cudaError_t run_pauli_sum(qip_prec prec, void *dst, const void *src, uint32_t n,
                           const double *coeffs, cudaStream_t s, uint64_t *launches) {
   const size_t amp_bytes = (prec == QIP_F32 ? 2 * sizeof(float) : 2 * sizeof(double)) << n;
   if (terms.empty()) return cudaMemsetAsync(dst, 0, amp_bytes, s);  // the empty sum
-  std::vector<SumGroup> gr;
-  std::vector<SumSweep> sw;
-  plan_sum(n, terms, &gr, &sw);
-  const uint32_t L = std::min(kRotL, n);
-  const uint64_t low = (1ull << L) - 1;
-  std::vector<RotArgs> args(sw.size());
+  std::vector<RotArgs> args;
   std::vector<SumGroupDev> hg;
   std::vector<SumTermDev> ht;
-  std::vector<size_t> g_off(sw.size());
-  for (size_t k = 0; k < sw.size(); ++k) {
-    const SumSweep &S = sw[k];
-    RotArgs &a = args[k];
-    memset(&a, 0, sizeof(a));
-    std::vector<uint32_t> hi_pos;
-    rot_geometry(n, L, S.geo.hi, S.geo.x_out, &a, &hi_pos);
-    const uint64_t tile = low | S.geo.hi;
-    a.n_terms = (uint32_t)S.groups.size();  // groups, for this kernel
-    g_off[k] = hg.size();
-    for (uint32_t gi : S.groups) {
-      const SumGroup &G = gr[gi];
-      const uint64_t xo = G.x & ~tile;
-      if (xo != 0 && xo != S.geo.x_out) return cudaErrorInvalidValue;  // the planner's invariant
-      SumGroupDev gd;
-      gd.x_in = compact_tile_bits(G.x & tile, L, hi_pos);
-      gd.pair = xo ? 1u : 0u;
-      gd.first = (uint32_t)ht.size();
-      for (uint32_t t : G.terms) {
-        const PauliTerm &P = terms[t];
-        SumTermDev td;
-        td.z_out = P.z & ~tile;
-        td.z_in = compact_tile_bits(P.z & tile, L, hi_pos);
-        td.odd = P.n_y & 1;
-        td.c = ((P.n_y & 3) >= 2) ? -coeffs[t] : coeffs[t];  // i^nY = 1, i, -1, -i
-        ht.push_back(td);
-      }
-      gd.end = (uint32_t)ht.size();
-      hg.push_back(gd);
-    }
-  }
+  std::vector<size_t> g_off;
+  if (!build_sum_tables(n, terms, coeffs, 1.0, &args, &hg, &ht, &g_off)) return cudaErrorInvalidValue;
   const size_t gbytes = hg.size() * sizeof(SumGroupDev), tbytes = ht.size() * sizeof(SumTermDev);
   char *d = nullptr;
   cudaError_t e = cudaMallocAsync((void **)&d, tbytes + gbytes, s);
@@ -586,16 +671,54 @@ cudaError_t run_pauli_sum(qip_prec prec, void *dst, const void *src, uint32_t n,
   // pageable sources: the copies are staged before cudaMemcpyAsync returns
   e = cudaMemcpyAsync(dt, ht.data(), tbytes, cudaMemcpyHostToDevice, s);
   if (e == cudaSuccess) e = cudaMemcpyAsync(dg, hg.data(), gbytes, cudaMemcpyHostToDevice, s);
-  for (size_t k = 0; k < sw.size() && e == cudaSuccess; ++k) {
-    const uint32_t acc = k > 0;
-    const SumGroupDev *g = dg + g_off[k];
-    if (prec == QIP_F32)
-      e = args[k].x_out ? launch_sum<float, true>(dst, src, args[k], g, dt, acc, s)
-                        : launch_sum<float, false>(dst, src, args[k], g, dt, acc, s);
-    else
-      e = args[k].x_out ? launch_sum<double, true>(dst, src, args[k], g, dt, acc, s)
-                        : launch_sum<double, false>(dst, src, args[k], g, dt, acc, s);
+  const EvoSweep none = {};
+  for (size_t k = 0; k < args.size() && e == cudaSuccess; ++k) {
+    e = launch_sum_any<false>(prec, dst, src, args[k], dg + g_off[k], dt, k > 0, none, s);
     ++*launches;
+  }
+  const cudaError_t ef = cudaFreeAsync(d, s);
+  return e != cudaSuccess ? e : ef;
+}
+
+cudaError_t run_pauli_evolution(qip_prec prec, void *state, void *work_a, void *work_b, uint32_t n,
+                                const std::vector<PauliTerm> &terms, const double *coeffs, double half_width,
+                                const std::vector<double> &C, cudaStream_t s, uint64_t *launches) {
+  const uint32_t K = (uint32_t)(C.size() / 2) - 1;
+  if (terms.empty() || K < 2) return cudaErrorInvalidValue;
+  // H~ = (H - a) / b: step 1 applies it with coefficients RN(c_h / b), later steps 2 H~ with RN(c_h (2 / b))
+  std::vector<RotArgs> args, args2;
+  std::vector<SumGroupDev> hg, hg2;
+  std::vector<SumTermDev> h1, h2;
+  std::vector<size_t> g_off, g_off2;
+  if (!build_sum_tables(n, terms, coeffs, 1.0 / half_width, &args, &hg, &h1, &g_off) ||
+      !build_sum_tables(n, terms, coeffs, 2.0 / half_width, &args2, &hg2, &h2, &g_off2))
+    return cudaErrorInvalidValue;
+  const size_t gbytes = hg.size() * sizeof(SumGroupDev), tbytes = h1.size() * sizeof(SumTermDev);
+  char *d = nullptr;
+  cudaError_t e = cudaMallocAsync((void **)&d, 2 * tbytes + gbytes, s);
+  if (e != cudaSuccess) return e;
+  SumTermDev *dt1 = (SumTermDev *)d, *dt2 = (SumTermDev *)(d + tbytes);
+  SumGroupDev *dg = (SumGroupDev *)(d + 2 * tbytes);
+  e = cudaMemcpyAsync(dt1, h1.data(), tbytes, cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(dt2, h2.data(), tbytes, cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(dg, hg.data(), gbytes, cudaMemcpyHostToDevice, s);
+  const uint32_t S = (uint32_t)args.size();
+  EvoSweep ev = {};
+  ev.state = state;
+  ev.c0 = make_double2(C[0], C[1]);
+  ev.c1 = make_double2(C[2], C[3]);
+  // T_k lives in work_a for odd k and in work_b for even k; step k >= 3 overwrites T_(k-2) in place
+  for (uint32_t k = 1; k <= K && e == cudaSuccess; ++k) {
+    void *dst = (k & 1) ? work_a : work_b;
+    const void *src = k == 1 ? state : (k & 1) ? work_b : work_a;
+    ev.c2 = make_double2(C[2 * k], C[2 * k + 1]);
+    for (uint32_t j = 0; j < S && e == cudaSuccess; ++j) {
+      ev.from = j > 0 ? dst : k == 1 ? nullptr : k == 2 ? state : dst;
+      ev.negate = j == 0 && k >= 2;
+      ev.update = j + 1 < S ? 0u : k == 1 ? 0u : k == 2 ? 1u : 2u;
+      e = launch_sum_any<true>(prec, dst, src, args[j], dg + g_off[j], k == 1 ? dt1 : dt2, 0, ev, s);
+      ++*launches;
+    }
   }
   const cudaError_t ef = cudaFreeAsync(d, s);
   return e != cudaSuccess ? e : ef;

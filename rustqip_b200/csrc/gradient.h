@@ -35,6 +35,15 @@ uint32_t pauli_adjoint_sweep_count(uint32_t n, const std::vector<PauliTerm> &ans
 cudaError_t run_pauli_sum(qip_prec prec, void *dst, const void *src, uint32_t n, const std::vector<PauliTerm> &terms,
                           const double *coeffs, cudaStream_t s, uint64_t *launches);
 
+// The Chebyshev series of qipb200_state_evolve_pauli_sum (evolve.h): steps k = 1..K of the recurrence over the
+// non-identity `terms` (masks on physical index bits) and their coefficients, with H~ = (H - a) / half_width, each step
+// one kernel per sweep of the sum plan; state <- sum_k C_k T_k(H~) state for C = C_0..C_K (re, im), K >= 2.  work_a
+// and work_b are scratch of the state's size and precision (their contents afterwards are unspecified).  Launches K x
+// sweeps kernels, stream-ordered.
+cudaError_t run_pauli_evolution(qip_prec prec, void *state, void *work_a, void *work_b, uint32_t n,
+                                const std::vector<PauliTerm> &terms, const double *coeffs, double half_width,
+                                const std::vector<double> &C, cudaStream_t s, uint64_t *launches);
+
 // The adjoint gradient: state <- U state (run_pauli_rotations), work <- H state (run_pauli_sum), then the backward
 // sweeps, each one adjoint kernel and one reduction kernel.  Launches forward + sum + 2 backward sweeps.  Writes
 // *energy and grad[0..T); synchronises the stream.  grid: CTAs per forward sweep.

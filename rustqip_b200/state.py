@@ -346,6 +346,28 @@ class State:
             _ptr(hq), hl, _ptr(hlen), hlen.shape[0], _ptr(c) if c.shape[0] else None, _ptr(energy), _ptr(grad)))
         return float(energy[0]), grad[: len(ansatz)]
 
+    def evolve_pauli_sum(self, work_a: "State", work_b: "State", terms, coeffs, time: float, tol=None):
+        """Set this state to exp(-i time H)|psi> for H = sum_h coeffs[h] P_h, a real Pauli sum, on the device.
+
+        Terms are encoded as for ``apply_pauli_sum``.  A Chebyshev series in H~ = (H - a) / b (a: the identity terms'
+        sum, b = sum |coeffs| of the others) is cut at the smallest degree K >= 2 whose tail bound tau_K is <= tol
+        (default 1e-12 for complex128, 1e-6 for complex64); in exact arithmetic the result is then within
+        tau_K |psi| of exp(-iHt)|psi>.  Returns (K, tau_K).  ``work_a`` and ``work_b`` are two more states of the same
+        context, precision and size, used as scratch (their contents afterwards are unspecified).  Each of the K
+        steps is one read-write sweep per sweep of ``pauli_sum_plan`` of the non-identity terms
+        (``pauli_evolution_plan`` gives the counts); deterministic and stream-ordered.  K above 65536 is refused:
+        split the time over several calls."""
+        c = np.ascontiguousarray(np.asarray(coeffs, dtype=np.float64).reshape(-1))
+        terms = list(terms)
+        if c.shape[0] != len(terms):
+            raise ValueError("evolve_pauli_sum: %d terms but %d coefficients" % (len(terms), c.shape[0]))
+        qs, ls, lens = _marshal_paulis(terms)
+        degree, tail = C.c_uint32(), C.c_double()
+        self._chk(_lib.lib().qipb200_state_evolve_pauli_sum(
+            self._h, work_a._h, work_b._h, _ptr(qs), ls, _ptr(lens), lens.shape[0], _ptr(c) if c.shape[0] else None,
+            float(time), float(_default_tol(self.dtype) if tol is None else tol), C.byref(degree), C.byref(tail)))
+        return int(degree.value), float(tail.value)
+
     def reduced_density(self, qubits: Sequence[int]) -> np.ndarray:
         """Reduced density matrix of ``qubits`` (1 to 10 of them) on the state as it is (not renormalised), computed
         on the device: complex128 of shape (2^k, 2^k) with rho[a, b] = sum_r psi(r, a) conj(psi(r, b)).
@@ -444,6 +466,32 @@ def pauli_gradient_plan(n: int, dtype, ansatz, hamiltonian):
     _lib.check(_lib.lib().qipb200_pauli_gradient_plan(prec_of(dtype), int(n), _ptr(qs), ls, _ptr(lens), lens.shape[0],
                                                       _ptr(hq), hl, _ptr(hlen), hlen.shape[0], v), None)
     return int(v[0]), int(v[1]), int(v[2])
+
+
+def _default_tol(dtype):
+    return 1e-12 if np.dtype(cdtype(prec_of(dtype))) == np.complex128 else 1e-6
+
+
+def pauli_evolution_plan(n: int, dtype, terms, coeffs, time: float, tol=None):
+    """(degree, sweeps per step, kernels, tail, C) of State.evolve_pauli_sum on an unsharded n-qubit state (needs no
+    GPU): C[k] (complex128, K + 1 of them) are the series coefficients (2 - delta_k0) (-i)^k J_k(bt) e^{-iat}."""
+    c = np.ascontiguousarray(np.asarray(coeffs, dtype=np.float64).reshape(-1))
+    terms = list(terms)
+    if c.shape[0] != len(terms):
+        raise ValueError("pauli_evolution_plan: %d terms but %d coefficients" % (len(terms), c.shape[0]))
+    qs, ls, lens = _marshal_paulis(terms)
+    tol = float(_default_tol(dtype) if tol is None else tol)
+    v, tail = (C.c_uint32 * 3)(), C.c_double()
+
+    def call(out, cap):
+        _lib.check(_lib.lib().qipb200_pauli_evolution_plan(
+            prec_of(dtype), int(n), _ptr(qs), ls, _ptr(lens), lens.shape[0], _ptr(c) if c.shape[0] else None,
+            float(time), tol, v, C.byref(tail), out, cap), None)
+
+    call(None, 0)
+    out = np.zeros(2 * (int(v[0]) + 1), dtype=np.float64)
+    call(_ptr(out), out.shape[0])
+    return int(v[0]), int(v[1]), int(v[2]), float(tail.value), out.view(np.complex128)
 
 
 def plan_exchanges(ops: Sequence[MatrixOp], n: int, world_size: int, dtype=np.complex128):
