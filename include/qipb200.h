@@ -376,6 +376,45 @@ int qipb200_state_evolve_pauli_sum(qipb200_state *state, qipb200_state *work_a, 
  * e^{-iat} (C_0 = 1 for a no-op, e^{-iat} alone for identity-only H).  Validates as the call does. */
 int qipb200_pauli_evolution_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms, const double *coeffs, double time, double tol, uint32_t *out3, double *tail, double *coeffs_out, size_t coeffs_cap);
 
+/* The lowest eigenvalue of a real Pauli sum H = sum_h coeffs[h] P_h reachable from the start state, by plain Lanczos
+ * (no reorthogonalisation) on the device (absent in the reference).  Terms are encoded and validated as for
+ * qipb200_state_apply_pauli_sum (same codes and messages).  The identity terms sum to a; the others give the scale
+ * b = sum |coeffs[h]|.  From v_0 = state / |state| step j forms alpha_j = <v_j|H v_j> and beta_(j+1) =
+ * |H v_j - alpha_j v_j - beta_j v_(j-1)|; after m steps the host takes the lowest eigenvalue theta of the tridiagonal
+ * T_m and its unit eigenvector y (qipb200_lanczos_ritz) and stops at the first m with the estimate
+ * rho_m = beta_m |y_(m-1)| <= tol b (*converged = 1; a breakdown, beta_m = 0, counts), else at max_steps
+ * (*converged = 0, the best estimate returned).  Only the part of H's spectrum the state has weight on is reachable: a
+ * start state in a symmetry sector (fixed S_z, parity, ...) gives that sector's ground state.  *steps = m;
+ * alpha[0..m) and beta[0..m] (beta[0] = |state|) are written when not NULL (room for max_steps and max_steps + 1).
+ * flags 0 (energy only): the state is read and not written; out3 = {theta, rho_m, 0}.  QIPB200_LANCZOS_VECTOR: a
+ * second pass reruns the recurrence with the same scalars (so the same bits) and accumulates x = sum_j y_j v_j into
+ * the state, which ends as x / |x|; out3 = {E, |H x - E x|, |x| before normalisation}, E = <x|H x>, both computed on
+ * the device after the pass (|x| far from 1 shows loss of orthogonality).  In exact arithmetic some eigenvalue of H
+ * lies within out3[1] of out3[0] in both modes.  The arithmetic, its order and the rounding bounds of alpha and beta
+ * are documented in rustqip_b200/csrc/lanczos.cu; the same inputs give the same bits.  work_a and work_b are scratch
+ * (their contents afterwards are unspecified).  b == 0 (no terms, or identity terms only): every vector is an
+ * eigenvector: out3 = {a, 0, 1 or 0}, *steps = 0, *converged = 1, and vector mode normalises the state.
+ * Errors: a state passed twice, NULL or non-finite coeffs (n_terms > 0), max_steps 0 or above 4096, tol not in
+ * (0, 1), unknown flags or NULL steps / converged / out3 give QIPB200_ERR_INVALID_ARG; states of different contexts,
+ * precisions or sizes QIPB200_ERR_SIZE_MISMATCH; sharded or multi-device states QIPB200_ERR_UNSUPPORTED; all before
+ * any device work (a refused call leaves the three states and a pending collapse as they were).  A start state of zero
+ * (or non-finite) norm gives QIPB200_ERR_INVALID_ARG after the first read sweep, the state unchanged.  A collapse
+ * pending on state is applied first; ones pending on the work states are dropped, and they take the state's layout.
+ * Synchronises once per first-pass step.  With {s, k1, k2, k0} = qipb200_pauli_lanczos_plan it launches 1 + m k1
+ * kernels (energy only) or m k1 + (m - 1) k2 + k0 (vector mode), plus one for a pending collapse; b == 0 launches 1
+ * (2 in vector mode). */
+enum { QIPB200_LANCZOS_VECTOR = 1u };
+int qipb200_state_lanczos_pauli_sum(qipb200_state *state, qipb200_state *work_a, qipb200_state *work_b, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms, const double *coeffs, uint32_t max_steps, double tol, uint32_t flags, uint32_t *steps, uint32_t *converged, double *alpha, double *beta, double *out3);
+/* Host-only (no GPU, ctx-free): out4 = {sum sweeps per step, kernels per first-pass step, kernels per second-pass step,
+ * kernels outside the steps in vector mode} of the call above on an unsharded n-qubit state in canonical layout
+ * ({0, 0, 0, 2} when every term is the identity).  Validates the terms as the call does. */
+int qipb200_pauli_lanczos_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms, uint32_t *out4);
+/* Host-only (no GPU, ctx-free): the tridiagonal solve the call runs after each step, on alpha[0..m) and beta[0..m]
+ * laid out as above: the lowest eigenvalue *theta of T_m (diagonal alpha, off-diagonal beta[1..m)), its unit
+ * eigenvector y (m doubles, sign fixed by y[0] >= 0; may be NULL) and *estimate = beta[m] |y[m-1]|.  NULL alpha, beta,
+ * theta or estimate, m == 0 or a non-finite value give QIPB200_ERR_INVALID_ARG. */
+int qipb200_lanczos_ritz(const double *alpha, const double *beta, uint32_t m, double *theta, double *y, double *estimate);
+
 /* ---- multi-GPU: the 2^n state sharded by its top log2(world) index bits,
  *      one process per GPU (absent in the reference; its only hook is the
  *      input_offset/output_offset slice model, matrix_ops.rs:74-89) -------------- */

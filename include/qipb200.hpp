@@ -341,6 +341,40 @@ class B200State {
                                               coeffs.data(), time, tol, &out.first, &out.second));
     return out;
   }
+  // the lowest eigenvalue of H = sum_h coeffs[h] P_h reachable from this state, by plain Lanczos until the Ritz
+  // estimate is <= tol sum |c_h| (non-identity terms) or max_steps; with vector, this state ends as the normalised
+  // Ritz vector.  work_a and work_b are scratch of the same context, precision and size (absent in the reference)
+  struct LanczosResult {
+    double energy = 0.0, residual = 0.0, ritz_norm = 0.0;
+    uint32_t steps = 0;
+    bool converged = false;
+    std::vector<double> alpha, beta;  // alpha_0..alpha_(steps-1); beta_0 = |psi| .. beta_steps
+  };
+  LanczosResult lanczos_pauli_sum(B200State &work_a, B200State &work_b,
+                                  const std::vector<std::vector<std::pair<char, uint64_t>>> &terms,
+                                  const std::vector<double> &coeffs, uint32_t max_steps, double tol,
+                                  bool vector = true) {
+    if (coeffs.size() != terms.size())
+      throw CircuitError("lanczos_pauli_sum: " + std::to_string(terms.size()) + " terms but " +
+                         std::to_string(coeffs.size()) + " coefficients");
+    Flat f(terms);
+    LanczosResult r;
+    const size_t cap = max_steps ? max_steps : 1;
+    r.alpha.assign(cap, 0.0);
+    r.beta.assign(cap + 1, 0.0);
+    double out3[3] = {0.0, 0.0, 0.0};
+    uint32_t conv = 0;
+    ctx_.check(qipb200_state_lanczos_pauli_sum(st_, work_a.st_, work_b.st_, f.q(), f.l(), f.lens.data(), terms.size(),
+                                               coeffs.data(), max_steps, tol, vector ? QIPB200_LANCZOS_VECTOR : 0u,
+                                               &r.steps, &conv, r.alpha.data(), r.beta.data(), out3));
+    r.alpha.resize(r.steps);
+    r.beta.resize(r.steps + 1);
+    r.energy = out3[0];
+    r.residual = out3[1];
+    r.ritz_norm = out3[2];
+    r.converged = conv != 0;
+    return r;
+  }
   // reduced density matrix of up to 10 qubits, row-major 2^k x 2^k; bit i of the row and column index is the value of
   // qubits[i], as in measure_probs (absent in the reference)
   std::vector<std::complex<double>> reduced_density(const std::vector<uint64_t> &qubits) {

@@ -34,7 +34,8 @@ EXPORTS = [
     "qipb200_state_measure", "qipb200_state_expect_paulis", "qipb200_expect_plan", "qipb200_state_reduced_density",
     "qipb200_state_apply_pauli_rotations", "qipb200_pauli_rotation_plan", "qipb200_state_apply_pauli_sum",
     "qipb200_pauli_sum_plan", "qipb200_state_pauli_energy_gradient", "qipb200_pauli_gradient_plan",
-    "qipb200_state_evolve_pauli_sum", "qipb200_pauli_evolution_plan",
+    "qipb200_state_evolve_pauli_sum", "qipb200_pauli_evolution_plan", "qipb200_state_lanczos_pauli_sum",
+    "qipb200_pauli_lanczos_plan", "qipb200_lanczos_ritz",
     "qipb200_state_new_sharded", "qipb200_state_ipc_export", "qipb200_state_ipc_import",
     "qipb200_state_qubit_map", "qipb200_state_exchange_bytes", "qipb200_plan_exchanges",
     "qipb200_state_save", "qipb200_state_load", "qipb200_schedule_parse", "qipb200_schedule_ops", "qipb200_schedule_free", "qipb200_schedule_serialise",
@@ -127,6 +128,13 @@ def lib():
     L.qipb200_pauli_evolution_plan.restype = i32
     L.qipb200_pauli_evolution_plan.argtypes = [i32, u32, vp, vp, vp, C.c_size_t, vp, C.c_double, C.c_double, vp,
                                                C.POINTER(C.c_double), vp, C.c_size_t]
+    L.qipb200_state_lanczos_pauli_sum.restype = i32
+    L.qipb200_state_lanczos_pauli_sum.argtypes = [vp, vp, vp, vp, vp, vp, C.c_size_t, vp, u32, C.c_double, u32,
+                                                  C.POINTER(u32), C.POINTER(u32), vp, vp, vp]
+    L.qipb200_pauli_lanczos_plan.restype = i32
+    L.qipb200_pauli_lanczos_plan.argtypes = [i32, u32, vp, vp, vp, C.c_size_t, vp]
+    L.qipb200_lanczos_ritz.restype = i32
+    L.qipb200_lanczos_ritz.argtypes = [vp, vp, u32, C.POINTER(C.c_double), vp, C.POINTER(C.c_double)]
     L.qipb200_state_new_sharded.restype = i32
     L.qipb200_state_new_sharded.argtypes = [vp, i32, u32, i32, i32, C.POINTER(vp)]
     L.qipb200_state_ipc_export.restype, L.qipb200_state_ipc_export.argtypes = i32, [vp, vp, vp]

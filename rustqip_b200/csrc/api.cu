@@ -23,6 +23,7 @@
 #include "kernels.cuh"
 #include "opcompile.h"
 #include "evolve.h"
+#include "lanczos.h"
 #include "gradient.h"
 #include "pauli_rot.h"
 #include "rdm.h"
@@ -2249,6 +2250,98 @@ extern "C" int qipb200_pauli_evolution_plan(qip_prec prec, uint32_t n_qubits, co
     out3[2] = p.kind == EvolutionPlan::kPhase ? 1u : (uint32_t)std::min<uint64_t>(p.degree * s, UINT32_MAX);
     *tail = p.tail;
     if (coeffs_out && coeffs_cap >= p.C.size()) std::copy(p.C.begin(), p.C.end(), coeffs_out);
+    return (int)QIPB200_OK;
+  });
+}
+
+// ===================================================================================
+// the lowest eigenvalue of a real Pauli sum by Lanczos (lanczos.cu)
+// ===================================================================================
+
+extern "C" int qipb200_state_lanczos_pauli_sum(qipb200_state *state, qipb200_state *work_a, qipb200_state *work_b,
+                                               const uint64_t *qubits, const char *paulis, const uint32_t *term_len,
+                                               size_t n_terms, const double *coeffs, uint32_t max_steps, double tol,
+                                               uint32_t flags, uint32_t *steps, uint32_t *converged, double *alpha,
+                                               double *beta, double *out3) {
+  const std::string who = "lanczos_pauli_sum";
+  if (!state || !work_a || !work_b) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, who + ": NULL state");
+  return guarded(state->ctx, [&]() -> int {
+    // every check runs before any device work: a refused call leaves the three states (and a pending collapse) as
+    // they were
+    if (state == work_a || state == work_b || work_a == work_b)
+      return set_err(state->ctx, QIPB200_ERR_INVALID_ARG, who + ": the three states must differ");
+    int st = check_state_pair(work_a, state, who);
+    if (st == QIPB200_OK) st = check_state_pair(work_b, state, who);
+    if (st != QIPB200_OK) return st;
+    std::vector<PauliTerm> terms;
+    std::string err;
+    st = parse_pauli_terms(state->n, qubits, paulis, term_len, n_terms, &terms, &err);
+    if (st != QIPB200_OK) return set_err(state->ctx, st, err);
+    if ((st = check_finite(state->ctx, coeffs, n_terms, who, "coefficient")) != QIPB200_OK) return st;
+    if (max_steps == 0 || max_steps > kLanczosMaxSteps)
+      return set_err(state->ctx, QIPB200_ERR_INVALID_ARG,
+                     who + ": max_steps must be in 1.." + std::to_string(kLanczosMaxSteps));
+    if (!(tol > 0.0 && tol < 1.0)) return set_err(state->ctx, QIPB200_ERR_INVALID_ARG, who + ": tol must be in (0, 1)");
+    if (flags & ~(uint32_t)QIPB200_LANCZOS_VECTOR)
+      return set_err(state->ctx, QIPB200_ERR_INVALID_ARG, who + ": unknown flags");
+    if (!steps || !converged || !out3)
+      return set_err(state->ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL steps, converged or out3");
+    double a = 0.0, b = 0.0;  // the identity terms' sum and the scale of the others, in list order
+    for (size_t h = 0; h < n_terms; ++h) {
+      if (terms[h].x == 0 && terms[h].z == 0)
+        a += coeffs[h];
+      else
+        b += std::fabs(coeffs[h]);
+    }
+    qipb200_ctx *ctx = state->ctx;
+    CU(ctx, cudaSetDevice(ctx->device));
+    if ((st = prepare_out_of_place(work_a, state)) != QIPB200_OK) return st;
+    if ((st = prepare_out_of_place(work_b, state)) != QIPB200_OK) return st;
+    LanczosResult r;
+    CU(ctx, run_lanczos(state->prec, state->buf, work_a->buf, work_b->buf, state->n_local, phys_terms(state, terms),
+                        coeffs, a, b, max_steps, tol, (flags & QIPB200_LANCZOS_VECTOR) != 0, ctx->stream,
+                        &ctx->launches, &r));
+    if (r.zero_norm)
+      return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": the start state has zero (or non-finite) norm");
+    *steps = r.steps;
+    *converged = r.converged;
+    if (alpha) std::copy(r.alpha.begin(), r.alpha.end(), alpha);
+    if (beta) std::copy(r.beta.begin(), r.beta.end(), beta);
+    out3[0] = r.energy;
+    out3[1] = r.residual;
+    out3[2] = r.xnorm;
+    return (int)QIPB200_OK;
+  });
+}
+
+extern "C" int qipb200_pauli_lanczos_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, const char *paulis,
+                                          const uint32_t *term_len, size_t n_terms, uint32_t *out4) {
+  if (!out4 || (prec != QIP_F32 && prec != QIP_F64) || n_qubits == 0 || n_qubits > 40)
+    return set_err(nullptr, QIPB200_ERR_INVALID_ARG,
+                   "pauli_lanczos_plan: NULL out4, bad precision or n_qubits not in 1..40");
+  return guarded(nullptr, [&]() -> int {
+    std::vector<PauliTerm> terms;
+    std::string err;
+    int st = parse_pauli_terms(n_qubits, qubits, paulis, term_len, n_terms, &terms, &err);
+    if (st != QIPB200_OK) return set_err(nullptr, st, err);
+    lanczos_plan_counts(n_qubits, terms, out4);
+    return (int)QIPB200_OK;
+  });
+}
+
+extern "C" int qipb200_lanczos_ritz(const double *alpha, const double *beta, uint32_t m, double *theta, double *y,
+                                    double *estimate) {
+  const std::string who = "lanczos_ritz";
+  if (!alpha || !beta || !theta || !estimate || m == 0)
+    return set_err(nullptr, QIPB200_ERR_INVALID_ARG, who + ": NULL alpha, beta, theta or estimate, or m == 0");
+  return guarded(nullptr, [&]() -> int {
+    for (uint32_t i = 0; i < m; ++i)
+      if (!std::isfinite(alpha[i]))
+        return set_err(nullptr, QIPB200_ERR_INVALID_ARG, who + ": alpha " + std::to_string(i) + " is not finite");
+    for (uint32_t i = 0; i <= m; ++i)
+      if (!std::isfinite(beta[i]))
+        return set_err(nullptr, QIPB200_ERR_INVALID_ARG, who + ": beta " + std::to_string(i) + " is not finite");
+    lanczos_ritz(alpha, beta, m, theta, y, estimate);
     return (int)QIPB200_OK;
   });
 }

@@ -28,7 +28,8 @@
 // work_a for odd k, work_b for even k; src = T_(k-1) (S for k = 1) is the only operand read at partner indices and is
 // never written in the step, so no sweep has a read-after-write hazard.  Per amplitude, in double, no FMA:
 //   - the first sweep's acc starts at +0.0 (k = 1), at -S (k = 2) or at -T_(k-2) (k >= 3, read from dst, which it
-//     overwrites in place), an exact negation of the value widened to double; later sweeps start at the stored dst;
+//     overwrites in place), RN(start v) of the value v widened to double with start = -1, so an exact negation; later
+//     sweeps start at the stored dst (start = 1);
 //   - the groups add as above, and each sweep stores acc rounded to the state's precision;
 //   - the last sweep of step k >= 2 then updates S at the own index from the stored (rounded) t = T_k, with
 //     cmul(c, v) = (RN(RN(c.x v.x) - RN(c.y v.y)), RN(RN(c.x v.y) + RN(c.y v.x))) and RN additions:
@@ -41,7 +42,10 @@
 // the start value and the rounding of RN(c_h / b)), step k adds a local error e_k with |e_1| <= delta |psi| and
 // |e_k| <= 3 delta |psi| (|A| <= sum_h |2 c_h / b| |T| = 2 |T|, plus |T_(k-2)|).  The error of T_k is
 // sum_(m <= k) U_(k-m)(H~) e_m, and |U_j(H~)| <= j + 1 (Chebyshev polynomials of the second kind), so it is at most
-// 3 delta k (k + 1) / 2 |psi|: quadratic in k.  With C = sum_k |C_k| (|S| <= C |psi| after any step),
+// 3 delta k (k + 1) / 2 |psi|: quadratic in k.  A Lanczos step (run_lanczos_sum, lanczos.cu) uses the same mode with
+// update = 0, start = -RN(beta_j / beta_(j-1)) (an inexact scaling, rounded once), and in its last sweep adds
+// Re(conj(src_j) dst_j) of the stored dst_j (src_j is staged at the own index) into a per-thread double, reduced per
+// warp, then per CTA in warp order into dot[CTA].  With C = sum_k |C_k| (|S| <= C |psi| after any step),
 //   |S_device - sum_k C_k T_k(H~) psi| <= [3 delta sum_k |C_k| k (k + 1) / 2 + sqrt(2) (2 gamma_4(2^-53) + u) K C]
 //                                        x (1 + 3 delta K (K + 1) / 2) |psi|,
 // the second term for the K accumulations into S.  tests/evolve_ref.py: bound().
@@ -96,13 +100,15 @@ struct SumTermDev {
   double c;        // c_h times the sign of Re / Im of i^nY
 };
 
-// One sweep of a Chebyshev step (k_pauli_sum<R, PAIR, true>), see "k_pauli_sum, evolution mode" above.
+// One sweep of a Chebyshev step or a Lanczos step (k_pauli_sum<R, PAIR, true>), see "k_pauli_sum, evolution mode"
+// above and lanczos.cu.
 struct EvoSweep {
-  const void *from;  // the accumulator starts at -from (negate) or +from at the own index; NULL: at +0.0
+  const void *from;  // the accumulator starts at RN(start from) at the own index; NULL: at +0.0
   void *state;       // S, updated at the own index after the store when update != 0
-  uint32_t negate;
+  double start;      // -1 (a Chebyshev step's first sweep), RN(-beta_j / beta_(j-1)) (a Lanczos step's) or 1
   uint32_t update;   // 0: none; 1: S <- c0 S + c1 src + c2 dst (step 2); 2: S <- S + c2 dst (steps >= 3)
   double2 c0, c1, c2;
+  double *dot;       // not NULL: dot[CTA] = the CTA's sum of Re(conj(src_j) dst_j), dst_j as stored (Lanczos)
 };
 
 __device__ __forceinline__ double2 widen(float2 v) { return make_double2(v.x, v.y); }
@@ -166,6 +172,7 @@ __global__ void __launch_bounds__(kGradThreads, 2)
     cp_async_commit();
   }
   int cur = 0;
+  double dsum = 0.0;  // Lanczos: this thread's share of Re<src|dst>, over its amplitudes in visit order
   for (; v < a.n_visits; v += gridDim.x) {
     V *sA, *sB, *dA, *dB;
     if (PAIR) {
@@ -200,7 +207,7 @@ __global__ void __launch_bounds__(kGradThreads, 2)
         const uint32_t e = t + kGradThreads * k;
         acc[k] = make_double2(0.0, 0.0);
         if (load && e < tsize) acc[k] = widen(D[e]);
-        if (EVO && ev.negate) acc[k] = make_double2(-acc[k].x, -acc[k].y);
+        if (EVO) acc[k] = make_double2(__dmul_rn(ev.start, acc[k].x), __dmul_rn(ev.start, acc[k].y));
         if (EVO && ev.update && e < tsize)
           sv[k] = *reinterpret_cast<const V *>((const R *)ev.state + 2 * (b | off[k]));
       }
@@ -240,6 +247,12 @@ __global__ void __launch_bounds__(kGradThreads, 2)
         const uint32_t e = t + kGradThreads * k;
         if (e >= tsize) continue;
         narrow(acc[k], reinterpret_cast<V *>(dst + 2 * (b | off[k])));
+        if (EVO && ev.dot) {
+          V o;
+          narrow(acc[k], &o);
+          const double2 u = widen(own[e]), w = widen(o);
+          dsum = fma(u.x, w.x, fma(u.y, w.y, dsum));
+        }
         if (EVO && ev.update) {
           V o;
           narrow(acc[k], &o);
@@ -255,6 +268,18 @@ __global__ void __launch_bounds__(kGradThreads, 2)
     if (!PAIR) cur ^= 1;
   }
   cp_async_wait<0>();
+  if (EVO && ev.dot) {  // butterfly in the warp, then the 8 warps in order: fixed for a fixed grid
+    __shared__ double wsum[kGradWarps];
+#pragma unroll
+    for (int o = 16; o; o >>= 1) dsum += __shfl_xor_sync(0xffffffffu, dsum, o);
+    if ((t & 31) == 0) wsum[t >> 5] = dsum;
+    __syncthreads();
+    if (t == 0) {
+      double s = 0.0;
+      for (int w = 0; w < kGradWarps; ++w) s += wsum[w];
+      ev.dot[blockIdx.x] = s;
+    }
+  }
 }
 
 // Re(conj(l) w) for w = i^ph (+-1) p as rot1 forms it: swap: w = (-p.y, p.x), else (p.x, p.y), times (-1)^neg.
@@ -714,12 +739,43 @@ cudaError_t run_pauli_evolution(qip_prec prec, void *state, void *work_a, void *
     ev.c2 = make_double2(C[2 * k], C[2 * k + 1]);
     for (uint32_t j = 0; j < S && e == cudaSuccess; ++j) {
       ev.from = j > 0 ? dst : k == 1 ? nullptr : k == 2 ? state : dst;
-      ev.negate = j == 0 && k >= 2;
+      ev.start = j == 0 && k >= 2 ? -1.0 : 1.0;
       ev.update = j + 1 < S ? 0u : k == 1 ? 0u : k == 2 ? 1u : 2u;
       e = launch_sum_any<true>(prec, dst, src, args[j], dg + g_off[j], k == 1 ? dt1 : dt2, 0, ev, s);
       ++*launches;
     }
   }
+  const cudaError_t ef = cudaFreeAsync(d, s);
+  return e != cudaSuccess ? e : ef;
+}
+
+cudaError_t run_lanczos_sum(qip_prec prec, void *dst, const void *src, const void *from, double start, uint32_t n,
+                            const std::vector<PauliTerm> &terms, const double *coeffs, double scale, double *dot,
+                            uint32_t *dot_grid, cudaStream_t s, uint64_t *launches) {
+  std::vector<RotArgs> args;
+  std::vector<SumGroupDev> hg;
+  std::vector<SumTermDev> ht;
+  std::vector<size_t> g_off;
+  if (terms.empty() || !build_sum_tables(n, terms, coeffs, scale, &args, &hg, &ht, &g_off))
+    return cudaErrorInvalidValue;
+  const size_t gbytes = hg.size() * sizeof(SumGroupDev), tbytes = ht.size() * sizeof(SumTermDev);
+  char *d = nullptr;
+  cudaError_t e = cudaMallocAsync((void **)&d, tbytes + gbytes, s);
+  if (e != cudaSuccess) return e;
+  SumTermDev *dt = (SumTermDev *)d;
+  SumGroupDev *dg = (SumGroupDev *)(d + tbytes);
+  e = cudaMemcpyAsync(dt, ht.data(), tbytes, cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(dg, hg.data(), gbytes, cudaMemcpyHostToDevice, s);
+  EvoSweep ev = {};
+  const size_t S = args.size();
+  for (size_t j = 0; j < S && e == cudaSuccess; ++j) {
+    ev.from = j > 0 ? dst : from;
+    ev.start = j > 0 ? 1.0 : start;
+    ev.dot = j + 1 == S ? dot : nullptr;
+    e = launch_sum_any<true>(prec, dst, src, args[j], dg + g_off[j], dt, 0, ev, s);
+    ++*launches;
+  }
+  *dot_grid = (uint32_t)std::min<uint64_t>(args.back().n_visits, (uint64_t)kAdjGrid);
   const cudaError_t ef = cudaFreeAsync(d, s);
   return e != cudaSuccess ? e : ef;
 }

@@ -44,6 +44,14 @@ cudaError_t run_pauli_evolution(qip_prec prec, void *state, void *work_a, void *
                                 const std::vector<PauliTerm> &terms, const double *coeffs, double half_width,
                                 const std::vector<double> &C, cudaStream_t s, uint64_t *launches);
 
+// One Lanczos sum (lanczos.cu): dst <- sum_h RN(coeffs[h] scale) P_h src, the accumulator of the first sweep started at
+// RN(start from) (from NULL: at +0.0), one kernel per sweep of the sum plan.  When dot is not NULL the last sweep writes
+// dot[c] = CTA c's sum of Re(conj(src_j) dst_j) over the stored dst, for c < *dot_grid (a fixed function of the plan).
+// terms must not be empty.  Stream-ordered, no synchronisation.
+cudaError_t run_lanczos_sum(qip_prec prec, void *dst, const void *src, const void *from, double start, uint32_t n,
+                            const std::vector<PauliTerm> &terms, const double *coeffs, double scale, double *dot,
+                            uint32_t *dot_grid, cudaStream_t s, uint64_t *launches);
+
 // The adjoint gradient: state <- U state (run_pauli_rotations), work <- H state (run_pauli_sum), then the backward
 // sweeps, each one adjoint kernel and one reduction kernel.  Launches forward + sum + 2 backward sweeps.  Writes
 // *energy and grad[0..T); synchronises the stream.  grid: CTAs per forward sweep.

@@ -7,7 +7,7 @@ amplitudes stay in HBM between gates; only explicit download copies them out.
 from __future__ import annotations
 
 import ctypes as C
-from typing import Optional, Sequence
+from typing import NamedTuple, Optional, Sequence
 
 import numpy as np
 
@@ -368,6 +368,39 @@ class State:
             float(time), float(_default_tol(self.dtype) if tol is None else tol), C.byref(degree), C.byref(tail)))
         return int(degree.value), float(tail.value)
 
+    def lanczos_pauli_sum(self, work_a: "State", work_b: "State", terms, coeffs, max_steps: int = 300, tol=None,
+                          vector: bool = True) -> "LanczosResult":
+        """The lowest eigenvalue of H = sum_h coeffs[h] P_h, a real Pauli sum, reachable from this state, by plain
+        Lanczos on the device.
+
+        Terms are encoded as for ``apply_pauli_sum``.  Runs from v_0 = psi / |psi| until the estimate
+        rho_m = beta_m |y_(m-1)| of the m-step tridiagonal's lowest Ritz pair (theta, y) is <= tol b, b = sum |coeffs|
+        of the non-identity terms (default tol 1e-8 for complex128, 1e-3 for complex64), or ``max_steps`` (<= 4096)
+        steps: reaching the cap is not an error (``converged`` is False).  Only the part of the spectrum psi has weight
+        on is reachable: a start state in a symmetry sector (fixed S_z, parity, ...) gives that sector's ground state.
+        ``vector=False``: this state is not written, and (energy, residual) = (theta, rho_m).  ``vector=True``: a
+        second pass rebuilds the same Lanczos vectors and this state ends as the normalised Ritz vector x / |x|;
+        energy = <x|H|x> and residual = |Hx - energy x|, both computed on the device, and ``ritz_norm`` = |x| before
+        normalisation (far from 1: loss of orthogonality).  In exact arithmetic some eigenvalue of H lies within
+        residual of energy.  ``work_a`` and ``work_b`` are two more states of the same context, precision and size,
+        used as scratch.  Deterministic; synchronises once per step (``pauli_lanczos_plan`` gives the kernel
+        counts)."""
+        c = np.ascontiguousarray(np.asarray(coeffs, dtype=np.float64).reshape(-1))
+        terms = list(terms)
+        if c.shape[0] != len(terms):
+            raise ValueError("lanczos_pauli_sum: %d terms but %d coefficients" % (len(terms), c.shape[0]))
+        qs, ls, lens = _marshal_paulis(terms)
+        cap = max(1, min(int(max_steps), 4096))
+        alpha, beta, out3 = np.zeros(cap), np.zeros(cap + 1), np.zeros(3)
+        steps, conv = C.c_uint32(), C.c_uint32()
+        self._chk(_lib.lib().qipb200_state_lanczos_pauli_sum(
+            self._h, work_a._h, work_b._h, _ptr(qs), ls, _ptr(lens), lens.shape[0], _ptr(c) if c.shape[0] else None,
+            int(max_steps), float(_default_lanczos_tol(self.dtype) if tol is None else tol), 1 if vector else 0,
+            C.byref(steps), C.byref(conv), _ptr(alpha), _ptr(beta), _ptr(out3)))
+        m = int(steps.value)
+        return LanczosResult(float(out3[0]), float(out3[1]), m, bool(conv.value), alpha[:m].copy(),
+                             beta[: m + 1].copy(), float(out3[2]))
+
     def reduced_density(self, qubits: Sequence[int]) -> np.ndarray:
         """Reduced density matrix of ``qubits`` (1 to 10 of them) on the state as it is (not renormalised), computed
         on the device: complex128 of shape (2^k, 2^k) with rho[a, b] = sum_r psi(r, a) conj(psi(r, b)).
@@ -492,6 +525,49 @@ def pauli_evolution_plan(n: int, dtype, terms, coeffs, time: float, tol=None):
     out = np.zeros(2 * (int(v[0]) + 1), dtype=np.float64)
     call(_ptr(out), out.shape[0])
     return int(v[0]), int(v[1]), int(v[2]), float(tail.value), out.view(np.complex128)
+
+
+class LanczosResult(NamedTuple):
+    """What State.lanczos_pauli_sum returns: alpha[0..steps), beta[0..steps] (beta[0] = |psi|)."""
+    energy: float
+    residual: float
+    steps: int
+    converged: bool
+    alpha: np.ndarray
+    beta: np.ndarray
+    ritz_norm: float
+
+
+def _default_lanczos_tol(dtype):
+    return 1e-8 if np.dtype(cdtype(prec_of(dtype))) == np.complex128 else 1e-3
+
+
+def pauli_lanczos_plan(n: int, dtype, terms):
+    """(sum sweeps per step, kernels per first-pass step, kernels per second-pass step, kernels outside the steps in
+    vector mode) of State.lanczos_pauli_sum on an unsharded n-qubit state (needs no GPU).  A call of m steps launches
+    1 + m k1 kernels without the vector, m k1 + (m - 1) k2 + k0 with it; (0, 0, 0, 2) when every term is the
+    identity."""
+    qs, ls, lens = _marshal_paulis(terms)
+    v = (C.c_uint32 * 4)()
+    _lib.check(_lib.lib().qipb200_pauli_lanczos_plan(prec_of(dtype), int(n), _ptr(qs), ls, _ptr(lens), lens.shape[0],
+                                                     v), None)
+    return tuple(int(x) for x in v)
+
+
+def lanczos_ritz(alpha, beta):
+    """(theta, y, estimate) for the tridiagonal of alpha[0..m) and beta[0..m] as State.lanczos_pauli_sum returns them:
+    the lowest eigenvalue theta of T_m (off-diagonal beta[1..m)), its unit eigenvector y (y[0] >= 0) and
+    beta[m] |y[m-1]| -- the solve the call runs after every step (needs no GPU)."""
+    a = np.ascontiguousarray(np.asarray(alpha, dtype=np.float64).reshape(-1))
+    b = np.ascontiguousarray(np.asarray(beta, dtype=np.float64).reshape(-1))
+    m = a.shape[0]
+    if b.shape[0] != m + 1:
+        raise ValueError("lanczos_ritz: %d alphas need %d betas, got %d" % (m, m + 1, b.shape[0]))
+    theta, est = C.c_double(), C.c_double()
+    y = np.zeros(max(1, m))
+    _lib.check(_lib.lib().qipb200_lanczos_ritz(_ptr(a) if m else None, _ptr(b), m, C.byref(theta), _ptr(y),
+                                               C.byref(est)), None)
+    return float(theta.value), y[:m], float(est.value)
 
 
 def plan_exchanges(ops: Sequence[MatrixOp], n: int, world_size: int, dtype=np.complex128):
