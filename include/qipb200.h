@@ -278,6 +278,31 @@ int qipb200_state_expect_paulis(qipb200_state *state, const uint64_t *qubits, co
  * terms on an unsharded n-qubit state in canonical layout (0 for n_terms == 0).  Validates as the call above does. */
 int qipb200_expect_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms, uint32_t *sweeps);
 
+/* <bra|P_t|ket> for n_terms Pauli strings, on the two states AS THEY ARE (not renormalised); absent in the reference.
+ * Terms are encoded and validated as for qipb200_state_expect_paulis (same codes and messages).  With P = i^nY X^x Z^z,
+ *   <bra|P|ket> = sum_j conj(bra_j) (P ket)_j = i^nY sum_j (-1)^popc(j & z) conj(bra_{j ^ x}) ket_j.
+ * out (HOST, 2 * n_terms doubles) receives (Re, Im) of term t at out[2t], out[2t + 1]; the empty term gives the overlap
+ * <bra|ket>, and <bra|P|ket> is conj(<ket|P|bra>).  bra == ket is allowed (then out[2t] is expect_paulis' value up to
+ * rounding).  Accumulated in double for both precisions (f32 amplitudes are widened before they are multiplied) over a
+ * fixed grid with fixed-order per-CTA partials and one reduction kernel per batch, no floating-point atomics: the same
+ * states and terms give bit-identical out; synchronises.  The summation order and its rounding bound are documented in
+ * rustqip_b200/csrc/expect.cu.  Sweeps are planned as for expect_paulis with two rows (Re and Im) per term, so a read
+ * sweep of both states carries up to 8192 terms; one kernel per sweep plus one reduction kernel per batch of at most
+ * 16384 rows (qipb200_transition_plan reports both counts).
+ * Errors, all before any device work (a refused call leaves both states and a pending collapse as they were): NULL bra
+ * or ket, and NULL out with n_terms > 0, give QIPB200_ERR_INVALID_ARG; a term error the code and message of
+ * expect_paulis; states of different contexts, precisions or sizes QIPB200_ERR_SIZE_MISMATCH; sharded or multi-device
+ * states QIPB200_ERR_UNSUPPORTED.  n_terms == 0 is a no-op.  A collapse pending on either state is applied first (one
+ * kernel each).  Layouts: two states with the same qubit map (canonical, or permuted alike by QIPB200_ROTATE) are read
+ * where they are and keep their layout; otherwise each permuted state is first restored to the canonical layout, with
+ * the kernels of that restore (swap-only tile passes under QIPB200_ROTATE, one bit-swap kernel per transposition
+ * otherwise), and its amplitudes stay logically the same, as before a download. */
+int qipb200_state_transition_paulis(qipb200_state *bra, qipb200_state *ket, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms, double *out);
+/* Host-only (no GPU, ctx-free): out2 = {read sweeps, kernels} of the call above on unsharded n-qubit states in
+ * canonical layout with nothing pending ({0, 0} for n_terms == 0).  Validates as the call above does; NULL out2, a bad
+ * precision or n_qubits not in 1..40 give QIPB200_ERR_INVALID_ARG. */
+int qipb200_transition_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms, uint32_t *out2);
+
 /* Reduced density matrix of the k = n_qubits_kept qubits `qubits` on the state AS IT IS (not renormalised, like
  * measure_probs); absent in the reference.  out (HOST, 2 * 4^k doubles, interleaved re/im) receives
  *   rho[a * 2^k + b] = sum_r psi(r, a) conj(psi(r, b))      (partial trace over every other qubit)

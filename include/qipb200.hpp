@@ -273,6 +273,20 @@ class B200State {
                                            out.data()));
     return out;
   }
+  // <this|P_t|ket> for Pauli strings encoded as in expect_paulis; ket is a state of the same context, precision and
+  // size (it may be this one), and the empty term gives the overlap (absent in the reference)
+  std::vector<std::complex<double>> transition_paulis(B200State &ket,
+                                                      const std::vector<std::vector<std::pair<char, uint64_t>>> &terms) {
+    Flat f(terms);
+    std::vector<std::complex<double>> out(terms.size());
+    ctx_.check(qipb200_state_transition_paulis(st_, ket.st_, f.q(), f.l(), f.lens.data(), terms.size(),
+                                               reinterpret_cast<double *>(out.data())));
+    return out;
+  }
+  // <this|ket>
+  std::complex<double> overlap(B200State &ket) {
+    return transition_paulis(ket, std::vector<std::vector<std::pair<char, uint64_t>>>(1))[0];
+  }
   // psi <- exp(-i angles[T-1]/2 P_{T-1}) ... exp(-i angles[0]/2 P_0) psi for Pauli strings encoded as in
   // expect_paulis, term 0 first (absent in the reference)
   void apply_pauli_rotations(const std::vector<std::vector<std::pair<char, uint64_t>>> &terms,

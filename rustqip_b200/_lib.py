@@ -31,7 +31,8 @@ EXPORTS = [
     "qipb200_state_apply_op", "qipb200_state_apply_schedule", "qipb200_state_norm2",
     "qipb200_state_sync", "qipb200_state_max_abs_diff", "qipb200_calculate_state", "qipb200_state_measure_probs",
     "qipb200_state_measure_prob", "qipb200_state_soft_measure", "qipb200_state_sample", "qipb200_state_collapse",
-    "qipb200_state_measure", "qipb200_state_expect_paulis", "qipb200_expect_plan", "qipb200_state_reduced_density",
+    "qipb200_state_measure", "qipb200_state_expect_paulis", "qipb200_expect_plan", "qipb200_state_transition_paulis",
+    "qipb200_transition_plan", "qipb200_state_reduced_density",
     "qipb200_state_apply_pauli_rotations", "qipb200_pauli_rotation_plan", "qipb200_state_apply_pauli_sum",
     "qipb200_pauli_sum_plan", "qipb200_state_pauli_energy_gradient", "qipb200_pauli_gradient_plan",
     "qipb200_state_evolve_pauli_sum", "qipb200_pauli_evolution_plan", "qipb200_state_lanczos_pauli_sum",
@@ -106,6 +107,10 @@ def lib():
     L.qipb200_state_expect_paulis.argtypes = [vp, vp, vp, vp, C.c_size_t, vp]
     L.qipb200_expect_plan.restype = i32
     L.qipb200_expect_plan.argtypes = [i32, u32, vp, vp, vp, C.c_size_t, C.POINTER(u32)]
+    L.qipb200_state_transition_paulis.restype = i32
+    L.qipb200_state_transition_paulis.argtypes = [vp, vp, vp, vp, vp, C.c_size_t, vp]
+    L.qipb200_transition_plan.restype = i32
+    L.qipb200_transition_plan.argtypes = [i32, u32, vp, vp, vp, C.c_size_t, vp]
     L.qipb200_state_reduced_density.restype = i32
     L.qipb200_state_reduced_density.argtypes = [vp, vp, u32, vp]
     L.qipb200_state_apply_pauli_rotations.restype = i32

@@ -1950,6 +1950,55 @@ extern "C" int qipb200_expect_plan(qip_prec prec, uint32_t n_qubits, const uint6
   });
 }
 
+extern "C" int qipb200_state_transition_paulis(qipb200_state *bra, qipb200_state *ket, const uint64_t *qubits,
+                                               const char *paulis, const uint32_t *term_len, size_t n_terms,
+                                               double *out) {
+  const std::string who = "transition_paulis";
+  if (!bra || !ket) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, who + ": NULL state");
+  return guarded(bra->ctx, [&]() -> int {
+    // every check runs before any device work: a refused call leaves both states (and a pending collapse) as they were
+    std::vector<PauliTerm> terms;
+    std::string err;
+    int st = parse_pauli_terms(bra->n, qubits, paulis, term_len, n_terms, &terms, &err);
+    if (st != QIPB200_OK) return set_err(bra->ctx, st, err);
+    if (bra->ctx != ket->ctx || bra->prec != ket->prec || bra->n != ket->n)
+      return set_err(bra->ctx, QIPB200_ERR_SIZE_MISMATCH, who + ": the states differ in context, precision or size");
+    if (bra->world > 1 || !bra->shards.empty() || ket->world > 1 || !ket->shards.empty())
+      return set_err(bra->ctx, QIPB200_ERR_UNSUPPORTED, who + ": sharded states are not supported");
+    if (n_terms == 0) return (int)QIPB200_OK;
+    if (!out) return set_err(bra->ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL out");
+    qipb200_ctx *ctx = bra->ctx;
+    CU(ctx, cudaSetDevice(ctx->device));
+    if ((st = materialise_collapse(bra)) != QIPB200_OK) return st;
+    if ((st = materialise_collapse(ket)) != QIPB200_OK) return st;
+    // One qubit map: the states are read where they are (Pauli masks permute with the bits).  Two maps: each permuted
+    // state goes back to the canonical layout first, as before a download.
+    if (bra->phys_of_logical != ket->phys_of_logical) {
+      if ((st = restore_layout(bra)) != QIPB200_OK) return st;
+      if ((st = restore_layout(ket)) != QIPB200_OK) return st;
+    }
+    CU(ctx, run_transition(bra->prec, bra->buf, ket->buf, bra->n_local, phys_terms(bra, terms), out, ctx->stream,
+                           &ctx->launches));
+    return (int)QIPB200_OK;
+  });
+}
+
+extern "C" int qipb200_transition_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, const char *paulis,
+                                       const uint32_t *term_len, size_t n_terms, uint32_t *out2) {
+  if (!out2 || (prec != QIP_F32 && prec != QIP_F64) || n_qubits == 0 || n_qubits > 40)
+    return set_err(nullptr, QIPB200_ERR_INVALID_ARG,
+                   "transition_plan: NULL out2, bad precision or n_qubits not in 1..40");
+  return guarded(nullptr, [&]() -> int {
+    std::vector<PauliTerm> terms;
+    std::string err;
+    int st = parse_pauli_terms(n_qubits, qubits, paulis, term_len, n_terms, &terms, &err);
+    if (st != QIPB200_OK) return set_err(nullptr, st, err);
+    out2[0] = out2[1] = 0;
+    if (!terms.empty()) transition_plan_counts(n_qubits, terms, out2);
+    return (int)QIPB200_OK;
+  });
+}
+
 // ===================================================================================
 // reduced density matrices (rdm.cu)
 // ===================================================================================

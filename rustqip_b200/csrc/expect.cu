@@ -31,6 +31,25 @@
 // Scratch: at most kExpBatchTerms rows per batch, 8 B per row and CTA (34.6 MB for kExpGrid = 264) plus the term
 // tables; a longer term list runs in several batches, each with its own reduction kernel.  Shared memory: at most
 // 111.4 KiB per CTA (f64 tile pair), so two CTAs fit on an SM.
+//
+// Two-state mode (k_expect<R, true>, qipb200_state_transition_paulis): <bra|P|ket> = i^nY sum_j (-1)^popc(j & z) c_j
+// with c_j = conj(bra_{j^x}) ket_j.  The conjugate-symmetry shortcut needs bra == ket, so a tile pair (B, B') sums both
+// sides explicitly for every group: side B from conj(bra_B') ket_B, side B' from conj(bra_B) ket_B', the diagonal group
+// from conj(bra_B) ket_B and conj(bra_B') ket_B'; every amplitude of each state is still read once per sweep.  c_j is
+// complex for the diagonal group too, so every term keeps both components: it is two rows, Re(i^nY w) and Im(i^nY w),
+// i.e. a +-1 times one component of w (nY = 0..3: (re, im), (-im, re), (-re, -im), (im, -re)).  The planner and the
+// batches count rows, so a sweep carries up to kExpBatchTerms / 2 terms.  Staged tiles: ket_B and bra_B (the one-state
+// pair footprint, 111.4 KiB at f64), on a tile pair also ket_B' and bra_B' (175.4 KiB at f64: one CTA per SM; 111.4 KiB
+// at f32).
+// Rounding, each component, in units of S = sum_j |bra_{j^x}| |ket_j| (tests/transition_ref.py):
+//   - c_j: two double products and one add per component (f32 amplitudes are exact in double): gamma_2;
+//   - per tile: a Walsh-Hadamard output (11 add levels), or a per-thread sum of 8 (8 adds), a warp sum (5) and a sum
+//     over 8 warps (8 adds) after the tile loop: at most 21;
+//   - signs and the +-1 of i^nY are exact;
+//   - each thread adds its tile values sequentially over the visits of its CTA, both sides of a pair for every term:
+//     at most 2 ceil(V / G) adds for V = 2^(n-11) tiles over G = 264 CTAs;
+//   - the per-CTA partials are summed sequentially over the G CTAs.
+// Depth D = 2 + 21 + 2 ceil(V / G) + G, the one-state depth, and |got - want| <= gamma_D S per component.
 #include "expect.h"
 
 #include <algorithm>
@@ -147,16 +166,20 @@ __device__ __forceinline__ void wht_tile(double (&c)[kExpPer][2], double *cbuf) 
   __syncthreads();
 }
 
-template <typename R>
+// TWO (qipb200_state_transition_paulis): psi is the ket, bra the bra.  Tiles staged in shared memory: ket_B, bra_B
+// (and ket_B', bra_B' on a tile pair, B' = B ^ x_out).  Every group is summed over both sides of a pair (side B from
+// conj(bra_B') ket_B, side B' from conj(bra_B) ket_B'; the diagonal group from conj(bra_B) ket_B and
+// conj(bra_B') ket_B'), its products are complex (the diagonal group too) and each term is two rows, Re and Im.
+template <typename R, bool TWO>
 __global__ void __launch_bounds__(kExpThreads, 2)
     k_expect(const R *__restrict__ psi, const __grid_constant__ ExpArgs a, const ExpGroupDev *__restrict__ groups,
-             const ExpTermDev *__restrict__ terms, double *__restrict__ partials) {
+             const ExpTermDev *__restrict__ terms, double *__restrict__ partials, const R *__restrict__ bra) {
   typedef typename ExpV<R>::type V;
   extern __shared__ __align__(16) unsigned char smem[];
   const bool pair = a.x_out != 0;
   V *sA = reinterpret_cast<V *>(smem);
   V *sP = sA + kExpTile;
-  double *cbuf = reinterpret_cast<double *>(smem + (pair ? 2 : 1) * kExpTile * sizeof(V));
+  double *cbuf = reinterpret_cast<double *>(smem + (TWO ? (pair ? 4 : 2) : (pair ? 2 : 1)) * kExpTile * sizeof(V));
   double *red = cbuf + 2 * kExpTile;                          // [warp][direct slot]
   const uint32_t n_smem_terms = min(a.n_terms, kExpSmemTerms), n_smem_groups = min(a.n_groups, kExpSmemGroups);
   double *acc_s = red + (kExpThreads / 32) * kExpMaxDirect;                  // [sweep term < kExpSmemTerms]
@@ -190,6 +213,25 @@ __global__ void __launch_bounds__(kExpThreads, 2)
       const uint32_t e = t + kExpThreads * k;
       V u, w;
       u.x = u.y = w.x = w.y = (R)0;
+      if (TWO) {  // ket_B, bra_B, then ket_B', bra_B'
+        V u2, w2;
+        u2.x = u2.y = w2.x = w2.y = (R)0;
+        if (e < tsize) {
+          u = *reinterpret_cast<const V *>(psi + 2 * (base | off[k]));
+          w = *reinterpret_cast<const V *>(bra + 2 * (base | off[k]));
+          if (pair) {
+            u2 = *reinterpret_cast<const V *>(psi + 2 * ((base ^ a.x_out) | off[k]));
+            w2 = *reinterpret_cast<const V *>(bra + 2 * ((base ^ a.x_out) | off[k]));
+          }
+        }
+        sA[e] = u;
+        sP[e] = w;
+        if (pair) {
+          sA[2 * kExpTile + e] = u2;
+          sA[3 * kExpTile + e] = w2;
+        }
+        continue;
+      }
       if (e < tsize) {
         u = *reinterpret_cast<const V *>(psi + 2 * (base | off[k]));
         if (pair) w = *reinterpret_cast<const V *>(psi + 2 * ((base ^ a.x_out) | off[k]));
@@ -200,14 +242,22 @@ __global__ void __launch_bounds__(kExpThreads, 2)
     __syncthreads();
     for (uint32_t g = 0; g < a.n_groups; ++g) {
       const ExpGroupDev G = g < kExpSmemGroups ? sg[g] : groups[g];
-      const int sides = (G.diag && pair) ? 2 : 1;  // the diagonal group sums over both tiles of a pair
+      // the diagonal group sums over both tiles of a pair; with two states every group does
+      const int sides = TWO ? (pair ? 2 : 1) : ((G.diag && pair) ? 2 : 1);
       for (int side = 0; side < sides; ++side) {
         const uint64_t sbase = side ? base ^ a.x_out : base;
         double c[kExpPer][2];
 #pragma unroll
         for (int k = 0; k < kExpPer; ++k) {
           const uint32_t e = t + kExpThreads * k;
-          if (G.diag) {
+          if (TWO) {  // conj(bra_{j ^ x}) ket_j: the bra of the same side for the diagonal group, else the other one
+            const V *sk = sA + (side ? 2 * kExpTile : 0);
+            const V *sb = sA + (((G.diag ? side : side ^ 1) && pair) ? 3 * kExpTile : kExpTile);
+            const V u = sk[e];
+            const V w = sb[e ^ G.x_in];
+            c[k][0] = (double)w.x * (double)u.x + (double)w.y * (double)u.y;
+            c[k][1] = (double)w.x * (double)u.y - (double)w.y * (double)u.x;
+          } else if (G.diag) {
             const V u = (side ? sP : sA)[e];
             c[k][0] = (double)u.x * (double)u.x + (double)u.y * (double)u.y;
             c[k][1] = 0.0;
@@ -232,11 +282,11 @@ __global__ void __launch_bounds__(kExpThreads, 2)
             acc[d] += sd[d].coef * parity_sign(sbase & sd[d].z_out) * s;
           }
         } else {
-          if (G.diag)
+          if (G.diag && !TWO)
             wht_tile<1>(c, cbuf);
           else
             wht_tile<2>(c, cbuf);
-          const uint32_t nc = G.diag ? 1 : 2;
+          const uint32_t nc = (G.diag && !TWO) ? 1 : 2;
           for (uint32_t i = G.first + t; i < G.end; i += kExpThreads) {
             const ExpTermDev T = terms[i];
             const double v = T.coef * parity_sign(sbase & T.z_out) * cbuf[T.z_in * nc + T.comp];
@@ -384,26 +434,54 @@ uint32_t compact(uint64_t v, uint32_t L, const std::vector<uint32_t> &hi_pos) {
   return r;
 }
 
-template <typename R>
-cudaError_t launch_sweep(const void *psi, const ExpArgs &a, const ExpGroupDev *g, const ExpTermDev *t, double *partials,
-                         cudaStream_t s) {
-  const size_t smem = (a.x_out ? 2 : 1) * kExpTile * sizeof(typename ExpV<R>::type) + 2 * kExpTile * sizeof(double) +
-                      (kExpThreads / 32) * kExpMaxDirect * sizeof(double) +
+// Shared memory of a sweep past its staged tiles: the transform buffer, the warp sums of the direct slots, the first
+// accumulators, the direct slots' terms and the first groups.
+constexpr size_t kExpSmemRest = 2 * kExpTile * sizeof(double) + (kExpThreads / 32) * kExpMaxDirect * sizeof(double) +
+                                kExpSmemTerms * sizeof(double) + kExpMaxDirect * sizeof(ExpTermDev) +
+                                kExpSmemGroups * sizeof(ExpGroupDev);
+static_assert(2 * kExpTile * sizeof(double2) + kExpSmemRest <= 113 * 1024,
+              "two CTAs per SM: at most 113 KiB of shared memory each (one state, or two states on one tile)");
+static_assert(4 * kExpTile * sizeof(double2) + kExpSmemRest <= 227 * 1024,
+              "two states on a tile pair: four tiles, one CTA per SM");
+
+// Tiles a sweep stages: ket (and partner), times two with a bra.
+uint32_t staged_tiles(bool two, bool pair) { return (two ? 2u : 1u) * (pair ? 2u : 1u); }
+
+template <typename R, bool TWO>
+cudaError_t launch_sweep(const void *psi, const void *bra, const ExpArgs &a, const ExpGroupDev *g,
+                         const ExpTermDev *t, double *partials, cudaStream_t s) {
+  const size_t smem = staged_tiles(TWO, a.x_out != 0) * kExpTile * sizeof(typename ExpV<R>::type) +
+                      2 * kExpTile * sizeof(double) + (kExpThreads / 32) * kExpMaxDirect * sizeof(double) +
                       std::min(a.n_terms, kExpSmemTerms) * sizeof(double) + kExpMaxDirect * sizeof(ExpTermDev) +
                       std::min(a.n_groups, kExpSmemGroups) * sizeof(ExpGroupDev);
-  const size_t smem_max = 2 * kExpTile * sizeof(double2) + 2 * kExpTile * sizeof(double) +
-                          (kExpThreads / 32) * kExpMaxDirect * sizeof(double) +
-                          kExpSmemTerms * sizeof(double) + kExpMaxDirect * sizeof(ExpTermDev) +
-                          kExpSmemGroups * sizeof(ExpGroupDev);
-  static_assert(2 * kExpTile * sizeof(double2) + 2 * kExpTile * sizeof(double) +
-                        (kExpThreads / 32) * kExpMaxDirect * sizeof(double) + kExpSmemTerms * sizeof(double) +
-                        kExpMaxDirect * sizeof(ExpTermDev) + kExpSmemGroups * sizeof(ExpGroupDev) <= 113 * 1024,
-                "two CTAs per SM: at most 113 KiB of shared memory each");
-  cudaError_t e = cudaFuncSetAttribute(k_expect<R>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
+  const size_t smem_max = staged_tiles(TWO, true) * kExpTile * sizeof(double2) + kExpSmemRest;
+  cudaError_t e = cudaFuncSetAttribute(k_expect<R, TWO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
   if (e != cudaSuccess) return e;
-  k_expect<R><<<kExpGrid, kExpThreads, smem, s>>>((const R *)psi, a, g, t, partials);
+  k_expect<R, TWO><<<kExpGrid, kExpThreads, smem, s>>>((const R *)psi, a, g, t, partials, (const R *)bra);
   return cudaGetLastError();
 }
+
+// End of the reduction batch that starts at sweep k: whole sweeps of at most kExpBatchTerms rows in all.
+size_t batch_end(const std::vector<Sweep> &sw, size_t k) {
+  size_t e = k, rows = 0;
+  while (e < sw.size() && rows + sw[e].n_terms <= kExpBatchTerms) rows += sw[e++].n_terms;
+  return e;
+}
+
+// The rows a call sums: one per term (one state: the real part), or two (two states: Re at row 2t, Im at 2t + 1).
+std::vector<PauliTerm> term_rows(const std::vector<PauliTerm> &terms, bool two) {
+  if (!two) return terms;
+  std::vector<PauliTerm> rows;
+  rows.reserve(2 * terms.size());
+  for (const PauliTerm &p : terms) {
+    rows.push_back(p);
+    rows.push_back(p);
+  }
+  return rows;
+}
+
+cudaError_t run_sweeps(qip_prec prec, const void *psi, const void *bra, uint32_t n,
+                       const std::vector<PauliTerm> &terms, double *out, cudaStream_t s, uint64_t *launches);
 
 }  // namespace
 
@@ -456,9 +534,33 @@ uint32_t expect_sweep_count(uint32_t n, const std::vector<PauliTerm> &terms) {
   return (uint32_t)sw.size();
 }
 
+void transition_plan_counts(uint32_t n, const std::vector<PauliTerm> &terms, uint32_t *out2) {
+  std::vector<Sweep> sw;
+  plan_sweeps(n, term_rows(terms, true), &sw);
+  uint32_t batches = 0;
+  for (size_t k = 0; k < sw.size(); k = batch_end(sw, k)) ++batches;
+  out2[0] = (uint32_t)sw.size();
+  out2[1] = (uint32_t)sw.size() + batches;
+}
+
 cudaError_t run_expect(qip_prec prec, const void *psi, uint32_t n, const std::vector<PauliTerm> &terms, double *out,
                        cudaStream_t s, uint64_t *launches) {
-  if (terms.empty()) return cudaSuccess;
+  return run_sweeps(prec, psi, nullptr, n, terms, out, s, launches);
+}
+
+cudaError_t run_transition(qip_prec prec, const void *bra, const void *ket, uint32_t n,
+                           const std::vector<PauliTerm> &terms, double *out, cudaStream_t s, uint64_t *launches) {
+  return run_sweeps(prec, ket, bra, n, terms, out, s, launches);
+}
+
+namespace {
+
+// One state (bra == NULL): out[t] = Re <psi|P_t|psi>.  Two: out[2t], out[2t + 1] = Re, Im <bra|P_t|psi>.
+cudaError_t run_sweeps(qip_prec prec, const void *psi, const void *bra, uint32_t n,
+                       const std::vector<PauliTerm> &terms_in, double *out, cudaStream_t s, uint64_t *launches) {
+  if (terms_in.empty()) return cudaSuccess;
+  const bool two = bra != nullptr;
+  const std::vector<PauliTerm> terms = term_rows(terms_in, two);
   std::vector<Sweep> sw;
   plan_sweeps(n, terms, &sw);
   const uint32_t L = std::min(kExpL, n);
@@ -509,7 +611,11 @@ cudaError_t run_expect(qip_prec prec, const void *psi, uint32_t n, const std::ve
         const uint32_t ph = P.n_y & 3;  // Re(i^ph w): +Re, -Im, -Re, +Im
         td.comp = ph & 1;
         td.coef = (ph == 0 || ph == 3) ? 1.0 : -1.0;
-        if (S.x_out && !gd.diag) {  // + the partner tile: w + eta conj(w)
+        if (two && (G.terms[j] & 1)) {  // Im(i^ph w): +Im, +Re, -Im, -Re
+          td.comp = (ph & 1) ^ 1;
+          td.coef = ph < 2 ? 1.0 : -1.0;
+        }
+        if (S.x_out && !gd.diag && !two) {  // + the partner tile: w + eta conj(w)
           const double eta = (popc64(P.x & P.z) & 1) ? -1.0 : 1.0;
           td.coef *= td.comp ? 1.0 - eta : 1.0 + eta;
         }
@@ -527,8 +633,9 @@ cudaError_t run_expect(qip_prec prec, const void *psi, uint32_t n, const std::ve
   std::vector<std::pair<size_t, size_t>> batches;  // [first sweep, end sweep)
   size_t rows_cap = 0, groups_cap = 0;
   for (size_t k = 0; k < sw.size();) {
-    size_t e = k, rows = 0;
-    while (e < sw.size() && rows + sw[e].n_terms <= kExpBatchTerms) rows += sw[e++].n_terms;
+    const size_t e = batch_end(sw, k);
+    size_t rows = 0;
+    for (size_t i = k; i < e; ++i) rows += sw[i].n_terms;
     batches.push_back(std::make_pair(k, e));
     rows_cap = std::max(rows_cap, rows);
     groups_cap = std::max(groups_cap, (e < sw.size() ? g_off[e] : hg.size()) - g_off[k]);
@@ -561,7 +668,12 @@ cudaError_t run_expect(qip_prec prec, const void *psi, uint32_t n, const std::ve
       a.rows = rows;
       const ExpGroupDev *g = d_groups + (g_off[k] - g_off[k0]);
       const ExpTermDev *t = d_terms + a.row_off;
-      e = prec == QIP_F32 ? launch_sweep<float>(psi, a, g, t, d_part, s) : launch_sweep<double>(psi, a, g, t, d_part, s);
+      if (two)
+        e = prec == QIP_F32 ? launch_sweep<float, true>(psi, bra, a, g, t, d_part, s)
+                            : launch_sweep<double, true>(psi, bra, a, g, t, d_part, s);
+      else
+        e = prec == QIP_F32 ? launch_sweep<float, false>(psi, nullptr, a, g, t, d_part, s)
+                            : launch_sweep<double, false>(psi, nullptr, a, g, t, d_part, s);
       ++*launches;
     }
     if (e == cudaSuccess) {
@@ -580,5 +692,7 @@ cudaError_t run_expect(qip_prec prec, const void *psi, uint32_t n, const std::ve
   for (size_t r = 0; r < res.size(); ++r) out[orig[r]] = res[r];
   return cudaSuccess;
 }
+
+}  // namespace
 
 }  // namespace qipb200

@@ -30,4 +30,13 @@ uint32_t expect_sweep_count(uint32_t n, const std::vector<PauliTerm> &terms);
 cudaError_t run_expect(qip_prec prec, const void *psi, uint32_t n, const std::vector<PauliTerm> &terms, double *out,
                        cudaStream_t s, uint64_t *launches);
 
+// out2 = {read sweeps, kernels} run_transition makes for these terms on an unsharded 2^n state.
+void transition_plan_counts(uint32_t n, const std::vector<PauliTerm> &terms, uint32_t *out2);
+
+// out[2t], out[2t + 1] = Re, Im <bra|P_t|ket> for terms on physical index bits of two unsharded 2^n states of the same
+// layout (bra == ket allowed).  The sweeps of run_expect over two rows per term (Re and Im), each sweep reading both
+// states once; one kernel per sweep and one reduction kernel per batch; synchronises the stream.
+cudaError_t run_transition(qip_prec prec, const void *bra, const void *ket, uint32_t n,
+                           const std::vector<PauliTerm> &terms, double *out, cudaStream_t s, uint64_t *launches);
+
 }  // namespace qipb200

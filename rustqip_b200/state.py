@@ -290,6 +290,26 @@ class State:
         self._chk(_lib.lib().qipb200_state_expect_paulis(self._h, _ptr(qs), ls, _ptr(lens), lens.shape[0], _ptr(out)))
         return out[: lens.shape[0]]
 
+    def transition_paulis(self, ket: "State", terms) -> np.ndarray:
+        """<self|P_t|ket> (complex128) for each Pauli string P_t, on the two states as they are (not renormalised),
+        computed on the device; this state is the bra.
+
+        Terms are encoded as for ``expect_paulis``; an empty term gives the overlap <self|ket>.  ``ket`` must be a
+        state of the same context, precision and size (it may be this state).  Pending collapses are applied first;
+        states with the same qubit layout are read where they are, otherwise each permuted one is restored first.  A
+        read sweep of both states carries up to 8192 terms (``transition_plan`` gives the counts); deterministic;
+        synchronises.  For <phi|H|psi> with H = sum_t c_t P_t take ``np.dot(c, phi.transition_paulis(psi, P))``."""
+        qs, ls, lens = _marshal_paulis(terms)
+        out = np.zeros(max(1, 2 * lens.shape[0]), dtype=np.float64)
+        self._chk(_lib.lib().qipb200_state_transition_paulis(self._h, ket._h, _ptr(qs), ls, _ptr(lens), lens.shape[0],
+                                                             _ptr(out)))
+        return out[: 2 * lens.shape[0]].view(np.complex128)
+
+    def overlap(self, ket: "State") -> complex:
+        """<self|ket> on the device (``transition_paulis`` of the empty term); the fidelity of two normalised states
+        is ``abs(a.overlap(b)) ** 2``."""
+        return complex(self.transition_paulis(ket, [[]])[0])
+
     def apply_pauli_rotations(self, terms, angles):
         """Apply exp(-i angles[t]/2 P_t) for each Pauli string P_t, term 0 first, on the device.
 
@@ -469,6 +489,16 @@ def expect_plan(n: int, dtype, terms) -> int:
     _lib.check(_lib.lib().qipb200_expect_plan(prec_of(dtype), int(n), _ptr(qs), ls, _ptr(lens), lens.shape[0],
                                              C.byref(v)), None)
     return int(v.value)
+
+
+def transition_plan(n: int, dtype, terms):
+    """(read sweeps, kernels) of State.transition_paulis for these terms on unsharded n-qubit states in canonical
+    layout with nothing pending (needs no GPU); (0, 0) for no terms."""
+    qs, ls, lens = _marshal_paulis(terms)
+    v = (C.c_uint32 * 2)()
+    _lib.check(_lib.lib().qipb200_transition_plan(prec_of(dtype), int(n), _ptr(qs), ls, _ptr(lens), lens.shape[0], v),
+               None)
+    return int(v[0]), int(v[1])
 
 
 def pauli_rotation_plan(n: int, dtype, terms) -> int:
