@@ -336,6 +336,44 @@ int qipb200_state_apply_pauli_rotations(qipb200_state *state, const uint64_t *qu
  * n-qubit state in canonical layout (0 for n_terms == 0).  Validates the terms as the call above does. */
 int qipb200_pauli_rotation_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms, uint32_t *sweeps);
 
+/* Classical functions applied to a register: U |x>|y> = e^{i theta(x)} |x>|y XOR f(x)> for a function given as a table
+ * (the row rule of the reference's FunctionOpIterator, qip-iterators/src/iterators/qubit_iterators.rs:221-271, which
+ * no MatrixOp reaches): Grover and Shor oracles, modular arithmetic, cost-table phases.
+ * Bit convention (that of measure_probs): bit i of x is the value of qubit in_qubits[i], and bit i of f(x) is XORed
+ * into qubit out_qubits[i].  In the reference's numbering of the op's rows (indices = in ++ out, indices[0] the most
+ * significant bit), row (x, y) therefore reads column (x, y ^ flip_bits(n_out, f(flip_bits(n_in, x)))).
+ *
+ * A function is a handle bound to the context it was made on, kept on its device, and applies to states of either
+ * precision.  function_new validates and uploads the table once (an oracle is applied many times): f[x] for
+ * x < 2^n_in (n_out-bit values, kept as u32; may be NULL when n_out == 0) and, when theta is not NULL, the pair
+ * (cos theta[x], sin theta[x]) computed in double on the host.  Errors: NULL ctx or out, n_in == 0, f NULL with
+ * n_out > 0, n_out == 0 with theta NULL (nothing to apply), f[x] >= 2^n_out or a non-finite theta[x] (the message
+ * names the first such x) give QIPB200_ERR_INVALID_ARG; n_in > 26 (the tables would exceed 1.25 GiB), n_out > 32 and
+ * multi-device contexts QIPB200_ERR_UNSUPPORTED; a failed device allocation QIPB200_ERR_OOM.  Synchronises.
+ * function_free is stream-ordered (cudaFreeAsync on the context's stream), so it may follow an apply at once; free
+ * every function before its context is shut down. */
+typedef struct qipb200_function qipb200_function;
+int qipb200_function_new(qipb200_ctx *ctx, uint32_t n_in, uint32_t n_out, const uint64_t *f, const double *theta, qipb200_function **out);
+void qipb200_function_free(qipb200_function *fn);
+/* psi <- U psi with x on the fn's n_in qubits in_qubits and y on its n_out qubits out_qubits (may be NULL when
+ * n_out == 0).  Arithmetic (fixed, so that it can be emulated bit for bit): without theta the op moves amplitudes and
+ * is exact (-0 is preserved); with theta, c = RN(cos theta(x)) and s = RN(sin theta(x)) in the state's precision and,
+ * for the partner amplitude (a, b) = psi_{j ^ d},
+ *   psi'_j = (RN(RN(c a) - RN(s b)), RN(RN(c b) + RN(s a)))
+ * without FMA, so the result depends neither on the path nor on the layout.  Errors, all before any device work (a
+ * refused call leaves the state and a pending collapse as they were): NULL state or fn, or NULL qubit arrays where
+ * their count is > 0, QIPB200_ERR_INVALID_ARG; a qubit >= n, or one repeated within or across the two registers,
+ * QIPB200_ERR_BAD_INDEX; sharded and multi-device states QIPB200_ERR_UNSUPPORTED; fn made on another context
+ * QIPB200_ERR_INVALID_ARG.  A pending collapse is applied first (one more kernel); a permuted layout is worked on where
+ * it is and keeps its qubit map.  Stream-ordered like apply_schedule (does not synchronise); exactly one kernel, one
+ * read-write sweep of the state: a staged tile path when the low 4 index bits and the out register's index bits fit
+ * one tile of T_max = 11 (f64) or 12 (f32) bits, a pair path otherwise (rustqip_b200/csrc/function.h). */
+int qipb200_state_apply_function(qipb200_state *state, const qipb200_function *fn, const uint64_t *in_qubits, const uint64_t *out_qubits);
+/* Host-only (no GPU, ctx-free): out2 = {path: 0 staged tile / 1 pair, tile bits of the staged path (0 for pair)} of the
+ * call above on an unsharded n-qubit state in canonical layout.  NULL out2, a bad precision or n_qubits not in 1..40
+ * give QIPB200_ERR_INVALID_ARG; n_in and n_out are checked as function_new checks them, the qubits as the call does. */
+int qipb200_function_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *in_qubits, uint32_t n_in, const uint64_t *out_qubits, uint32_t n_out, uint32_t *out2);
+
 /* dst <- sum_h coeffs[h] P_h src, out of place: H|psi> for a Hamiltonian given as a real Pauli sum (absent in the
  * reference).  Terms are encoded and validated as for qipb200_state_expect_paulis (same codes and messages); an empty
  * term is coeffs[h] times the identity.  NULL coeffs with n_terms > 0, a non-finite coefficient or dst == src give

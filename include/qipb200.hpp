@@ -191,6 +191,33 @@ void apply_op_overwrite(Context &ctx, size_t n, const MatrixOp<P> &op, const std
                                        output.data(), output.size(), input_offset, output_offset));
 }
 
+// ---- classical functions on the device (FunctionOpIterator, qip-iterators/src/iterators/qubit_iterators.rs:221-271) --
+// U|x>|y> = e^{i theta(x)} |x>|y ^ f(x)> for a table of 2^n_in entries, checked and uploaded once; bit i of x is qubit
+// in_qubits[i], bit i of f(x) goes to out_qubits[i] (B200State::apply_function).  f may be empty when n_out == 0,
+// theta empty for a pure permutation.
+class B200Function {
+ public:
+  B200Function(Context &ctx, uint32_t n_in, uint32_t n_out, const std::vector<uint64_t> &f,
+               const std::vector<double> &theta = {})
+      : n_in_(n_in), n_out_(n_out) {
+    const size_t size = n_in < 64 ? size_t(1) << n_in : 0;
+    if ((!f.empty() && f.size() != size) || (!theta.empty() && theta.size() != size))
+      throw CircuitError("B200Function: f and theta need 2^n_in = " + std::to_string(size) + " entries each");
+    ctx.check(qipb200_function_new(ctx.get(), n_in, n_out, f.empty() ? nullptr : f.data(),
+                                   theta.empty() ? nullptr : theta.data(), &fn_));
+  }
+  ~B200Function() { qipb200_function_free(fn_); }
+  B200Function(const B200Function &) = delete;
+  B200Function &operator=(const B200Function &) = delete;
+  uint32_t n_in() const { return n_in_; }
+  uint32_t n_out() const { return n_out_; }
+  const qipb200_function *get() const { return fn_; }
+
+ private:
+  uint32_t n_in_, n_out_;
+  qipb200_function *fn_ = nullptr;
+};
+
 // ---- device-resident state: the body of LocalBuilder::calculate_state_with_init -------------------
 template <typename P>
 class B200State {
@@ -310,6 +337,16 @@ class B200State {
     ctx_.check(qipb200_state_apply_pauli_rotations(st_, qubits.empty() ? &no_qubit : qubits.data(),
                                                    letters.empty() ? &no_letter : letters.data(), lens.data(),
                                                    terms.size(), angles.data()));
+  }
+  // psi <- U psi for U|x>|y> = e^{i theta(x)} |x>|y ^ f(x)>: x on in_qubits, y on out_qubits (absent from the
+  // reference's MatrixOp)
+  void apply_function(const B200Function &fn, const std::vector<uint64_t> &in_qubits,
+                      const std::vector<uint64_t> &out_qubits = {}) {
+    if (in_qubits.size() != fn.n_in() || out_qubits.size() != fn.n_out())
+      throw CircuitError("apply_function: the function takes " + std::to_string(fn.n_in()) + " input and " +
+                         std::to_string(fn.n_out()) + " output qubits");
+    ctx_.check(qipb200_state_apply_function(st_, fn.get(), in_qubits.empty() ? nullptr : in_qubits.data(),
+                                            out_qubits.empty() ? nullptr : out_qubits.data()));
   }
   // this state <- H src for H = sum_h coeffs[h] P_h, Pauli strings encoded as in expect_paulis; src is another state
   // of the same context, precision and size, and this state takes its layout (absent in the reference)

@@ -33,7 +33,8 @@ EXPORTS = [
     "qipb200_state_measure_prob", "qipb200_state_soft_measure", "qipb200_state_sample", "qipb200_state_collapse",
     "qipb200_state_measure", "qipb200_state_expect_paulis", "qipb200_expect_plan", "qipb200_state_transition_paulis",
     "qipb200_transition_plan", "qipb200_state_reduced_density",
-    "qipb200_state_apply_pauli_rotations", "qipb200_pauli_rotation_plan", "qipb200_state_apply_pauli_sum",
+    "qipb200_state_apply_pauli_rotations", "qipb200_pauli_rotation_plan", "qipb200_function_new",
+    "qipb200_function_free", "qipb200_state_apply_function", "qipb200_function_plan", "qipb200_state_apply_pauli_sum",
     "qipb200_pauli_sum_plan", "qipb200_state_pauli_energy_gradient", "qipb200_pauli_gradient_plan",
     "qipb200_state_evolve_pauli_sum", "qipb200_pauli_evolution_plan", "qipb200_state_lanczos_pauli_sum",
     "qipb200_pauli_lanczos_plan", "qipb200_lanczos_ritz",
@@ -117,6 +118,13 @@ def lib():
     L.qipb200_state_apply_pauli_rotations.argtypes = [vp, vp, vp, vp, C.c_size_t, vp]
     L.qipb200_pauli_rotation_plan.restype = i32
     L.qipb200_pauli_rotation_plan.argtypes = [i32, u32, vp, vp, vp, C.c_size_t, C.POINTER(u32)]
+    L.qipb200_function_new.restype = i32
+    L.qipb200_function_new.argtypes = [vp, u32, u32, vp, vp, C.POINTER(vp)]
+    L.qipb200_function_free.restype, L.qipb200_function_free.argtypes = None, [vp]
+    L.qipb200_state_apply_function.restype = i32
+    L.qipb200_state_apply_function.argtypes = [vp, vp, vp, vp]
+    L.qipb200_function_plan.restype = i32
+    L.qipb200_function_plan.argtypes = [i32, u32, vp, u32, vp, u32, vp]
     L.qipb200_state_apply_pauli_sum.restype = i32
     L.qipb200_state_apply_pauli_sum.argtypes = [vp, vp, vp, vp, vp, C.c_size_t, vp]
     L.qipb200_pauli_sum_plan.restype = i32

@@ -24,6 +24,7 @@
 #include "opcompile.h"
 #include "evolve.h"
 #include "lanczos.h"
+#include "function.h"
 #include "gradient.h"
 #include "pauli_rot.h"
 #include "rdm.h"
@@ -2088,6 +2089,165 @@ extern "C" int qipb200_pauli_rotation_plan(qip_prec prec, uint32_t n_qubits, con
     int st = parse_pauli_terms(n_qubits, qubits, paulis, term_len, n_terms, &terms, &err);
     if (st != QIPB200_OK) return set_err(nullptr, st, err);
     *sweeps = pauli_rotation_sweep_count(n_qubits, terms);
+    return (int)QIPB200_OK;
+  });
+}
+
+// ===================================================================================
+// classical function ops (function.cu)
+// ===================================================================================
+
+namespace {
+
+// The in and out registers of an n-qubit state: NULL arrays, then every qubit in range and none repeated within or
+// across the two registers.
+int check_function_registers(const qipb200_ctx *ctx, const std::string &who, uint32_t n, const uint64_t *in_q,
+                             uint32_t n_in, const uint64_t *out_q, uint32_t n_out) {
+  if ((n_in && !in_q) || (n_out && !out_q)) return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL qubit array");
+  uint64_t seen = 0;
+  for (int r = 0; r < 2; ++r) {
+    const uint64_t *q = r ? out_q : in_q;
+    const uint32_t m = r ? n_out : n_in;
+    for (uint32_t i = 0; i < m; ++i) {
+      if (q[i] >= n)
+        return set_err(ctx, QIPB200_ERR_BAD_INDEX, who + ": qubit " + std::to_string(q[i]) + " out of range for " +
+                                                       std::to_string(n) + " qubits");
+      if ((seen >> q[i]) & 1)
+        return set_err(ctx, QIPB200_ERR_BAD_INDEX, who + ": qubit " + std::to_string(q[i]) + " repeated");
+      seen |= 1ull << q[i];
+    }
+  }
+  return QIPB200_OK;
+}
+
+// n_in and n_out of a function: the limits function_new and function_plan share.
+int check_function_sizes(const qipb200_ctx *ctx, const std::string &who, uint32_t n_in, uint32_t n_out) {
+  if (n_in == 0) return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": n_in must be at least 1");
+  if (n_in > kFnMaxIn)
+    return set_err(ctx, QIPB200_ERR_UNSUPPORTED,
+                   who + ": at most 26 input qubits (the table of 2^n_in entries would exceed 1.25 GiB)");
+  if (n_out > kFnMaxOut) return set_err(ctx, QIPB200_ERR_UNSUPPORTED, who + ": at most 32 output qubits");
+  return QIPB200_OK;
+}
+
+void free_function_tables(qipb200_function *fn) {
+  cudaSetDevice(fn->ctx->device);
+  if (fn->d_f) cudaFreeAsync(fn->d_f, fn->ctx->stream);
+  if (fn->d_cs) cudaFreeAsync(fn->d_cs, fn->ctx->stream);
+  fn->d_f = nullptr;
+  fn->d_cs = nullptr;
+}
+
+}  // namespace
+
+extern "C" int qipb200_function_new(qipb200_ctx *ctx, uint32_t n_in, uint32_t n_out, const uint64_t *f,
+                                    const double *theta, qipb200_function **out) {
+  const std::string who = "function_new";
+  if (!ctx || !out) return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL context or out-pointer");
+  *out = nullptr;
+  return guarded(ctx, [&]() -> int {
+    // the whole table is checked before anything is allocated
+    int st = check_function_sizes(ctx, who, n_in, n_out);
+    if (st != QIPB200_OK) return st;
+    if (n_out && !f) return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL f with n_out > 0");
+    if (!n_out && !theta)
+      return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": no output qubits and no theta: nothing to apply");
+    const uint64_t N = 1ull << n_in;
+    if (f)
+      for (uint64_t x = 0; x < N; ++x)
+        if (f[x] >> n_out)
+          return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": f[" + std::to_string(x) + "] = " +
+                                                           std::to_string(f[x]) + " does not fit in " +
+                                                           std::to_string(n_out) + " output bits");
+    if (theta)
+      for (uint64_t x = 0; x < N; ++x)
+        if (!std::isfinite(theta[x]))
+          return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": theta[" + std::to_string(x) + "] is not finite");
+    if (!ctx->children.empty())
+      return set_err(ctx, QIPB200_ERR_UNSUPPORTED, who + ": multi-device contexts are not supported");
+    // host copies first: an allocation failure here (std::bad_alloc) leaves nothing behind
+    std::vector<uint32_t> hf(n_out ? N : 0);
+    for (size_t x = 0; x < hf.size(); ++x) hf[x] = (uint32_t)f[x];
+    std::vector<double2> hcs(theta ? N : 0);
+    for (size_t x = 0; x < hcs.size(); ++x) hcs[x] = make_double2(cos(theta[x]), sin(theta[x]));
+    qipb200_function *fn = new qipb200_function();
+    fn->ctx = ctx;
+    fn->n_in = n_in;
+    fn->n_out = n_out;
+    auto fail = [&](cudaError_t e, const char *what) {
+      const int code = cuda_fail(ctx, e, what);
+      free_function_tables(fn);
+      delete fn;
+      return code;
+    };
+    cudaError_t e = cudaSetDevice(ctx->device);
+    if (e != cudaSuccess) return fail(e, "cudaSetDevice");
+    if (n_out) {
+      if ((e = cudaMallocAsync((void **)&fn->d_f, N * sizeof(uint32_t), ctx->stream)) != cudaSuccess)
+        return fail(e, "cudaMallocAsync(function table)");
+      if ((e = cudaMemcpyAsync(fn->d_f, hf.data(), N * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream)) !=
+          cudaSuccess)
+        return fail(e, "cudaMemcpyAsync(function table)");
+    }
+    if (theta) {
+      if ((e = cudaMallocAsync((void **)&fn->d_cs, N * sizeof(double2), ctx->stream)) != cudaSuccess)
+        return fail(e, "cudaMallocAsync(phase table)");
+      if ((e = cudaMemcpyAsync(fn->d_cs, hcs.data(), N * sizeof(double2), cudaMemcpyHostToDevice, ctx->stream)) !=
+          cudaSuccess)
+        return fail(e, "cudaMemcpyAsync(phase table)");
+    }
+    if ((e = cudaStreamSynchronize(ctx->stream)) != cudaSuccess) return fail(e, "cudaStreamSynchronize");
+    *out = fn;
+    return (int)QIPB200_OK;
+  });
+}
+
+extern "C" void qipb200_function_free(qipb200_function *fn) {
+  if (!fn) return;
+  free_function_tables(fn);  // stream-ordered: an apply queued before runs first
+  delete fn;
+}
+
+extern "C" int qipb200_state_apply_function(qipb200_state *s, const qipb200_function *fn, const uint64_t *in_qubits,
+                                            const uint64_t *out_qubits) {
+  const std::string who = "apply_function";
+  if (!s || !fn) return set_err(s ? s->ctx : nullptr, QIPB200_ERR_INVALID_ARG, who + ": NULL state or function");
+  return guarded(s->ctx, [&]() -> int {
+    // every check runs before any device work: a refused call leaves the state (and a pending collapse) as it was
+    int st = check_function_registers(s->ctx, who, s->n, in_qubits, fn->n_in, out_qubits, fn->n_out);
+    if (st != QIPB200_OK) return st;
+    if (s->world > 1 || !s->shards.empty())
+      return set_err(s->ctx, QIPB200_ERR_UNSUPPORTED, who + ": sharded states are not supported");
+    if (fn->ctx != s->ctx)
+      return set_err(s->ctx, QIPB200_ERR_INVALID_ARG, who + ": the function was made on another context");
+    qipb200_ctx *ctx = s->ctx;
+    CU(ctx, cudaSetDevice(ctx->device));
+    if ((st = materialise_collapse(s)) != QIPB200_OK) return st;
+    // A permuted layout (QIPB200_ROTATE) needs no restore: the registers are read and written where their qubits are.
+    uint32_t in_pos[kFnMaxIn], out_pos[kFnMaxOut];
+    for (uint32_t i = 0; i < fn->n_in; ++i) in_pos[i] = s->phys_of_logical[s->n - 1 - (uint32_t)in_qubits[i]];
+    for (uint32_t i = 0; i < fn->n_out; ++i) out_pos[i] = s->phys_of_logical[s->n - 1 - (uint32_t)out_qubits[i]];
+    CU(ctx, run_function(s->prec, s->buf, s->n_local, in_pos, fn->n_in, out_pos, fn->n_out, fn->d_f, fn->d_cs,
+                         ctx->sm_count, ctx->stream, &ctx->launches));
+    return (int)QIPB200_OK;
+  });
+}
+
+extern "C" int qipb200_function_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *in_qubits, uint32_t n_in,
+                                     const uint64_t *out_qubits, uint32_t n_out, uint32_t *out2) {
+  const std::string who = "function_plan";
+  if (!out2 || (prec != QIP_F32 && prec != QIP_F64) || n_qubits == 0 || n_qubits > 40)
+    return set_err(nullptr, QIPB200_ERR_INVALID_ARG, who + ": NULL out2, bad precision or n_qubits not in 1..40");
+  return guarded(nullptr, [&]() -> int {
+    int st = check_function_sizes(nullptr, who, n_in, n_out);
+    if (st != QIPB200_OK) return st;
+    if ((st = check_function_registers(nullptr, who, n_qubits, in_qubits, n_in, out_qubits, n_out)) != QIPB200_OK)
+      return st;
+    uint32_t out_pos[kFnMaxOut];
+    for (uint32_t i = 0; i < n_out; ++i) out_pos[i] = n_qubits - 1 - (uint32_t)out_qubits[i];
+    const FnPlan p = plan_function(prec, n_qubits, out_pos, n_out);
+    out2[0] = p.path;
+    out2[1] = p.tile_bits;
     return (int)QIPB200_OK;
   });
 }

@@ -93,6 +93,15 @@ struct qipb200_state {
   double pend_p_mult = 1.0;
 };
 
+// A classical function of an n_in-bit register (qipb200_function_new): its tables live on ctx's device and are freed
+// on ctx's stream.
+struct qipb200_function {
+  qipb200_ctx *ctx = nullptr;
+  uint32_t n_in = 0, n_out = 0;
+  uint32_t *d_f = nullptr;    // f[x] for x < 2^n_in, NULL when n_out == 0
+  double2 *d_cs = nullptr;    // (cos, sin) of theta[x] in double, NULL without phases
+};
+
 namespace qipb200 {
 
 // RAII bracket of one profiled region (no-op unless ctx->profile).

@@ -325,6 +325,21 @@ class State:
         self._chk(_lib.lib().qipb200_state_apply_pauli_rotations(self._h, _ptr(qs), ls, _ptr(lens), lens.shape[0],
                                                                  _ptr(a) if a.shape[0] else None))
 
+    def apply_function(self, fn: "Function", in_qubits: Sequence[int], out_qubits: Sequence[int] = ()):
+        """Apply U|x>|y> = e^{i theta(x)} |x>|y XOR f(x)> of ``fn`` on the device: bit i of x is the value of qubit
+        ``in_qubits[i]`` and bit i of f(x) is XORed into qubit ``out_qubits[i]`` (the convention of
+        ``measure_probs``).
+
+        One read-write sweep of the state in one kernel, in place (``function_plan`` gives the path).  Without theta
+        the op only moves amplitudes and is exact.  Stream-ordered like ``apply_schedule``."""
+        ia = np.ascontiguousarray(np.asarray(list(in_qubits), dtype=np.uint64))
+        oa = np.ascontiguousarray(np.asarray(list(out_qubits), dtype=np.uint64))
+        if ia.shape[0] != fn.n_in or oa.shape[0] != fn.n_out:
+            raise ValueError("apply_function: the function takes %d input and %d output qubits, got %d and %d" % (
+                fn.n_in, fn.n_out, ia.shape[0], oa.shape[0]))
+        self._chk(_lib.lib().qipb200_state_apply_function(self._h, fn.handle, _ptr(ia) if ia.shape[0] else None,
+                                                          _ptr(oa) if oa.shape[0] else None))
+
     def apply_pauli_sum(self, src: "State", terms, coeffs):
         """Set this state to H|src> for H = sum_h coeffs[h] P_h, a real Pauli sum, on the device (out of place).
 
@@ -456,6 +471,68 @@ class State:
         v = C.c_uint64()
         self._chk(_lib.lib().qipb200_state_exchange_bytes(self._h, C.byref(v)))
         return int(v.value)
+
+
+class Function:
+    """A classical function of an ``n_in``-qubit register kept on the device of ``ctx`` (qipb200_function), for
+    ``State.apply_function``: U|x>|y> = e^{i theta(x)} |x>|y XOR f(x)>.
+
+    ``f`` (n_out-bit integers) and ``theta`` (finite floats, radians) are arrays of length 2^n_in; ``f`` may be None
+    when ``n_out`` is 0 (a phase oracle) and ``theta`` None for a pure permutation.  The table is checked and uploaded
+    once, and the handle serves states of either precision on this context.  n_in <= 26, n_out <= 32."""
+
+    def __init__(self, ctx: Context, n_in: int, n_out: int, f=None, theta=None):
+        self.ctx, self.n_in, self.n_out = ctx, int(n_in), int(n_out)
+        self._h = C.c_void_p()
+        size = 1 << self.n_in if 1 <= self.n_in <= 26 else None  # other sizes are refused by the C entry
+        fa = ta = None
+        if f is not None:
+            fa = np.ascontiguousarray(np.asarray(f, dtype=np.uint64).reshape(-1))
+            if size is not None and fa.shape[0] != size:
+                raise ValueError("Function: f has %d entries, 2^n_in = %d" % (fa.shape[0], size))
+        if theta is not None:
+            ta = np.ascontiguousarray(np.asarray(theta, dtype=np.float64).reshape(-1))
+            if size is not None and ta.shape[0] != size:
+                raise ValueError("Function: theta has %d entries, 2^n_in = %d" % (ta.shape[0], size))
+        _lib.check(_lib.lib().qipb200_function_new(ctx.handle, self.n_in, self.n_out,
+                                                   None if fa is None else _ptr(fa), None if ta is None else _ptr(ta),
+                                                   C.byref(self._h)), ctx.handle)
+
+    @property
+    def handle(self):
+        return self._h
+
+    def free(self):
+        """Release the device tables (stream-ordered: safe straight after an apply)."""
+        if self._h:
+            _lib.lib().qipb200_function_free(self._h)
+            self._h = C.c_void_p()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.free()
+
+    def __del__(self):  # pragma: no cover
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
+FUNCTION_TILE, FUNCTION_PAIR = 0, 1
+
+
+def function_plan(n: int, dtype, in_qubits: Sequence[int], out_qubits: Sequence[int] = ()):
+    """(path, tile bits) of State.apply_function on an unsharded n-qubit state in canonical layout (needs no GPU):
+    path FUNCTION_TILE (0, the staged tile path) or FUNCTION_PAIR (1, tile bits 0)."""
+    ia = np.ascontiguousarray(np.asarray(list(in_qubits), dtype=np.uint64))
+    oa = np.ascontiguousarray(np.asarray(list(out_qubits), dtype=np.uint64))
+    v = (C.c_uint32 * 2)()
+    _lib.check(_lib.lib().qipb200_function_plan(prec_of(dtype), int(n), _ptr(ia) if ia.shape[0] else None,
+                                                ia.shape[0], _ptr(oa) if oa.shape[0] else None, oa.shape[0], v), None)
+    return int(v[0]), int(v[1])
 
 
 def validate_op(op: MatrixOp, n: int, dtype=np.complex128):
