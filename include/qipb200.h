@@ -414,6 +414,39 @@ int qipb200_state_pauli_energy_gradient(qipb200_state *state, qipb200_state *wor
  * in canonical layout.  Validates both term lists as the call does. */
 int qipb200_pauli_gradient_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms, const uint64_t *ham_qubits, const char *ham_paulis, const uint32_t *ham_term_len, size_t n_ham, uint32_t *out3);
 
+/* The quantum geometric tensor of a Pauli-rotation circuit (absent in the reference).  With U = R_{T-1} ... R_0,
+ * R_t = exp(-i angles[t]/2 P_t) (the convention of qipb200_state_apply_pauli_rotations), psi0 the state on entry,
+ * psi_t = R_t ... R_0 psi0, psi = U psi0 and d_t psi = R_{T-1} ... R_{t+1} (-i/2) P_t psi_t:
+ *   qgt[2 (i T + j) + {0, 1}] = Re, Im of G_ij = <d_i psi|d_j psi> - <d_i psi|psi><psi|d_j psi>,
+ *   expect[t] = e_t = <psi_t|P_t|psi_t> (also <P_t> just before R_t; expect may be NULL).
+ * Re G is the Fubini-Study metric (the matrix of a quantum-natural-gradient step and of McLachlan's imaginary-time
+ * equation), 4 Re G the quantum Fisher information, Im G the antisymmetric part of variational real-time evolution.
+ * In exact arithmetic that is the tensor for a unit-norm psi0; the call computes
+ *   G_tt = (|psi_t|^2 - e_t^2) / 4,   G_ij = (M_ij - e_i e_j) / 4 for i < j,   G_ji = conj(G_ij) (Im G_tt = +0.0),
+ * with M_ij = <mu|P_j|phi>, phi = psi_i and mu = P_i psi_i both carried forward through R_{i+1} .. R_{j-1}.  For
+ * i = 0 .. T-1 in order: a fork (state <- R_i state with the arithmetic of apply_pauli_rotations, work_a <- state,
+ * work_b <- P_i state exactly, |psi_i|^2 and e_i summed in double), then the segment: the sweeps of terms i+1 .. T-1,
+ * each term j adding Re and Im of <work_b|P_j|work_a> and then rotating both work states by R_j with the same
+ * host-rounded c and s.  The order is fixed, so the same inputs give the same bits; the forward error bound is
+ * documented in rustqip_b200/csrc/gradient.cu.  At exit `state` holds U psi0 bit-identical to
+ * qipb200_state_apply_pauli_rotations, `work_a` the same bits and `work_b` P_{T-1} U psi0 exactly.  An empty string
+ * is a global phase: its row and column of G are zero up to rounding.  A parameter shared by several strings gets
+ * A^T G A for its term-to-parameter matrix A (on the host).
+ * Terms are validated as for qipb200_state_expect_paulis (same codes and messages).  A state passed twice, NULL or
+ * non-finite angles or NULL qgt (n_terms > 0) give QIPB200_ERR_INVALID_ARG; states of different contexts, precisions
+ * or sizes QIPB200_ERR_SIZE_MISMATCH; sharded or multi-device states, and n_terms > 2048 (the result alone is 2 T^2
+ * doubles), QIPB200_ERR_UNSUPPORTED; all before any device work (a refused call leaves the three states and a pending
+ * collapse as they were).  A collapse pending on state is applied first; ones pending on the work states are dropped,
+ * and they take the state's layout (a permuted layout is worked on in physical bits and keeps its qubit map).
+ * n_terms == 0 launches no kernel beyond a pending collapse on state and leaves the work states as they are.
+ * Synchronises once, at the end.  Launches the kernel count of qipb200_pauli_geometric_tensor_plan (plus one for a
+ * pending collapse). */
+int qipb200_state_pauli_geometric_tensor(qipb200_state *state, qipb200_state *work_a, qipb200_state *work_b, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms, const double *angles, double *qgt, double *expect);
+/* Host-only (no GPU, ctx-free): out3 = {forks (= T), segment sweeps (the sum over i of the sweeps of terms
+ * i+1 .. T-1), kernels the call launches (T + 2 sweeps + 1, or 0 for T == 0)} on an unsharded n-qubit state in
+ * canonical layout.  Validates the terms as the call does (n_terms > 2048: QIPB200_ERR_UNSUPPORTED). */
+int qipb200_pauli_geometric_tensor_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms, uint32_t *out3);
+
 /* state <- exp(-i time H) state for a real Pauli sum H = sum_h coeffs[h] P_h, by a Chebyshev expansion (absent in the
  * reference).  Terms are encoded and validated as for qipb200_state_apply_pauli_sum (same codes and messages).  The
  * identity terms sum to a; the others give the half-width b = sum |coeffs[h]| >= |H - a|; with H~ = (H - a) / b,

@@ -377,6 +377,23 @@ class B200State {
                                                    coeffs.data(), &out.first, out.second.data()));
     return out;
   }
+  // the quantum geometric tensor of the ansatz (strings encoded as in expect_paulis, term 0 first): returns (G row-major
+  // T x T, e) with G_ij = <d_i psi|d_j psi> - <d_i psi|psi><psi|d_j psi> and e_t = <psi_t|P_t|psi_t>; this state ends
+  // at U psi0, work_a and work_b are scratch of the same context, precision and size (absent in the reference)
+  std::pair<std::vector<std::complex<double>>, std::vector<double>> geometric_tensor(
+      B200State &work_a, B200State &work_b, const std::vector<std::vector<std::pair<char, uint64_t>>> &ansatz,
+      const std::vector<double> &angles) {
+    if (angles.size() != ansatz.size())
+      throw CircuitError("geometric_tensor: " + std::to_string(ansatz.size()) + " terms but " +
+                         std::to_string(angles.size()) + " angles");
+    Flat a(ansatz);
+    std::pair<std::vector<std::complex<double>>, std::vector<double>> out(
+        std::vector<std::complex<double>>(ansatz.size() * ansatz.size()), std::vector<double>(ansatz.size()));
+    ctx_.check(qipb200_state_pauli_geometric_tensor(st_, work_a.st_, work_b.st_, a.q(), a.l(), a.lens.data(),
+                                                    ansatz.size(), angles.data(),
+                                                    reinterpret_cast<double *>(out.first.data()), out.second.data()));
+    return out;
+  }
   // this state <- exp(-i time H) this state for H = sum_h coeffs[h] P_h, by a Chebyshev series cut at the smallest
   // degree K >= 2 whose tail bound is <= tol; work_a and work_b are scratch of the same context, precision and size.
   // Returns (K, tail bound) (absent in the reference)

@@ -36,6 +36,7 @@ EXPORTS = [
     "qipb200_state_apply_pauli_rotations", "qipb200_pauli_rotation_plan", "qipb200_function_new",
     "qipb200_function_free", "qipb200_state_apply_function", "qipb200_function_plan", "qipb200_state_apply_pauli_sum",
     "qipb200_pauli_sum_plan", "qipb200_state_pauli_energy_gradient", "qipb200_pauli_gradient_plan",
+    "qipb200_state_pauli_geometric_tensor", "qipb200_pauli_geometric_tensor_plan",
     "qipb200_state_evolve_pauli_sum", "qipb200_pauli_evolution_plan", "qipb200_state_lanczos_pauli_sum",
     "qipb200_pauli_lanczos_plan", "qipb200_lanczos_ritz",
     "qipb200_state_new_sharded", "qipb200_state_ipc_export", "qipb200_state_ipc_import",
@@ -135,6 +136,10 @@ def lib():
     L.qipb200_pauli_gradient_plan.restype = i32
     L.qipb200_pauli_gradient_plan.argtypes = [i32, u32, vp, vp, vp, C.c_size_t, vp, vp, vp, C.c_size_t,
                                               C.POINTER(u32)]
+    L.qipb200_state_pauli_geometric_tensor.restype = i32
+    L.qipb200_state_pauli_geometric_tensor.argtypes = [vp, vp, vp, vp, vp, vp, C.c_size_t, vp, vp, vp]
+    L.qipb200_pauli_geometric_tensor_plan.restype = i32
+    L.qipb200_pauli_geometric_tensor_plan.argtypes = [i32, u32, vp, vp, vp, C.c_size_t, vp]
     L.qipb200_state_evolve_pauli_sum.restype = i32
     L.qipb200_state_evolve_pauli_sum.argtypes = [vp, vp, vp, vp, vp, vp, C.c_size_t, vp, C.c_double, C.c_double,
                                                  C.POINTER(u32), C.POINTER(C.c_double)]

@@ -2378,6 +2378,75 @@ extern "C" int qipb200_pauli_gradient_plan(qip_prec prec, uint32_t n_qubits, con
 }
 
 // ===================================================================================
+// the quantum geometric tensor of a Pauli-rotation circuit (gradient.cu)
+// ===================================================================================
+
+namespace {
+
+const size_t kQgtMaxTerms = 2048;  // the result alone is 2 T^2 doubles (64 MiB at this size)
+
+int check_qgt_terms(qipb200_ctx *ctx, const std::string &who, size_t n_terms) {
+  if (n_terms > kQgtMaxTerms)
+    return set_err(ctx, QIPB200_ERR_UNSUPPORTED,
+                   who + ": " + std::to_string(n_terms) + " terms, at most " + std::to_string(kQgtMaxTerms));
+  return QIPB200_OK;
+}
+
+}  // namespace
+
+extern "C" int qipb200_state_pauli_geometric_tensor(qipb200_state *state, qipb200_state *work_a,
+                                                    qipb200_state *work_b, const uint64_t *qubits,
+                                                    const char *paulis, const uint32_t *term_len, size_t n_terms,
+                                                    const double *angles, double *qgt, double *expect) {
+  const std::string who = "pauli_geometric_tensor";
+  if (!state || !work_a || !work_b) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, who + ": NULL state");
+  return guarded(state->ctx, [&]() -> int {
+    // every check runs before any device work: a refused call leaves the three states (and a pending collapse) as
+    // they were
+    if (state == work_a || state == work_b || work_a == work_b)
+      return set_err(state->ctx, QIPB200_ERR_INVALID_ARG, who + ": the three states must differ");
+    int st = check_state_pair(work_a, state, who);
+    if (st == QIPB200_OK) st = check_state_pair(work_b, state, who);
+    if (st != QIPB200_OK) return st;
+    std::vector<PauliTerm> ansatz;
+    std::string err;
+    st = parse_pauli_terms(state->n, qubits, paulis, term_len, n_terms, &ansatz, &err);
+    if (st != QIPB200_OK) return set_err(state->ctx, st, err);
+    if ((st = check_finite(state->ctx, angles, n_terms, who, "angle")) != QIPB200_OK) return st;
+    if (n_terms && !qgt) return set_err(state->ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL qgt");
+    if ((st = check_qgt_terms(state->ctx, who, n_terms)) != QIPB200_OK) return st;
+    qipb200_ctx *ctx = state->ctx;
+    CU(ctx, cudaSetDevice(ctx->device));
+    if (n_terms == 0) return materialise_collapse(state);  // the work states are not touched
+    if ((st = prepare_out_of_place(work_a, state)) != QIPB200_OK) return st;
+    if ((st = prepare_out_of_place(work_b, state)) != QIPB200_OK) return st;
+    CU(ctx, run_pauli_qgt(state->prec, state->buf, work_a->buf, work_b->buf, state->n_local,
+                          phys_terms(state, ansatz), angles, ctx->stream, &ctx->launches, qgt, expect));
+    return (int)QIPB200_OK;
+  });
+}
+
+extern "C" int qipb200_pauli_geometric_tensor_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits,
+                                                   const char *paulis, const uint32_t *term_len, size_t n_terms,
+                                                   uint32_t *out3) {
+  const std::string who = "pauli_geometric_tensor_plan";
+  if (!out3 || (prec != QIP_F32 && prec != QIP_F64) || n_qubits == 0 || n_qubits > 40)
+    return set_err(nullptr, QIPB200_ERR_INVALID_ARG, who + ": NULL out3, bad precision or n_qubits not in 1..40");
+  return guarded(nullptr, [&]() -> int {
+    std::vector<PauliTerm> ansatz;
+    std::string err;
+    int st = parse_pauli_terms(n_qubits, qubits, paulis, term_len, n_terms, &ansatz, &err);
+    if (st != QIPB200_OK) return set_err(nullptr, st, err);
+    if ((st = check_qgt_terms(nullptr, who, n_terms)) != QIPB200_OK) return st;
+    const uint32_t T = (uint32_t)n_terms, S = pauli_qgt_sweep_count(n_qubits, ansatz);
+    out3[0] = T;
+    out3[1] = S;
+    out3[2] = T ? T + 2 * S + 1 : 0;
+    return (int)QIPB200_OK;
+  });
+}
+
+// ===================================================================================
 // exp(-iHt) for a real Pauli sum by a Chebyshev expansion (evolve.h, gradient.cu)
 // ===================================================================================
 

@@ -63,6 +63,33 @@
 // fixed kAdjGrid CTAs (or the visit count, when smaller): the same inputs give the same bits on any device.
 // A sweep holds at most kAdjMaxTerms terms so the slots fit shared memory: 64 KiB of tiles, 8 x 257 slots and the
 // staged descriptors, at most 91 KiB per CTA.
+//
+// The quantum geometric tensor (qipb200_state_pauli_geometric_tensor, run_pauli_qgt).  For each term i in order:
+//   - fork i (k_qgt_fork): state <- R_i state with the arithmetic of pauli_rot.cu (the same host-rounded c and s, the
+//     same rot1 per pair), work_a <- the rotated state, work_b <- P_i of it (a permutation, signs and component swaps:
+//     exact).  One thread per amplitude pair (j, j ^ x) of P_i, j with the lowest bit h of x clear, or per element when
+//     x == 0, kForkUnroll pairs in flight, loaded straight from global memory: the two loads of a warp touch the same
+//     32-byte sectors (h < 2 at f64) or two contiguous runs, so the fork reads the state once and writes three states.
+//     It adds |psi'_j|^2 = fma(x, x, y y) and Re(conj(psi'_j) (P psi')_j) = fma(x, px, y py) per element into two
+//     per-thread doubles, reduced by butterfly in the warp, then the 8 warps in order into scratch[2i + {0, 1}][CTA] on
+//     a fixed grid of min(kForkGrid, 2^(n-1) / 256) CTAs; one k_qgt_reduce at the end sums every fork's rows over the
+//     CTAs in order.
+//   - segment i: the walk of gradient.h over terms i + 1 .. T - 1 (the descriptors built with c and +s, so the walk
+//     runs forward) with k_pauli_adjoint in complex-row mode (QGT = true) on phi = work_a, lambda = work_b: per term it
+//     adds Re<lambda|P_j|phi> = sum Re(conj(lambda_k) i w_k) (dot_w_re: the fma policy of dot_w with the other swap)
+//     next to Im<lambda|P_j|phi> (dot_w), two rows per term, no energy row, then rotates both states by R_j.  The
+//     reduction is the adjoint's: per-thread double, warp butterfly, warp slots, CTA sums in warp order, then
+//     k_qgt_reduce sums each row over the CTAs in CTA order into M_ij at res[2 (i T + j)].  Shared memory: 64 KiB of
+//     tiles, 8 warps x 512 rows x 8 B and 256 descriptors x 40 B, 106 KiB per CTA: still two CTAs per SM.
+// The host downloads res (2 T^2 + 2 T doubles) once and forms G_tt = (|psi_t|^2 - e_t^2) / 4, G_ij = (M_ij - e_i e_j) / 4
+// for i < j and G_ji = conj(G_ij).  The grids, the plan and the order of every sum are fixed: the same inputs give the
+// same bits.  Forward error, to first order, for |psi0| = N and u the state's unit roundoff: a state after k rotations
+// is within sqrt(2) gamma_(5k)(u) N of exact (pauli_rot.cu), and psi_t, phi and mu have had at most T rotations (P is
+// exact), so each inner product M_ij, e_t and |psi_t|^2 errs by at most
+//   delta = (2 sqrt(2) gamma_(5T)(u) + gamma_D(2^-53)) N^2,   D = 2^n / 256 + 300 (elements per thread and visit, the
+// warp butterfly, the slots over visits, the warps and the CTAs), with f32 amplitudes widened exactly; |e_t| <= N^2, so
+// |G - G_exact| <= delta (1 + 2 N^2) / 4 + gamma_3(2^-53) N^4 per entry (the host's three roundings).  tests/qgt_ref.py:
+// qgt_bound().
 #include "gradient.h"
 
 #include <algorithm>
@@ -85,7 +112,12 @@ const int kGradPer = kGradTile / kGradThreads;  // tile amplitudes per thread
 const int kGradWarps = kGradThreads / 32;
 const uint32_t kAdjMaxTerms = 256;       // terms of one backward sweep
 const uint32_t kAdjRows = kAdjMaxTerms + 1;  // + the energy
+const uint32_t kQgtRows = 2 * kAdjMaxTerms;  // complex rows: Re and Im per term
 const int kAdjGrid = 264;
+const int kForkThreads = 256;
+const int kForkWarps = kForkThreads / 32;
+const int kForkUnroll = 2;   // amplitude pairs per thread in flight
+const int kForkGrid = 528;   // CTAs of a fork (fewer when the state has fewer items)
 
 struct SumGroupDev {
   uint32_t x_in;   // tile-local X/Y mask
@@ -288,26 +320,37 @@ __device__ __forceinline__ double dot_w(double2 l, double2 p, bool swap, uint32_
   return neg ? -d : d;
 }
 
+// Re(conj(l) i w) = Re<l|P|p> for the same w: dot_w with the other swap and one more negation when swap is set.
+__device__ __forceinline__ double dot_w_re(double2 l, double2 p, bool swap, uint32_t neg) {
+  return dot_w(l, p, !swap, neg ^ (uint32_t)swap);
+}
+
+template <uint32_t ROWS>
 __device__ __forceinline__ void slot_add(double *red, uint32_t row, double g) {
 #pragma unroll
   for (int o = 16; o; o >>= 1) g += __shfl_xor_sync(0xffffffffu, g, o);
-  if ((threadIdx.x & 31) == 0) red[(threadIdx.x >> 5) * kAdjRows + row] += g;
+  if ((threadIdx.x & 31) == 0) red[(threadIdx.x >> 5) * ROWS + row] += g;
 }
 
-template <typename R, bool PAIR>
+// QGT = false: the adjoint gradient (rows: Im<lambda|P_t|phi> per term, then the energy).  QGT = true: a segment of
+// the geometric tensor (rows 2r, 2r + 1: Re and Im of <lambda|P_t|phi> for the sweep's term r, no energy); the
+// direction of the walk comes from the descriptors alone.
+template <typename R, bool PAIR, bool QGT>
 __global__ void __launch_bounds__(kGradThreads, 2)
     k_pauli_adjoint(R *__restrict__ phi, R *__restrict__ lam, const __grid_constant__ RotArgs a,
                     const RotTermDev *__restrict__ terms, uint32_t energy, double *__restrict__ scratch) {
   typedef typename RotV<R>::type V;
+  constexpr uint32_t kRows = QGT ? kQgtRows : kAdjRows;
   extern __shared__ __align__(16) unsigned char smem[];
   // single tiles: [buffer][phi, lambda] double-buffered; pairs: phi A, phi B, lambda A, lambda B
   V *tiles = reinterpret_cast<V *>(smem);
   double *red = reinterpret_cast<double *>(smem + 4 * kGradTile * sizeof(V));  // [warp][row]
-  RotTermDev *sT = reinterpret_cast<RotTermDev *>(red + kGradWarps * kAdjRows);
+  RotTermDev *sT = reinterpret_cast<RotTermDev *>(red + kGradWarps * kRows);
   const int t = threadIdx.x;
-  const uint32_t rows = a.n_terms + (energy ? 1u : 0u);  // the energy is row n_terms
+  // the energy is row n_terms
+  const uint32_t rows = QGT ? 2 * a.n_terms : a.n_terms + (energy ? 1u : 0u);
   for (uint32_t i = t; i < a.n_terms; i += kGradThreads) sT[i] = terms[i];
-  for (uint32_t i = t; i < kGradWarps * kAdjRows; i += kGradThreads) red[i] = 0.0;  // ordered by the loop's barrier
+  for (uint32_t i = t; i < kGradWarps * kRows; i += kGradThreads) red[i] = 0.0;  // ordered by the loop's barrier
   const uint32_t tsize = 1u << a.tb;
   uint64_t off[kGradPer];
 #pragma unroll
@@ -364,7 +407,7 @@ __global__ void __launch_bounds__(kGradThreads, 2)
     }
     __syncthreads();
     const uint64_t bA = base_of(v), bB = bA ^ a.x_out;
-    if (energy) {  // Re<lambda|phi> on the thread's own elements, before any term is undone
+    if (!QGT && energy) {  // Re<lambda|phi> on the thread's own elements, before any term is undone
       double g = 0.0;
       for (int side = 0; side < (PAIR ? 2 : 1); ++side) {
         const V *P = side ? pB : pA, *Lm = side ? lB : lA;
@@ -374,7 +417,7 @@ __global__ void __launch_bounds__(kGradThreads, 2)
           if (e < tsize) g += dot_w(widen(Lm[e]), widen(P[e]), false, 0);
         }
       }
-      slot_add(red, a.n_terms, g);
+      slot_add<kRows>(red, a.n_terms, g);
       // the first term of a sweep carries no barrier and may update elements other warps have yet to read here
       __syncthreads();
     }
@@ -406,15 +449,21 @@ __global__ void __launch_bounds__(kGradThreads, 2)
             const uint32_t zk = D.z_in >> 8;
             const uint32_t par4 = ((zk & 1) ? 0xAu : 0u) ^ ((zk & 2) ? 0xCu : 0u);
             const uint32_t f = par4 ^ (((__popc((uint32_t)t & D.z_in) & 1) ^ (uint32_t)parity(b & D.z_out)) ? 0xFu : 0u);
-            double g = 0.0;
+            double g = 0.0, gr = 0.0;
 #pragma unroll
             for (int k = 0; k < kGradPer; ++k) {
               const uint32_t nk = (f >> k) & 1;
               g += dot_w(widen(q[k]), widen(r[k]), swap, nk ^ (ph >> 1));
+              if (QGT) gr += dot_w_re(widen(q[k]), widen(r[k]), swap, nk ^ (ph >> 1));
               r[k] = rot1<R, V>(r[k], r[k], c, flip_sign(s, nk), swap);
               q[k] = rot1<R, V>(q[k], q[k], c, flip_sign(s, nk), swap);
             }
-            slot_add(red, j, g);
+            if (QGT) {
+              slot_add<kRows>(red, 2 * j, gr);
+              slot_add<kRows>(red, 2 * j + 1, g);
+            } else {
+              slot_add<kRows>(red, j, g);
+            }
           }
 #pragma unroll
           for (int k = 0; k < kGradPer; ++k) {
@@ -431,7 +480,7 @@ __global__ void __launch_bounds__(kGradThreads, 2)
       const uint32_t ph = T.flags & kRotPhase;
       const bool swap = ph & 1;
       const R c = (R)T.c, s = flip_sign((R)T.s, ph >> 1);
-      double g = 0.0;
+      double g = 0.0, gr = 0.0;
       if (PAIR && (T.flags & kRotPair)) {  // (A[e], B[e ^ x_in]) for the thread's own e
         const uint32_t nA = parity(bA & T.z_out), nB = parity(bB & T.z_out);
 #pragma unroll
@@ -442,6 +491,9 @@ __global__ void __launch_bounds__(kGradThreads, 2)
           const uint32_t sa = nB ^ (__popc(f & T.z_in) & 1), sb = nA ^ (__popc(e & T.z_in) & 1);
           const V u = pA[e], w = pB[f], lu = lA[e], lw = lB[f];
           g += dot_w(widen(lu), widen(w), swap, sa ^ (ph >> 1)) + dot_w(widen(lw), widen(u), swap, sb ^ (ph >> 1));
+          if (QGT)
+            gr += dot_w_re(widen(lu), widen(w), swap, sa ^ (ph >> 1)) +
+                  dot_w_re(widen(lw), widen(u), swap, sb ^ (ph >> 1));
           pA[e] = rot1<R, V>(u, w, c, flip_sign(s, sa), swap);
           pB[f] = rot1<R, V>(w, u, c, flip_sign(s, sb), swap);
           lA[e] = rot1<R, V>(lu, lw, c, flip_sign(s, sa), swap);
@@ -461,6 +513,9 @@ __global__ void __launch_bounds__(kGradThreads, 2)
             const uint32_t se = no ^ (__popc(f & T.z_in) & 1), sf = no ^ (__popc(e & T.z_in) & 1);
             const V u = P[e], w = P[f], lu = Lm[e], lw = Lm[f];
             g += dot_w(widen(lu), widen(w), swap, se ^ (ph >> 1)) + dot_w(widen(lw), widen(u), swap, sf ^ (ph >> 1));
+            if (QGT)
+              gr += dot_w_re(widen(lu), widen(w), swap, se ^ (ph >> 1)) +
+                    dot_w_re(widen(lw), widen(u), swap, sf ^ (ph >> 1));
             P[e] = rot1<R, V>(u, w, c, flip_sign(s, se), swap);
             P[f] = rot1<R, V>(w, u, c, flip_sign(s, sf), swap);
             Lm[e] = rot1<R, V>(lu, lw, c, flip_sign(s, se), swap);
@@ -468,7 +523,12 @@ __global__ void __launch_bounds__(kGradThreads, 2)
           }
         }
       }
-      slot_add(red, i, g);
+      if (QGT) {
+        slot_add<kRows>(red, 2 * i, gr);
+        slot_add<kRows>(red, 2 * i + 1, g);
+      } else {
+        slot_add<kRows>(red, i, g);
+      }
       ++i;
     }
     __syncthreads();
@@ -490,7 +550,7 @@ __global__ void __launch_bounds__(kGradThreads, 2)
   __syncthreads();
   for (uint32_t r = t; r < rows; r += kGradThreads) {
     double s = 0.0;
-    for (int w = 0; w < kGradWarps; ++w) s += red[w * kAdjRows + r];
+    for (int w = 0; w < kGradWarps; ++w) s += red[w * kRows + r];
     scratch[(uint64_t)r * gridDim.x + blockIdx.x] = s;
   }
 }
@@ -505,6 +565,114 @@ __global__ void __launch_bounds__(256) k_adjoint_reduce(const double *__restrict
   double s = 0.0;
   for (uint32_t c = 0; c < grid; ++c) s += scratch[(uint64_t)r * grid + c];
   res[r == n_terms ? 0 : T - first - r] = s;
+}
+
+// res[r] = sum over CTAs in order of scratch[r][CTA], r < rows (a segment sweep's rows or every fork's two rows).
+__global__ void __launch_bounds__(256) k_qgt_reduce(const double *__restrict__ scratch, uint32_t rows, uint32_t grid,
+                                                     double *__restrict__ res) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= rows) return;
+  double s = 0.0;
+  for (uint32_t c = 0; c < grid; ++c) s += scratch[(uint64_t)r * grid + c];
+  res[r] = s;
+}
+
+struct ForkArgs {
+  uint64_t x, z;     // the term's X/Y and Z/Y masks on physical index bits
+  uint64_t n_items;  // amplitude pairs (x != 0) or amplitudes (x == 0)
+  uint32_t h;        // lowest bit of x (x != 0)
+  uint32_t ny;       // number of Y letters, mod 4
+  double c, s;       // as the term's RotTermDev: cos and sin of theta/2 rounded to the state's precision
+};
+
+// i^ny (-1)^neg p: (P psi)_j for the partner value p = psi_(j ^ x), a component swap and negations (exact)
+template <typename V>
+__device__ __forceinline__ V pauli_value(V p, uint32_t ny, uint32_t neg) {
+  V o = p;
+  if (ny & 1) {
+    o.x = -p.y;
+    o.y = p.x;
+  }
+  if (((ny >> 1) ^ neg) & 1) {
+    o.x = -o.x;
+    o.y = -o.y;
+  }
+  return o;
+}
+
+// The fork of the geometric tensor: state <- R state, work_a <- R state, work_b <- P R state, in one read of state and
+// three writes; scratch[0][CTA] and scratch[1][CTA] get the CTA's sums of |psi'_j|^2 and Re(conj(psi'_j) (P psi')_j).
+// One thread per pair (j, j ^ x) with bit h of j clear, or per element when x == 0, loaded straight from global memory.
+template <typename R>
+__global__ void __launch_bounds__(kForkThreads, 4)
+    k_qgt_fork(R *__restrict__ state, R *__restrict__ wa, R *__restrict__ wb, const __grid_constant__ ForkArgs f,
+               double *__restrict__ scratch) {
+  typedef typename RotV<R>::type V;
+  V *S = reinterpret_cast<V *>(state), *A = reinterpret_cast<V *>(wa), *B = reinterpret_cast<V *>(wb);
+  const uint32_t ph = (f.ny + 3) & 3;  // w = -i (P psi) = i^ph (+-1) psi_partner, as the rotation descriptors say
+  const bool swap = ph & 1;
+  const R c = (R)f.c, s = flip_sign((R)f.s, ph >> 1);
+  const uint64_t lo = (1ull << f.h) - 1, stride = (uint64_t)gridDim.x * kForkThreads;
+  double nrm = 0.0, ex = 0.0;
+  for (uint64_t p0 = (uint64_t)blockIdx.x * kForkThreads + threadIdx.x; p0 < f.n_items;
+       p0 += kForkUnroll * stride) {
+    uint64_t j[kForkUnroll];
+    V u[kForkUnroll], w[kForkUnroll];
+#pragma unroll
+    for (int k = 0; k < kForkUnroll; ++k) {  // every load of the group before any arithmetic
+      const uint64_t p = p0 + k * stride;
+      if (p >= f.n_items) continue;
+      j[k] = f.x ? ((p & ~lo) << 1) | (p & lo) : p;
+      u[k] = S[j[k]];
+      if (f.x) w[k] = S[j[k] ^ f.x];
+    }
+#pragma unroll
+    for (int k = 0; k < kForkUnroll; ++k) {
+      const uint64_t p = p0 + k * stride;
+      if (p >= f.n_items) continue;
+      const uint64_t jj = j[k], kk = jj ^ f.x;
+      const uint32_t sj = parity(kk & f.z), sk = parity(jj & f.z);  // the signs of (P psi)_j and (P psi)_k
+      if (f.x) {
+        const V a = rot1<R, V>(u[k], w[k], c, flip_sign(s, sj), swap);
+        const V b = rot1<R, V>(w[k], u[k], c, flip_sign(s, sk), swap);
+        const V pa = pauli_value(b, f.ny, sj), pb = pauli_value(a, f.ny, sk);
+        S[jj] = a;
+        S[kk] = b;
+        A[jj] = a;
+        A[kk] = b;
+        B[jj] = pa;
+        B[kk] = pb;
+        const double2 da = widen(a), db = widen(b), dpa = widen(pa), dpb = widen(pb);
+        nrm += fma(da.x, da.x, da.y * da.y) + fma(db.x, db.x, db.y * db.y);
+        ex += fma(da.x, dpa.x, da.y * dpa.y) + fma(db.x, dpb.x, db.y * dpb.y);
+      } else {
+        const V a = rot1<R, V>(u[k], u[k], c, flip_sign(s, sj), swap);
+        const V pa = pauli_value(a, f.ny, sj);
+        S[jj] = a;
+        A[jj] = a;
+        B[jj] = pa;
+        const double2 da = widen(a), dpa = widen(pa);
+        nrm += fma(da.x, da.x, da.y * da.y);
+        ex += fma(da.x, dpa.x, da.y * dpa.y);
+      }
+    }
+  }
+  __shared__ double wsum[kForkWarps][2];
+#pragma unroll
+  for (int o = 16; o; o >>= 1) {
+    nrm += __shfl_xor_sync(0xffffffffu, nrm, o);
+    ex += __shfl_xor_sync(0xffffffffu, ex, o);
+  }
+  if ((threadIdx.x & 31) == 0) {
+    wsum[threadIdx.x >> 5][0] = nrm;
+    wsum[threadIdx.x >> 5][1] = ex;
+  }
+  __syncthreads();
+  if (threadIdx.x < 2) {
+    double t = 0.0;
+    for (int w = 0; w < kForkWarps; ++w) t += wsum[w][threadIdx.x];
+    scratch[(uint64_t)threadIdx.x * gridDim.x + blockIdx.x] = t;
+  }
 }
 
 // ---- host ----------------------------------------------------------------------------------------------------------
@@ -552,17 +720,12 @@ void plan_sum(uint32_t n, const std::vector<PauliTerm> &terms, std::vector<SumGr
   for (SumSweep &S : sw) rot_sweep_fill(&S.geo, n, L, m);
 }
 
-void plan_adjoint(uint32_t n, const std::vector<PauliTerm> &rev, std::vector<RotSweep> *out) {
+// The walk of pauli_rot.h's planner with kGradM high tile bits over `terms`, a sweep cut after every kAdjMaxTerms
+// terms (no terms: no sweeps).
+void plan_walk(uint32_t n, const std::vector<PauliTerm> &terms, std::vector<RotSweep> *out) {
   std::vector<RotSweep> sw;
-  plan_rot_sweeps(n, kGradM, rev, &sw);
+  plan_rot_sweeps(n, kGradM, terms, &sw);
   out->clear();
-  if (sw.empty()) {  // no terms: one sweep for the energy, on the tile of the lowest bits
-    const uint32_t L = std::min(kRotL, n), m = std::min(kGradM, n - L);
-    RotSweep S;
-    rot_sweep_fill(&S, n, L, m);
-    out->push_back(S);
-    return;
-  }
   for (const RotSweep &S : sw)
     for (uint32_t f = S.first; f < S.end; f += kAdjMaxTerms) {
       RotSweep P = S;
@@ -570,6 +733,16 @@ void plan_adjoint(uint32_t n, const std::vector<PauliTerm> &rev, std::vector<Rot
       P.end = std::min(S.end, f + kAdjMaxTerms);
       out->push_back(P);
     }
+}
+
+void plan_adjoint(uint32_t n, const std::vector<PauliTerm> &rev, std::vector<RotSweep> *out) {
+  plan_walk(n, rev, out);
+  if (out->empty()) {  // no terms: one sweep for the energy, on the tile of the lowest bits
+    const uint32_t L = std::min(kRotL, n), m = std::min(kGradM, n - L);
+    RotSweep S;
+    rot_sweep_fill(&S, n, L, m);
+    out->push_back(S);
+  }
 }
 
 template <typename R, bool PAIR, bool EVO>
@@ -645,21 +818,41 @@ bool build_sum_tables(uint32_t n, const std::vector<PauliTerm> &terms, const dou
   return true;
 }
 
-template <typename R, bool PAIR>
+template <typename R, bool PAIR, bool QGT>
 cudaError_t launch_adjoint(void *phi, void *lam, const RotArgs &a, const RotTermDev *terms, uint32_t energy,
                            double *scratch, int grid, cudaStream_t s) {
   typedef typename RotV<R>::type V;
   static_assert(kGradThreads == 256 && kGradPer == 4, "the diagonal path's sign table assumes e = t + 256 k, k < 4");
-  const size_t fixed = 4 * kGradTile * sizeof(V) + kGradWarps * kAdjRows * sizeof(double);
+  const size_t fixed = 4 * kGradTile * sizeof(V) + kGradWarps * (QGT ? kQgtRows : kAdjRows) * sizeof(double);
   static_assert(4 * kGradTile * sizeof(double2) + kGradWarps * kAdjRows * sizeof(double) +
                         kAdjMaxTerms * sizeof(RotTermDev) <= 113 * 1024,
                 "two CTAs per SM: at most 113 KiB of shared memory each");
+  static_assert(4 * kGradTile * sizeof(double2) + kGradWarps * kQgtRows * sizeof(double) +
+                        kAdjMaxTerms * sizeof(RotTermDev) <= 113 * 1024,
+                "complex rows: still two CTAs per SM, at most 113 KiB of shared memory each");
   const size_t smem = fixed + a.n_terms * sizeof(RotTermDev);
-  cudaError_t e = cudaFuncSetAttribute(k_pauli_adjoint<R, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  cudaError_t e = cudaFuncSetAttribute(k_pauli_adjoint<R, PAIR, QGT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        (int)(fixed + kAdjMaxTerms * sizeof(RotTermDev)));
   if (e != cudaSuccess) return e;
-  k_pauli_adjoint<R, PAIR><<<grid, kGradThreads, smem, s>>>((R *)phi, (R *)lam, a, terms, energy, scratch);
+  k_pauli_adjoint<R, PAIR, QGT><<<grid, kGradThreads, smem, s>>>((R *)phi, (R *)lam, a, terms, energy, scratch);
   return cudaGetLastError();
+}
+
+template <bool QGT>
+cudaError_t launch_adjoint_any(qip_prec prec, void *phi, void *lam, const RotArgs &a, const RotTermDev *terms,
+                               uint32_t energy, double *scratch, int grid, cudaStream_t s) {
+  if (prec == QIP_F32)
+    return a.x_out ? launch_adjoint<float, true, QGT>(phi, lam, a, terms, energy, scratch, grid, s)
+                   : launch_adjoint<float, false, QGT>(phi, lam, a, terms, energy, scratch, grid, s);
+  return a.x_out ? launch_adjoint<double, true, QGT>(phi, lam, a, terms, energy, scratch, grid, s)
+                 : launch_adjoint<double, false, QGT>(phi, lam, a, terms, energy, scratch, grid, s);
+}
+
+// The segments of the geometric tensor: for fork i, the walk over terms i + 1 .. T - 1 (sw[i]).
+void plan_segments(uint32_t n, const std::vector<PauliTerm> &ansatz, std::vector<std::vector<RotSweep>> *sw) {
+  sw->assign(ansatz.size(), std::vector<RotSweep>());
+  for (size_t i = 0; i + 1 < ansatz.size(); ++i)
+    plan_walk(n, std::vector<PauliTerm>(ansatz.begin() + i + 1, ansatz.end()), &(*sw)[i]);
 }
 
 }  // namespace
@@ -808,12 +1001,7 @@ cudaError_t run_pauli_gradient(qip_prec prec, void *state, void *work, uint32_t 
     RotArgs &a = args[k];
     const uint32_t en = k == 0, g = (uint32_t)std::min<uint64_t>(a.n_visits, (uint64_t)kAdjGrid);
     const RotTermDev *td = dt + sw[k].first;
-    if (prec == QIP_F32)
-      e = a.x_out ? launch_adjoint<float, true>(state, work, a, td, en, scratch, g, s)
-                  : launch_adjoint<float, false>(state, work, a, td, en, scratch, g, s);
-    else
-      e = a.x_out ? launch_adjoint<double, true>(state, work, a, td, en, scratch, g, s)
-                  : launch_adjoint<double, false>(state, work, a, td, en, scratch, g, s);
+    e = launch_adjoint_any<false>(prec, state, work, a, td, en, scratch, g, s);
     ++*launches;
     if (e != cudaSuccess) break;
     const uint32_t rows = a.n_terms + en;
@@ -830,6 +1018,117 @@ cudaError_t run_pauli_gradient(qip_prec prec, void *state, void *work, uint32_t 
   if (es != cudaSuccess) return es;
   *energy = host[0];
   for (uint32_t t = 0; t < T; ++t) grad[t] = host[1 + t];
+  return cudaSuccess;
+}
+
+uint32_t pauli_qgt_sweep_count(uint32_t n, const std::vector<PauliTerm> &ansatz) {
+  std::vector<std::vector<RotSweep>> sw;
+  plan_segments(n, ansatz, &sw);
+  uint64_t count = 0;
+  for (const std::vector<RotSweep> &v : sw) count += v.size();
+  return (uint32_t)count;
+}
+
+cudaError_t run_pauli_qgt(qip_prec prec, void *state, void *work_a, void *work_b, uint32_t n,
+                          const std::vector<PauliTerm> &ansatz, const double *angles, cudaStream_t s,
+                          uint64_t *launches, double *qgt, double *expect) {
+  const uint32_t T = (uint32_t)ansatz.size();
+  if (T == 0) return cudaSuccess;
+  std::vector<std::vector<RotSweep>> sw;
+  plan_segments(n, ansatz, &sw);
+  // every segment's descriptors (they depend on its sweeps), uploaded once: segment i's from ht[t_off[i]]
+  std::vector<RotArgs> args;
+  std::vector<RotTermDev> ht;
+  std::vector<size_t> t_off(T), a_off(T);
+  for (uint32_t i = 0; i < T; ++i) {
+    t_off[i] = ht.size();
+    a_off[i] = args.size();
+    if (sw[i].empty()) continue;
+    std::vector<PauliTerm> seg(ansatz.begin() + i + 1, ansatz.end());
+    std::vector<RotArgs> a;
+    std::vector<RotTermDev> h;
+    if (!build_rot_tables(prec, n, seg, angles + i + 1, false, sw[i], &a, &h)) return cudaErrorInvalidValue;
+    args.insert(args.end(), a.begin(), a.end());
+    ht.insert(ht.end(), h.begin(), h.end());
+  }
+  // one fork grid per call, so that every fork's two rows reduce over the same CTAs at the end
+  const uint32_t gf = (uint32_t)std::min<uint64_t>(kForkGrid, std::max<uint64_t>(1, (1ull << (n - 1)) / kForkThreads));
+  const size_t tbytes = std::max<size_t>(1, ht.size()) * sizeof(RotTermDev);
+  const size_t sbytes = (size_t)kQgtRows * kAdjGrid * sizeof(double);
+  const size_t fbytes = (size_t)2 * T * gf * sizeof(double);
+  const size_t rcount = (size_t)2 * T * T + 2 * T, rbytes = rcount * sizeof(double);
+  char *d = nullptr;
+  cudaError_t e = cudaMallocAsync((void **)&d, tbytes + sbytes + fbytes + rbytes, s);
+  if (e != cudaSuccess) return e;
+  RotTermDev *dt = (RotTermDev *)d;
+  double *scratch = (double *)(d + tbytes);
+  double *fscratch = (double *)(d + tbytes + sbytes);
+  double *res = (double *)(d + tbytes + sbytes + fbytes);  // M (2 T^2), then (|psi_t|^2, e_t) per fork
+  if (!ht.empty()) e = cudaMemcpyAsync(dt, ht.data(), ht.size() * sizeof(RotTermDev), cudaMemcpyHostToDevice, s);
+  for (uint32_t i = 0; i < T && e == cudaSuccess; ++i) {
+    const PauliTerm &P = ansatz[i];
+    ForkArgs fa;
+    fa.x = P.x;
+    fa.z = P.z;
+    fa.n_items = P.x ? 1ull << (n - 1) : 1ull << n;
+    fa.h = P.x ? (uint32_t)__builtin_ctzll(P.x) : 0u;
+    fa.ny = P.n_y & 3;
+    // c and s exactly as build_rot_tables rounds them, so the fork rotates as the sweeps and pauli_rot.cu do
+    double c = cos(angles[i] / 2), sn = sin(angles[i] / 2);
+    if (prec == QIP_F32) {
+      c = (double)(float)c;
+      sn = (double)(float)sn;
+    }
+    fa.c = c;
+    fa.s = sn;
+    double *fs = fscratch + (size_t)2 * i * gf;
+    if (prec == QIP_F32)
+      k_qgt_fork<float><<<gf, kForkThreads, 0, s>>>((float *)state, (float *)work_a, (float *)work_b, fa, fs);
+    else
+      k_qgt_fork<double><<<gf, kForkThreads, 0, s>>>((double *)state, (double *)work_a, (double *)work_b, fa, fs);
+    e = cudaGetLastError();
+    ++*launches;
+    for (size_t k = 0; k < sw[i].size() && e == cudaSuccess; ++k) {
+      const RotArgs &a = args[a_off[i] + k];
+      const uint32_t g = (uint32_t)std::min<uint64_t>(a.n_visits, (uint64_t)kAdjGrid);
+      e = launch_adjoint_any<true>(prec, work_a, work_b, a, dt + t_off[i] + sw[i][k].first, 0, scratch, g, s);
+      ++*launches;
+      if (e != cudaSuccess) break;
+      // rows 2r + {0, 1} of the sweep belong to term j = i + 1 + first + r: M_ij at res[2 (i T + j)]
+      const uint32_t rows = 2 * a.n_terms;
+      k_qgt_reduce<<<(rows + 255) / 256, 256, 0, s>>>(scratch, rows, g,
+                                                      res + 2 * ((size_t)i * T + i + 1 + sw[i][k].first));
+      e = cudaGetLastError();
+      ++*launches;
+    }
+  }
+  if (e == cudaSuccess) {
+    k_qgt_reduce<<<(2 * T + 255) / 256, 256, 0, s>>>(fscratch, 2 * T, gf, res + (size_t)2 * T * T);
+    e = cudaGetLastError();
+    ++*launches;
+  }
+  std::vector<double> host(rcount);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(host.data(), res, rbytes, cudaMemcpyDeviceToHost, s);
+  const cudaError_t ef = cudaFreeAsync(d, s);
+  const cudaError_t es = cudaStreamSynchronize(s);
+  if (e != cudaSuccess) return e;
+  if (ef != cudaSuccess) return ef;
+  if (es != cudaSuccess) return es;
+  const double *M = host.data(), *F = host.data() + (size_t)2 * T * T;
+  for (uint32_t i = 0; i < T; ++i) {
+    const double ei = F[2 * i + 1];
+    if (expect) expect[i] = ei;
+    qgt[2 * ((size_t)i * T + i)] = 0.25 * (F[2 * i] - ei * ei);
+    qgt[2 * ((size_t)i * T + i) + 1] = 0.0;
+    for (uint32_t j = i + 1; j < T; ++j) {
+      const size_t ij = (size_t)i * T + j, ji = (size_t)j * T + i;
+      const double re = 0.25 * (M[2 * ij] - ei * F[2 * j + 1]), im = 0.25 * M[2 * ij + 1];
+      qgt[2 * ij] = re;
+      qgt[2 * ij + 1] = im;
+      qgt[2 * ji] = re;
+      qgt[2 * ji + 1] = -im;
+    }
+  }
   return cudaSuccess;
 }
 

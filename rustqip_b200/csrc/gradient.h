@@ -12,6 +12,9 @@
 // Adjoint planner (the backward sweeps qipb200_pauli_gradient_plan reports).  The rotation planner of pauli_rot.h with
 // m = min(6, n - L) runs over the reversed term list, and a sweep is cut after every 256 terms.  With no terms it is one
 // sweep that computes the energy only.
+//
+// Segment planner (the segment sweeps qipb200_pauli_geometric_tensor_plan reports).  For fork i the same walk runs over
+// terms i + 1 .. T - 1 in forward order, cut after every 256 terms; the last fork has no segment.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -58,5 +61,18 @@ cudaError_t run_lanczos_sum(qip_prec prec, void *dst, const void *src, const voi
 cudaError_t run_pauli_gradient(qip_prec prec, void *state, void *work, uint32_t n, const std::vector<PauliTerm> &ansatz,
                                const double *angles, const std::vector<PauliTerm> &ham, const double *coeffs, int grid,
                                cudaStream_t s, uint64_t *launches, double *energy, double *grad);
+
+// Segment sweeps run_pauli_qgt makes for this ansatz on an unsharded 2^n state (the sum over forks i of the walk over
+// terms i + 1 .. T - 1).
+uint32_t pauli_qgt_sweep_count(uint32_t n, const std::vector<PauliTerm> &ansatz);
+
+// The quantum geometric tensor of the ansatz (qipb200_state_pauli_geometric_tensor): for each term i one fork
+// (state <- R_i state, work_a <- state, work_b <- P_i state) and the segment sweeps over terms i + 1 .. T - 1 on
+// (work_a, work_b), each one walk kernel and one reduction kernel, then one reduction of the forks' rows.  Launches
+// T + 2 S + 1 kernels (none for T = 0).  Writes qgt[0 .. 2 T^2) (G row-major, (re, im) pairs) and, when expect is not
+// NULL, expect[0 .. T); synchronises the stream.
+cudaError_t run_pauli_qgt(qip_prec prec, void *state, void *work_a, void *work_b, uint32_t n,
+                          const std::vector<PauliTerm> &ansatz, const double *angles, cudaStream_t s,
+                          uint64_t *launches, double *qgt, double *expect);
 
 }  // namespace qipb200

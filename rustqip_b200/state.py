@@ -381,6 +381,33 @@ class State:
             _ptr(hq), hl, _ptr(hlen), hlen.shape[0], _ptr(c) if c.shape[0] else None, _ptr(energy), _ptr(grad)))
         return float(energy[0]), grad[: len(ansatz)]
 
+    def geometric_tensor(self, work_a: "State", work_b: "State", ansatz, angles):
+        """The quantum geometric tensor of the Pauli-rotation circuit U = R_{T-1} ... R_0, R_t = exp(-i angles[t]/2 P_t)
+        (``ansatz`` encoded as for ``apply_pauli_rotations``), at the state on entry psi0, on the device.
+
+        Returns (G, e): G is a complex128 (T, T) array with G_ij = <d_i psi|d_j psi> - <d_i psi|psi><psi|d_j psi>
+        for psi = U psi0, exactly Hermitian; e[t] = <psi_t|P_t|psi_t> (float64, (T,)), the expectation of P_t just
+        before R_t.  Re G is the Fubini-Study metric: the matrix a quantum-natural-gradient step solves against
+        (``np.linalg.lstsq(G.real, g)`` with g from ``energy_gradient``) and the A of McLachlan's imaginary-time
+        equation A theta' = -grad E.  4 Re G is the quantum Fisher information, and Im G is the antisymmetric term of
+        variational real-time evolution.  A parameter shared by several strings (one QAOA angle on many strings) gets
+        A^T G A for its term-to-parameter matrix A (A[t, k] = 1 when string t carries parameter k), computed on the
+        host.  ``work_a`` and ``work_b`` are two more states of the same context, precision and size, used as scratch;
+        this state ends at U psi0, bit-identical to ``apply_pauli_rotations``.  Deterministic; synchronises; at most
+        2048 terms (``pauli_geometric_tensor_plan`` gives the counts)."""
+        a = np.ascontiguousarray(np.asarray(angles, dtype=np.float64).reshape(-1))
+        ansatz = list(ansatz)
+        T = len(ansatz)
+        if a.shape[0] != T:
+            raise ValueError("geometric_tensor: %d terms but %d angles" % (T, a.shape[0]))
+        qs, ls, lens = _marshal_paulis(ansatz)
+        g = np.zeros(max(1, 2 * T * T), dtype=np.float64)
+        e = np.zeros(max(1, T), dtype=np.float64)
+        self._chk(_lib.lib().qipb200_state_pauli_geometric_tensor(
+            self._h, work_a._h, work_b._h, _ptr(qs), ls, _ptr(lens), lens.shape[0], _ptr(a) if T else None, _ptr(g),
+            _ptr(e)))
+        return g[: 2 * T * T].view(np.complex128).reshape(T, T), e[:T]
+
     def evolve_pauli_sum(self, work_a: "State", work_b: "State", terms, coeffs, time: float, tol=None):
         """Set this state to exp(-i time H)|psi> for H = sum_h coeffs[h] P_h, a real Pauli sum, on the device.
 
@@ -605,6 +632,16 @@ def pauli_gradient_plan(n: int, dtype, ansatz, hamiltonian):
     v = (C.c_uint32 * 3)()
     _lib.check(_lib.lib().qipb200_pauli_gradient_plan(prec_of(dtype), int(n), _ptr(qs), ls, _ptr(lens), lens.shape[0],
                                                       _ptr(hq), hl, _ptr(hlen), hlen.shape[0], v), None)
+    return int(v[0]), int(v[1]), int(v[2])
+
+
+def pauli_geometric_tensor_plan(n: int, dtype, ansatz):
+    """(forks, segment sweeps, kernels) of State.geometric_tensor on an unsharded n-qubit state (needs no GPU): one
+    fork per term, the sweeps of terms i+1 .. T-1 summed over i, and T + 2 sweeps + 1 kernels (0 for no terms)."""
+    qs, ls, lens = _marshal_paulis(ansatz)
+    v = (C.c_uint32 * 3)()
+    _lib.check(_lib.lib().qipb200_pauli_geometric_tensor_plan(prec_of(dtype), int(n), _ptr(qs), ls, _ptr(lens),
+                                                              lens.shape[0], v), None)
     return int(v[0]), int(v[1]), int(v[2])
 
 
