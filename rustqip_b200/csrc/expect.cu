@@ -4,9 +4,9 @@
 //   <P> = i^nY * sum_j (-1)^popc(j & z) * c_j,   c_j = conj(a_{j^x}) a_j,
 // so terms with the same x share the products c_j and differ only in the sign pattern.
 //
-// Sweep = tile geometry + x_out.  A tile is the kExpL lowest index bits plus up to kExpM chosen high bits (2^11
-// amplitudes, read as runs of 16 contiguous amplitudes).  Each mask splits as x = x_in ^ x_out with x_in on tile bits;
-// the masks of one sweep share x_out.  With x_out == 0 a CTA holds one tile; otherwise it holds the pair of tiles
+// Sweep = tile geometry + x_out.  A tile (sweep.cuh) is the kSweepL lowest index bits plus up to kExpM chosen high bits
+// (2^11 amplitudes, read as runs of 16 contiguous amplitudes).  Each mask splits as x = x_in ^ x_out with x_in on tile
+// bits; the masks of one sweep share x_out.  With x_out == 0 a CTA holds one tile; otherwise it holds the pair of tiles
 // (B, B ^ x_out), visited once from the side whose lowest x_out bit is clear: the partner's half of the sum is
 // (-1)^popc(x & z) * conj(sum over B), so every amplitude is still read exactly once per sweep.
 //
@@ -57,14 +57,14 @@
 #include <map>
 
 #include "../../include/qipb200.h"
+#include "sweep.cuh"
 
 namespace qipb200 {
 
 namespace {
 
-const uint32_t kExpL = 4;               // low index bits of a tile (runs of 16 amplitudes)
 const uint32_t kExpM = 7;               // chosen high bits of a tile
-const uint32_t kExpTileLog2 = kExpL + kExpM;
+const uint32_t kExpTileLog2 = kSweepL + kExpM;
 const uint32_t kExpTile = 1u << kExpTileLog2;
 const int kExpThreads = 256;
 const int kExpPer = kExpTile / kExpThreads;  // tile amplitudes per thread (8: three in-register WHT stages)
@@ -75,6 +75,7 @@ const uint32_t kExpSmemTerms = 1024;    // accumulators in shared memory; a swee
 const uint32_t kExpSmemGroups = 256;    // group descriptors staged in shared memory; later ones are read from global
 const int kExpGrid = 264;               // CTAs per sweep: two per SM of a 132-SM H100
 static_assert(kExpPer == 8, "the WHT below assumes 8 amplitudes per thread");
+static_assert(kExpM <= kSweepMaxHi, "the high tile bits fit SweepTiles::hi_pos");
 
 struct ExpGroupDev {
   uint32_t x_in;          // tile-local X/Y mask
@@ -91,31 +92,16 @@ struct ExpTermDev {
 };
 
 struct ExpArgs {
-  uint64_t x_out;     // 0, or the out-of-tile X/Y mask shared by the sweep
-  uint64_t n_visits;  // tiles (x_out == 0) or tile pairs
-  uint32_t L, tb;     // low bits, tile bits
-  uint32_t n_out;     // bits of the visit index, spread over out_pos
-  uint32_t n_groups, n_terms, n_direct;
+  SweepTiles geo;
+  uint32_t n_terms, n_direct;
   uint32_t row_off;   // partial row of the sweep's first term in the batch
   uint32_t rows;      // rows of the batch (length of a CTA's column of partials)
-  uint8_t hi_pos[kExpM];
-  uint8_t out_pos[64];
+  uint32_t n_groups;
   uint16_t direct_term[kExpMaxDirect];
   ExpTermDev direct[kExpMaxDirect];  // the direct slots' terms (staged in shared memory by every CTA)
 };
 
-template <typename R>
-struct ExpV;
-template <>
-struct ExpV<float> {
-  typedef float2 type;
-};
-template <>
-struct ExpV<double> {
-  typedef double2 type;
-};
-
-__device__ __forceinline__ double parity_sign(uint64_t v) { return (__popcll(v) & 1) ? -1.0 : 1.0; }
+__device__ __forceinline__ double parity_sign(uint64_t v) { return parity(v) ? -1.0 : 1.0; }
 
 template <int NC>
 __device__ __forceinline__ void butterflies8(double (&c)[kExpPer][2]) {
@@ -174,9 +160,9 @@ template <typename R, bool TWO>
 __global__ void __launch_bounds__(kExpThreads, 2)
     k_expect(const R *__restrict__ psi, const __grid_constant__ ExpArgs a, const ExpGroupDev *__restrict__ groups,
              const ExpTermDev *__restrict__ terms, double *__restrict__ partials, const R *__restrict__ bra) {
-  typedef typename ExpV<R>::type V;
+  typedef typename SweepV<R>::type V;
   extern __shared__ __align__(16) unsigned char smem[];
-  const bool pair = a.x_out != 0;
+  const bool pair = a.geo.x_out != 0;
   V *sA = reinterpret_cast<V *>(smem);
   V *sP = sA + kExpTile;
   double *cbuf = reinterpret_cast<double *>(smem + (TWO ? (pair ? 4 : 2) : (pair ? 2 : 1)) * kExpTile * sizeof(V));
@@ -195,18 +181,12 @@ __global__ void __launch_bounds__(kExpThreads, 2)
   double acc[kExpMaxDirect];
 #pragma unroll
   for (uint32_t d = 0; d < kExpMaxDirect; ++d) acc[d] = 0.0;
-  const uint32_t tsize = 1u << a.tb;
+  const uint32_t tsize = 1u << a.geo.tb;
   uint64_t off[kExpPer];
 #pragma unroll
-  for (int k = 0; k < kExpPer; ++k) {
-    const uint32_t e = t + kExpThreads * k;
-    uint64_t o = e & ((1u << a.L) - 1);
-    for (uint32_t i = 0; i < a.tb - a.L; ++i) o |= (uint64_t)((e >> (a.L + i)) & 1u) << a.hi_pos[i];
-    off[k] = o;
-  }
-  for (uint64_t v = blockIdx.x; v < a.n_visits; v += gridDim.x) {
-    uint64_t base = 0;
-    for (uint32_t i = 0; i < a.n_out; ++i) base |= ((v >> i) & 1ull) << a.out_pos[i];
+  for (int k = 0; k < kExpPer; ++k) off[k] = tile_offset(a.geo, t + kExpThreads * k);
+  for (uint64_t v = blockIdx.x; v < a.geo.n_visits; v += gridDim.x) {
+    const uint64_t base = visit_base(a.geo, v);
     __syncthreads();  // the previous tile's readers are done
 #pragma unroll
     for (int k = 0; k < kExpPer; ++k) {
@@ -220,8 +200,8 @@ __global__ void __launch_bounds__(kExpThreads, 2)
           u = *reinterpret_cast<const V *>(psi + 2 * (base | off[k]));
           w = *reinterpret_cast<const V *>(bra + 2 * (base | off[k]));
           if (pair) {
-            u2 = *reinterpret_cast<const V *>(psi + 2 * ((base ^ a.x_out) | off[k]));
-            w2 = *reinterpret_cast<const V *>(bra + 2 * ((base ^ a.x_out) | off[k]));
+            u2 = *reinterpret_cast<const V *>(psi + 2 * ((base ^ a.geo.x_out) | off[k]));
+            w2 = *reinterpret_cast<const V *>(bra + 2 * ((base ^ a.geo.x_out) | off[k]));
           }
         }
         sA[e] = u;
@@ -234,7 +214,7 @@ __global__ void __launch_bounds__(kExpThreads, 2)
       }
       if (e < tsize) {
         u = *reinterpret_cast<const V *>(psi + 2 * (base | off[k]));
-        if (pair) w = *reinterpret_cast<const V *>(psi + 2 * ((base ^ a.x_out) | off[k]));
+        if (pair) w = *reinterpret_cast<const V *>(psi + 2 * ((base ^ a.geo.x_out) | off[k]));
       }
       sA[e] = u;
       if (pair) sP[e] = w;
@@ -245,7 +225,7 @@ __global__ void __launch_bounds__(kExpThreads, 2)
       // the diagonal group sums over both tiles of a pair; with two states every group does
       const int sides = TWO ? (pair ? 2 : 1) : ((G.diag && pair) ? 2 : 1);
       for (int side = 0; side < sides; ++side) {
-        const uint64_t sbase = side ? base ^ a.x_out : base;
+        const uint64_t sbase = side ? base ^ a.geo.x_out : base;
         double c[kExpPer][2];
 #pragma unroll
         for (int k = 0; k < kExpPer; ++k) {
@@ -328,9 +308,7 @@ __global__ void __launch_bounds__(256) k_expect_reduce(const double *__restrict_
 
 // ---- host: grouping and greedy packing ----------------------------------------------
 
-struct Group {
-  uint64_t x = 0;
-  std::vector<uint32_t> terms;
+struct Group : PauliGroup {
   bool direct = false;
 };
 
@@ -341,26 +319,13 @@ struct Sweep {
   std::vector<Group> groups;
 };
 
-int popc64(uint64_t v) { return __builtin_popcountll(v); }
-
 void plan_sweeps(uint32_t n, const std::vector<PauliTerm> &terms, std::vector<Sweep> *out) {
-  const uint32_t L = std::min(kExpL, n), m = std::min(kExpM, n - L);
+  const uint32_t L = std::min(kSweepL, n), m = std::min(kExpM, n - L);
   const uint64_t low = (1ull << L) - 1;
   // groups of equal X/Y mask in order of first appearance, cut into units of at most kExpBatchTerms terms
-  std::vector<Group> all;
-  std::map<uint64_t, size_t> where;
-  for (uint32_t t = 0; t < (uint32_t)terms.size(); ++t) {
-    auto it = where.find(terms[t].x);
-    if (it == where.end()) {
-      it = where.emplace(terms[t].x, all.size()).first;
-      all.push_back(Group());
-      all.back().x = terms[t].x;
-    }
-    all[it->second].terms.push_back(t);
-  }
   std::vector<Group> units;
   std::vector<uint32_t> diag;
-  for (const Group &g : all)
+  for (const PauliGroup &g : group_by_x(terms))
     if (g.x == 0) {
       diag = g.terms;
     } else {
@@ -387,7 +352,7 @@ void plan_sweeps(uint32_t n, const std::vector<PauliTerm> &terms, std::vector<Sw
         started = true;
       } else {
         const uint64_t h2 = s.hi | ((hx ^ s.x_out) & ~s.hi);
-        if ((uint32_t)popc64(h2) > m) continue;
+        if ((uint32_t)__builtin_popcountll(h2) > m) continue;
         s.hi = h2;
         s.x_out &= ~h2;
       }
@@ -410,14 +375,7 @@ void plan_sweeps(uint32_t n, const std::vector<PauliTerm> &terms, std::vector<Sw
     sw[k].groups.push_back(d);
   }
   for (Sweep &s : sw) {
-    // free tile bits: first x_out bits (fewer tile pairs), then the lowest free bits (longer contiguous runs)
-    for (uint32_t b = 0; b < n && (uint32_t)popc64(s.hi) < m; ++b)
-      if ((s.x_out >> b) & 1) {
-        s.hi |= 1ull << b;
-        s.x_out &= ~(1ull << b);
-      }
-    for (uint32_t b = L; b < n && (uint32_t)popc64(s.hi) < m; ++b)
-      if (!((s.hi >> b) & 1)) s.hi |= 1ull << b;
+    sweep_fill(&s.hi, &s.x_out, n, L, m);
     uint32_t slots = 0;
     for (Group &g : s.groups)
       if (g.terms.size() <= kExpDirectGroupTerms && slots + g.terms.size() <= kExpMaxDirect) {
@@ -426,12 +384,6 @@ void plan_sweeps(uint32_t n, const std::vector<PauliTerm> &terms, std::vector<Sw
       }
     std::stable_partition(s.groups.begin(), s.groups.end(), [](const Group &g) { return g.direct; });
   }
-}
-
-uint32_t compact(uint64_t v, uint32_t L, const std::vector<uint32_t> &hi_pos) {
-  uint32_t r = (uint32_t)(v & ((1ull << L) - 1));
-  for (size_t i = 0; i < hi_pos.size(); ++i) r |= (uint32_t)((v >> hi_pos[i]) & 1ull) << (L + i);
-  return r;
 }
 
 // Shared memory of a sweep past its staged tiles: the transform buffer, the warp sums of the direct slots, the first
@@ -450,7 +402,7 @@ uint32_t staged_tiles(bool two, bool pair) { return (two ? 2u : 1u) * (pair ? 2u
 template <typename R, bool TWO>
 cudaError_t launch_sweep(const void *psi, const void *bra, const ExpArgs &a, const ExpGroupDev *g,
                          const ExpTermDev *t, double *partials, cudaStream_t s) {
-  const size_t smem = staged_tiles(TWO, a.x_out != 0) * kExpTile * sizeof(typename ExpV<R>::type) +
+  const size_t smem = staged_tiles(TWO, a.geo.x_out != 0) * kExpTile * sizeof(typename SweepV<R>::type) +
                       2 * kExpTile * sizeof(double) + (kExpThreads / 32) * kExpMaxDirect * sizeof(double) +
                       std::min(a.n_terms, kExpSmemTerms) * sizeof(double) + kExpMaxDirect * sizeof(ExpTermDev) +
                       std::min(a.n_groups, kExpSmemGroups) * sizeof(ExpGroupDev);
@@ -528,6 +480,21 @@ int parse_pauli_terms(uint32_t n, const uint64_t *qubits, const char *paulis, co
   return QIPB200_OK;
 }
 
+std::vector<PauliGroup> group_by_x(const std::vector<PauliTerm> &terms) {
+  std::vector<PauliGroup> gr;
+  std::map<uint64_t, size_t> where;
+  for (uint32_t t = 0; t < (uint32_t)terms.size(); ++t) {
+    auto it = where.find(terms[t].x);
+    if (it == where.end()) {
+      it = where.emplace(terms[t].x, gr.size()).first;
+      gr.push_back(PauliGroup());
+      gr.back().x = terms[t].x;
+    }
+    gr[it->second].terms.push_back(t);
+  }
+  return gr;
+}
+
 uint32_t expect_sweep_count(uint32_t n, const std::vector<PauliTerm> &terms) {
   std::vector<Sweep> sw;
   plan_sweeps(n, terms, &sw);
@@ -563,7 +530,7 @@ cudaError_t run_sweeps(qip_prec prec, const void *psi, const void *bra, uint32_t
   const std::vector<PauliTerm> terms = term_rows(terms_in, two);
   std::vector<Sweep> sw;
   plan_sweeps(n, terms, &sw);
-  const uint32_t L = std::min(kExpL, n);
+  const uint32_t L = std::min(kSweepL, n);
   const uint64_t low = (1ull << L) - 1;
   // host tables of every sweep, rows in sweep order; batches of whole sweeps of at most kExpBatchTerms rows
   std::vector<ExpArgs> args(sw.size());
@@ -575,18 +542,8 @@ cudaError_t run_sweeps(qip_prec prec, const void *psi, const void *bra, uint32_t
     const Sweep &S = sw[k];
     ExpArgs &a = args[k];
     memset(&a, 0, sizeof(a));
-    std::vector<uint32_t> hi_pos;
-    for (uint32_t b = 0; b < n; ++b)
-      if ((S.hi >> b) & 1) hi_pos.push_back(b);
+    a.geo = sweep_tiles(n, L, S.hi, S.x_out);
     const uint64_t tile = low | S.hi;
-    a.x_out = S.x_out;
-    a.L = L;
-    a.tb = L + (uint32_t)hi_pos.size();
-    for (size_t i = 0; i < hi_pos.size(); ++i) a.hi_pos[i] = (uint8_t)hi_pos[i];
-    const int pair_bit = S.x_out ? __builtin_ctzll(S.x_out) : -1;
-    for (uint32_t b = 0; b < n; ++b)
-      if (!((tile >> b) & 1) && (int)b != pair_bit) a.out_pos[a.n_out++] = (uint8_t)b;
-    a.n_visits = 1ull << a.n_out;
     a.n_groups = (uint32_t)S.groups.size();
     a.n_terms = S.n_terms;
     g_off[k] = hg.size();
@@ -594,7 +551,7 @@ cudaError_t run_sweeps(qip_prec prec, const void *psi, const void *bra, uint32_t
     uint32_t first = 0;
     for (const Group &G : S.groups) {
       ExpGroupDev gd;
-      gd.x_in = compact(G.x & tile, L, hi_pos);
+      gd.x_in = tile_local(a.geo, G.x & tile);
       gd.diag = G.x == 0;
       gd.first = first;
       gd.end = first + (uint32_t)G.terms.size();
@@ -607,7 +564,7 @@ cudaError_t run_sweeps(qip_prec prec, const void *psi, const void *bra, uint32_t
         const PauliTerm &P = terms[G.terms[j]];
         ExpTermDev td;
         td.z_out = P.z & ~tile;
-        td.z_in = compact(P.z & tile, L, hi_pos);
+        td.z_in = tile_local(a.geo, P.z & tile);
         const uint32_t ph = P.n_y & 3;  // Re(i^ph w): +Re, -Im, -Re, +Im
         td.comp = ph & 1;
         td.coef = (ph == 0 || ph == 3) ? 1.0 : -1.0;
@@ -616,7 +573,7 @@ cudaError_t run_sweeps(qip_prec prec, const void *psi, const void *bra, uint32_t
           td.coef = ph < 2 ? 1.0 : -1.0;
         }
         if (S.x_out && !gd.diag && !two) {  // + the partner tile: w + eta conj(w)
-          const double eta = (popc64(P.x & P.z) & 1) ? -1.0 : 1.0;
+          const double eta = (__builtin_popcountll(P.x & P.z) & 1) ? -1.0 : 1.0;
           td.coef *= td.comp ? 1.0 - eta : 1.0 + eta;
         }
         if (G.direct) {

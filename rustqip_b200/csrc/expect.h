@@ -22,6 +22,15 @@ struct PauliTerm {
 int parse_pauli_terms(uint32_t n, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms,
                       std::vector<PauliTerm> *out, std::string *err);
 
+// Terms of one X/Y mask: indices into the term list, in list order.
+struct PauliGroup {
+  uint64_t x = 0;
+  std::vector<uint32_t> terms;
+};
+
+// The terms grouped by X/Y mask, groups in order of first appearance (the sweep planners of expect.cu and gradient.cu).
+std::vector<PauliGroup> group_by_x(const std::vector<PauliTerm> &terms);
+
 // Read sweeps run_expect makes for these terms (masks on physical index bits) on an unsharded 2^n state.
 uint32_t expect_sweep_count(uint32_t n, const std::vector<PauliTerm> &terms);
 

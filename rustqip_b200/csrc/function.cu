@@ -16,7 +16,8 @@
 // Index maps.  x(j) and d(f) are read from shared-memory chunk tables built per CTA: byte k of the physical index
 // gives its bits of x (5 tables of 256), byte k of f(x) gives its bits of d (4 tables of 256).
 //
-// Staged tile path (k_function_tile; plan in function.h).  Every out bit lies in the tile, so every partner does too.
+// Staged tile path (k_function_tile; plan in function.h, tile geometry of sweep.cuh).  Every out bit lies in the tile,
+// so every partner does too.
 // A CTA visits tiles in turn: the next tile is loaded with cp.async into the second buffer while the current one is
 // processed (as k_pauli_rot does).  A thread's elements e = t + threads k sit at fixed offsets off[k] in every tile, so
 // x = x(base) | x(off[k]): the CTA-uniform part costs five table reads per visit and the per-thread parts are computed
@@ -28,7 +29,7 @@
 // the thread with the highest bit of d clear in j swaps psi_j and psi_{j ^ d} with the phase.  Each pair has exactly
 // one owner, so the path is race-free in place, and every amplitude is read and written once.
 #include "function.h"
-#include "pauli_rot_dev.cuh"
+#include "sweep.cuh"
 
 #include <algorithm>
 #include <cstring>
@@ -37,24 +38,22 @@ namespace qipb200 {
 
 namespace {
 
-const uint32_t kFnL = 4;         // low index bits of a tile (runs of 16 amplitudes)
 const uint32_t kFnTileF64 = 11;  // T_max: 2^11 x 16 B = 32 KiB per tile buffer
 const uint32_t kFnTileF32 = 12;  // 2^12 x 8 B = 32 KiB
+static_assert(kFnTileF32 - kSweepL <= kSweepMaxHi && kFnTileF64 <= kFnTileF32,
+              "the high tile bits fit SweepTiles::hi_pos");
 const int kFnPer = 8;            // tile amplitudes per thread
 const int kFnPairThreads = 256;
 
 struct FnArgs {
   const uint32_t *f;   // f[x], or NULL (no out register)
   const double2 *cs;   // (cos, sin) of theta[x], or NULL (no phase)
-  uint64_t n_visits;   // tile path: tiles
+  SweepTiles geo;      // tile path (x_out = 0)
   uint32_t n;          // index bits of the state
   uint32_t xbytes;     // bytes of the index that hold in bits
   uint32_t n_out, fbytes;
-  uint32_t L, tb, n_vis;  // tile path: low bits, tile bits, visit-index bits
-  uint8_t xbit[40];       // physical index bit -> bit of x, or 0xFF
-  uint8_t dpos[32];       // bit i of f(x) -> index bit (pair path) or tile-local bit (tile path)
-  uint8_t hi_pos[kFnTileF32];  // tile path: the tile bits above L, increasing
-  uint8_t vis_pos[40];         // tile path: the index bits of the visit number, increasing
+  uint8_t xbit[40];    // physical index bit -> bit of x, or 0xFF
+  uint8_t dpos[32];    // bit i of f(x) -> index bit (pair path) or tile-local bit (tile path)
 };
 
 struct FnTables {
@@ -139,29 +138,19 @@ struct FnTile<float> {
 template <typename R, bool THETA>
 __global__ void __launch_bounds__((1 << FnTile<R>::kBits) / kFnPer, 2)
     k_function_tile(R *__restrict__ psi, const __grid_constant__ FnArgs a) {
-  typedef typename RotV<R>::type V;
+  typedef typename SweepV<R>::type V;
   constexpr int kTile = 1 << FnTile<R>::kBits, kThreads = kTile / kFnPer;
   extern __shared__ __align__(16) unsigned char smem[];
   V *tiles = reinterpret_cast<V *>(smem);  // [2][kTile]: double buffer
   FnTables *T = reinterpret_cast<FnTables *>(smem + 2 * kTile * sizeof(V));
   build_tables(T, a);
   const int t = threadIdx.x;
-  const uint32_t tsize = 1u << a.tb;  // below kTile only when the whole state is one tile
+  const uint32_t tsize = 1u << a.geo.tb;  // below kTile only when the whole state is one tile
   uint64_t off[kFnPer];
 #pragma unroll
-  for (int k = 0; k < kFnPer; ++k) {
-    const uint32_t e = t + kThreads * k;
-    uint64_t o = e & ((1u << a.L) - 1);
-    for (uint32_t i = 0; i < a.tb - a.L; ++i) o |= (uint64_t)((e >> (a.L + i)) & 1u) << a.hi_pos[i];
-    off[k] = o;
-  }
-  auto base_of = [&](uint64_t v) {
-    uint64_t b = 0;
-    for (uint32_t i = 0; i < a.n_vis; ++i) b |= ((v >> i) & 1ull) << a.vis_pos[i];
-    return b;
-  };
+  for (int k = 0; k < kFnPer; ++k) off[k] = tile_offset(a.geo, t + kThreads * k);
   auto issue = [&](uint64_t v, V *dst) {
-    const uint64_t b = base_of(v);
+    const uint64_t b = visit_base(a.geo, v);
 #pragma unroll
     for (int k = 0; k < kFnPer; ++k) {
       const uint32_t e = t + kThreads * k;
@@ -169,16 +158,16 @@ __global__ void __launch_bounds__((1 << FnTile<R>::kBits) / kFnPer, 2)
     }
   };
   uint64_t v = blockIdx.x;
-  if (v < a.n_visits) issue(v, tiles);
+  if (v < a.geo.n_visits) issue(v, tiles);
   cp_async_commit();
   __syncthreads();  // the tables
   uint32_t xo[kFnPer];
 #pragma unroll
   for (int k = 0; k < kFnPer; ++k) xo[k] = x_of(*T, off[k], a.xbytes);
   int cur = 0;
-  for (; v < a.n_visits; v += gridDim.x) {
+  for (; v < a.geo.n_visits; v += gridDim.x) {
     // the visit's table entries first: their L2 latency overlaps the wait for the tile
-    const uint64_t b = base_of(v);
+    const uint64_t b = visit_base(a.geo, v);
     const uint32_t xb = x_of(*T, b, a.xbytes);
     uint32_t de[kFnPer];
     V w[kFnPer];
@@ -190,7 +179,7 @@ __global__ void __launch_bounds__((1 << FnTile<R>::kBits) / kFnPer, 2)
       if (THETA && mine) w[k] = fn_cs<R, V>(a.cs, x);
     }
     const uint64_t nv = v + gridDim.x;  // the next tile into the other buffer, then wait for the current one only
-    if (nv < a.n_visits) issue(nv, tiles + (cur ^ 1) * kTile);
+    if (nv < a.geo.n_visits) issue(nv, tiles + (cur ^ 1) * kTile);
     cp_async_commit();
     cp_async_wait<1>();
     __syncthreads();
@@ -209,7 +198,7 @@ __global__ void __launch_bounds__((1 << FnTile<R>::kBits) / kFnPer, 2)
 
 template <typename R, bool THETA>
 __global__ void __launch_bounds__(kFnPairThreads) k_function_pair(R *__restrict__ psi, const __grid_constant__ FnArgs a) {
-  typedef typename RotV<R>::type V;
+  typedef typename SweepV<R>::type V;
   __shared__ FnTables T;
   build_tables(&T, a);
   __syncthreads();
@@ -230,7 +219,7 @@ __global__ void __launch_bounds__(kFnPairThreads) k_function_pair(R *__restrict_
 
 template <typename R, bool THETA>
 cudaError_t launch_tile(void *psi, const FnArgs &a, int sm_count, cudaStream_t s) {
-  typedef typename RotV<R>::type V;
+  typedef typename SweepV<R>::type V;
   constexpr int kTile = 1 << FnTile<R>::kBits, kThreads = kTile / kFnPer;
   const size_t smem = 2 * kTile * sizeof(V) + sizeof(FnTables);
   static_assert(2 * (1 << kFnTileF64) * sizeof(double2) + sizeof(FnTables) <= 113 * 1024,
@@ -238,7 +227,7 @@ cudaError_t launch_tile(void *psi, const FnArgs &a, int sm_count, cudaStream_t s
   cudaError_t e = cudaFuncSetAttribute(k_function_tile<R, THETA>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        (int)smem);
   if (e != cudaSuccess) return e;
-  const int grid = (int)std::min<uint64_t>(a.n_visits, (uint64_t)std::max(2 * sm_count, 1));
+  const int grid = (int)std::min<uint64_t>(a.geo.n_visits, (uint64_t)std::max(2 * sm_count, 1));
   k_function_tile<R, THETA><<<grid, kThreads, smem, s>>>((R *)psi, a);
   return cudaGetLastError();
 }
@@ -254,7 +243,7 @@ cudaError_t launch_pair(void *psi, const FnArgs &a, int sm_count, cudaStream_t s
 }  // namespace
 
 FnPlan plan_function(qip_prec prec, uint32_t n, const uint32_t *out_pos, uint32_t n_out) {
-  const uint32_t L = std::min(kFnL, n), T = std::min(prec == QIP_F32 ? kFnTileF32 : kFnTileF64, n);
+  const uint32_t L = std::min(kSweepL, n), T = std::min(prec == QIP_F32 ? kFnTileF32 : kFnTileF64, n);
   FnPlan p;
   for (uint32_t i = 0; i < n_out; ++i)
     if (out_pos[i] >= L) p.hi |= 1ull << out_pos[i];
@@ -289,22 +278,8 @@ cudaError_t run_function(qip_prec prec, void *psi, uint32_t n, const uint32_t *i
   if (p.path == 1) {
     for (uint32_t i = 0; i < n_out; ++i) a.dpos[i] = (uint8_t)out_pos[i];
   } else {
-    a.L = std::min(kFnL, n);
-    a.tb = p.tile_bits;
-    uint32_t h = 0;
-    uint8_t tile_of[64];
-    for (uint32_t b = 0; b < n; ++b) {
-      if (b < a.L) {
-        tile_of[b] = (uint8_t)b;
-      } else if ((p.hi >> b) & 1) {
-        tile_of[b] = (uint8_t)(a.L + h);
-        a.hi_pos[h++] = (uint8_t)b;
-      } else {
-        a.vis_pos[a.n_vis++] = (uint8_t)b;
-      }
-    }
-    for (uint32_t i = 0; i < n_out; ++i) a.dpos[i] = tile_of[out_pos[i]];
-    a.n_visits = 1ull << a.n_vis;
+    a.geo = sweep_tiles(n, std::min(kSweepL, n), p.hi, 0);
+    for (uint32_t i = 0; i < n_out; ++i) a.dpos[i] = (uint8_t)__builtin_ctz(tile_local(a.geo, 1ull << out_pos[i]));
   }
   cudaError_t e;
   const bool th = cs != nullptr;

@@ -4,7 +4,7 @@
 // Path plan (the policy qipb200_function_plan reports), on physical index bits.  With L = min(4, n) low bits and
 // T = min(T_max, n), T_max = 11 for f64 and 12 for f32 (one tile buffer is 32 KiB either way):
 //   - staged tile path when L + |{out bits >= L}| <= T: the tile is the L low bits, the out bits above them, and the
-//     lowest free bits from L up until it has T bits (as rot_sweep_fill fills a Pauli-rotation tile);
+//     lowest free bits from L up until it has T bits (as sweep_fill fills a Pauli-rotation tile);
 //   - pair path otherwise.
 // So an op without output qubits (phase only) always takes the tile path.
 #pragma once

@@ -2,9 +2,9 @@
 // adjoint-method gradient of E = <psi0|U^dagger H U|psi0> for U = R_{T-1} ... R_0, R_t = exp(-i theta_t/2 P_t)
 // (qipb200_state_pauli_energy_gradient).  Planner policies: gradient.h.
 //
-// Geometry.  Both kernels stage two states per CTA, so their tile is the kRotL = 4 lowest index bits plus up to
-// kGradM = 6 chosen high bits: 2^10 amplitudes, four per thread of 256.  One tile or tile pair of each of two states is
-// 64 KiB at f64 (four 16 KiB tiles), which keeps two CTAs per SM at under 113 KiB each.
+// Geometry.  Both kernels stage two states per CTA, so their tile (sweep.cuh) is the kSweepL = 4 lowest index bits plus
+// up to kGradM = 6 chosen high bits: 2^10 amplitudes, four per thread of 256.  One tile or tile pair of each of two
+// states is 64 KiB at f64 (four 16 KiB tiles), which keeps two CTAs per SM at under 113 KiB each.
 //
 // k_pauli_sum.  (P src)_j = i^nY (-1)^popc(k & z) src_k with k = j ^ x, so the terms of one X/Y mask x (a group) share
 // src_k and differ by a real or imaginary sign: the group's coefficient at j is a + i b with
@@ -60,7 +60,7 @@
 // otherwise starts right after the staging barrier), and its pairs may belong to threads of other warps.  Per term the
 // 32 lanes of a warp reduce by butterfly shuffles and lane 0 adds into the warp's slot in shared memory (one slot per warp and row, visits in order); when the CTA has done its tiles it sums its 8 warp slots
 // in warp order into scratch[row][CTA], and k_adjoint_reduce sums each row over the CTAs in CTA order.  The grid is a
-// fixed kAdjGrid CTAs (or the visit count, when smaller): the same inputs give the same bits on any device.
+// fixed kGradGrid CTAs (or the visit count, when smaller): the same inputs give the same bits on any device.
 // A sweep holds at most kAdjMaxTerms terms so the slots fit shared memory: 64 KiB of tiles, 8 x 257 slots and the
 // staged descriptors, at most 91 KiB per CTA.
 //
@@ -95,7 +95,6 @@
 #include <algorithm>
 #include <cmath>
 #include <cstring>
-#include <map>
 
 #include "../../include/qipb200.h"
 #include "pauli_rot.h"
@@ -106,14 +105,14 @@ namespace qipb200 {
 namespace {
 
 const uint32_t kGradM = 6;
-const uint32_t kGradTile = 1u << (kRotL + kGradM);
+static_assert(kGradM <= kSweepMaxHi, "the high tile bits fit SweepTiles::hi_pos");
+const uint32_t kGradTile = 1u << (kSweepL + kGradM);
 const int kGradThreads = 256;
 const int kGradPer = kGradTile / kGradThreads;  // tile amplitudes per thread
 const int kGradWarps = kGradThreads / 32;
 const uint32_t kAdjMaxTerms = 256;       // terms of one backward sweep
 const uint32_t kAdjRows = kAdjMaxTerms + 1;  // + the energy
 const uint32_t kQgtRows = 2 * kAdjMaxTerms;  // complex rows: Re and Im per term
-const int kAdjGrid = 264;
 const int kForkThreads = 256;
 const int kForkWarps = kForkThreads / 32;
 const int kForkUnroll = 2;   // amplitude pairs per thread in flight
@@ -162,30 +161,20 @@ __global__ void __launch_bounds__(kGradThreads, 2)
     k_pauli_sum(R *__restrict__ dst, const R *__restrict__ src, const __grid_constant__ RotArgs a,
                 const SumGroupDev *__restrict__ groups, const SumTermDev *__restrict__ terms, uint32_t accumulate,
                 const __grid_constant__ EvoSweep ev) {
-  typedef typename RotV<R>::type V;
+  typedef typename SweepV<R>::type V;
   extern __shared__ __align__(16) unsigned char smem[];
   // single tiles: [buffer][src, from] double-buffered; pairs: src A, src B, from A, from B
   V *tiles = reinterpret_cast<V *>(smem);
   const int t = threadIdx.x;
-  const uint32_t tsize = 1u << a.tb;
+  const uint32_t tsize = 1u << a.geo.tb;
   // where the accumulator starts: the stored partial (dst) or, in the first sweep of a Chebyshev step, T_(k-1)
   const R *from = EVO ? (const R *)ev.from : dst;
   const bool load = EVO ? ev.from != nullptr : accumulate != 0;
   uint64_t off[kGradPer];
 #pragma unroll
-  for (int k = 0; k < kGradPer; ++k) {
-    const uint32_t e = t + kGradThreads * k;
-    uint64_t o = e & ((1u << a.L) - 1);
-    for (uint32_t i = 0; i < a.tb - a.L; ++i) o |= (uint64_t)((e >> (a.L + i)) & 1u) << a.hi_pos[i];
-    off[k] = o;
-  }
-  auto base_of = [&](uint64_t v) {
-    uint64_t b = 0;
-    for (uint32_t i = 0; i < a.n_out; ++i) b |= ((v >> i) & 1ull) << a.out_pos[i];
-    return b;
-  };
+  for (int k = 0; k < kGradPer; ++k) off[k] = tile_offset(a.geo, t + kGradThreads * k);
   auto issue = [&](uint64_t v, V *S, V *D, V *S2, V *D2) {  // S2, D2: the pair's B tiles
-    const uint64_t b = base_of(v);
+    const uint64_t b = visit_base(a.geo, v);
 #pragma unroll
     for (int k = 0; k < kGradPer; ++k) {
       const uint32_t e = t + kGradThreads * k;
@@ -193,19 +182,19 @@ __global__ void __launch_bounds__(kGradThreads, 2)
       cp_async<sizeof(V)>(S + e, src + 2 * (b | off[k]));
       if (load) cp_async<sizeof(V)>(D + e, from + 2 * (b | off[k]));
       if (PAIR) {
-        cp_async<sizeof(V)>(S2 + e, src + 2 * ((b ^ a.x_out) | off[k]));
-        if (load) cp_async<sizeof(V)>(D2 + e, from + 2 * ((b ^ a.x_out) | off[k]));
+        cp_async<sizeof(V)>(S2 + e, src + 2 * ((b ^ a.geo.x_out) | off[k]));
+        if (load) cp_async<sizeof(V)>(D2 + e, from + 2 * ((b ^ a.geo.x_out) | off[k]));
       }
     }
   };
   uint64_t v = blockIdx.x;
   if (!PAIR) {
-    if (v < a.n_visits) issue(v, tiles, tiles + kGradTile, nullptr, nullptr);
+    if (v < a.geo.n_visits) issue(v, tiles, tiles + kGradTile, nullptr, nullptr);
     cp_async_commit();
   }
   int cur = 0;
   double dsum = 0.0;  // Lanczos: this thread's share of Re<src|dst>, over its amplitudes in visit order
-  for (; v < a.n_visits; v += gridDim.x) {
+  for (; v < a.geo.n_visits; v += gridDim.x) {
     V *sA, *sB, *dA, *dB;
     if (PAIR) {
       sA = tiles;
@@ -221,12 +210,12 @@ __global__ void __launch_bounds__(kGradThreads, 2)
       sB = dB = nullptr;
       const uint64_t nv = v + gridDim.x;
       V *nS = tiles + (cur ^ 1) * 2 * kGradTile;
-      if (nv < a.n_visits) issue(nv, nS, nS + kGradTile, nullptr, nullptr);
+      if (nv < a.geo.n_visits) issue(nv, nS, nS + kGradTile, nullptr, nullptr);
       cp_async_commit();
       cp_async_wait<1>();
     }
     __syncthreads();
-    const uint64_t bA = base_of(v), bB = bA ^ a.x_out;
+    const uint64_t bA = visit_base(a.geo, v), bB = bA ^ a.geo.x_out;
 #pragma unroll 1
     for (int side = 0; side < (PAIR ? 2 : 1); ++side) {
       const V *own = side ? sB : sA, *other = side ? sA : sB;
@@ -339,7 +328,7 @@ template <typename R, bool PAIR, bool QGT>
 __global__ void __launch_bounds__(kGradThreads, 2)
     k_pauli_adjoint(R *__restrict__ phi, R *__restrict__ lam, const __grid_constant__ RotArgs a,
                     const RotTermDev *__restrict__ terms, uint32_t energy, double *__restrict__ scratch) {
-  typedef typename RotV<R>::type V;
+  typedef typename SweepV<R>::type V;
   constexpr uint32_t kRows = QGT ? kQgtRows : kAdjRows;
   extern __shared__ __align__(16) unsigned char smem[];
   // single tiles: [buffer][phi, lambda] double-buffered; pairs: phi A, phi B, lambda A, lambda B
@@ -351,22 +340,12 @@ __global__ void __launch_bounds__(kGradThreads, 2)
   const uint32_t rows = QGT ? 2 * a.n_terms : a.n_terms + (energy ? 1u : 0u);
   for (uint32_t i = t; i < a.n_terms; i += kGradThreads) sT[i] = terms[i];
   for (uint32_t i = t; i < kGradWarps * kRows; i += kGradThreads) red[i] = 0.0;  // ordered by the loop's barrier
-  const uint32_t tsize = 1u << a.tb;
+  const uint32_t tsize = 1u << a.geo.tb;
   uint64_t off[kGradPer];
 #pragma unroll
-  for (int k = 0; k < kGradPer; ++k) {
-    const uint32_t e = t + kGradThreads * k;
-    uint64_t o = e & ((1u << a.L) - 1);
-    for (uint32_t i = 0; i < a.tb - a.L; ++i) o |= (uint64_t)((e >> (a.L + i)) & 1u) << a.hi_pos[i];
-    off[k] = o;
-  }
-  auto base_of = [&](uint64_t v) {
-    uint64_t b = 0;
-    for (uint32_t i = 0; i < a.n_out; ++i) b |= ((v >> i) & 1ull) << a.out_pos[i];
-    return b;
-  };
+  for (int k = 0; k < kGradPer; ++k) off[k] = tile_offset(a.geo, t + kGradThreads * k);
   auto issue = [&](uint64_t v, V *P, V *Lm, V *P2, V *L2) {  // P2, L2: the pair's B tiles
-    const uint64_t b = base_of(v);
+    const uint64_t b = visit_base(a.geo, v);
 #pragma unroll
     for (int k = 0; k < kGradPer; ++k) {
       const uint32_t e = t + kGradThreads * k;
@@ -374,18 +353,18 @@ __global__ void __launch_bounds__(kGradThreads, 2)
       cp_async<sizeof(V)>(P + e, phi + 2 * (b | off[k]));
       cp_async<sizeof(V)>(Lm + e, lam + 2 * (b | off[k]));
       if (PAIR) {
-        cp_async<sizeof(V)>(P2 + e, phi + 2 * ((b ^ a.x_out) | off[k]));
-        cp_async<sizeof(V)>(L2 + e, lam + 2 * ((b ^ a.x_out) | off[k]));
+        cp_async<sizeof(V)>(P2 + e, phi + 2 * ((b ^ a.geo.x_out) | off[k]));
+        cp_async<sizeof(V)>(L2 + e, lam + 2 * ((b ^ a.geo.x_out) | off[k]));
       }
     }
   };
   uint64_t v = blockIdx.x;
   if (!PAIR) {
-    if (v < a.n_visits) issue(v, tiles, tiles + kGradTile, nullptr, nullptr);
+    if (v < a.geo.n_visits) issue(v, tiles, tiles + kGradTile, nullptr, nullptr);
     cp_async_commit();
   }
   int cur = 0;
-  for (; v < a.n_visits; v += gridDim.x) {
+  for (; v < a.geo.n_visits; v += gridDim.x) {
     V *pA, *pB, *lA, *lB;
     if (PAIR) {
       pA = tiles;
@@ -401,12 +380,12 @@ __global__ void __launch_bounds__(kGradThreads, 2)
       pB = lB = nullptr;
       const uint64_t nv = v + gridDim.x;
       V *nP = tiles + (cur ^ 1) * 2 * kGradTile;
-      if (nv < a.n_visits) issue(nv, nP, nP + kGradTile, nullptr, nullptr);
+      if (nv < a.geo.n_visits) issue(nv, nP, nP + kGradTile, nullptr, nullptr);
       cp_async_commit();
       cp_async_wait<1>();
     }
     __syncthreads();
-    const uint64_t bA = base_of(v), bB = bA ^ a.x_out;
+    const uint64_t bA = visit_base(a.geo, v), bB = bA ^ a.geo.x_out;
     if (!QGT && energy) {  // Re<lambda|phi> on the thread's own elements, before any term is undone
       double g = 0.0;
       for (int side = 0; side < (PAIR ? 2 : 1); ++side) {
@@ -607,7 +586,7 @@ template <typename R>
 __global__ void __launch_bounds__(kForkThreads, 4)
     k_qgt_fork(R *__restrict__ state, R *__restrict__ wa, R *__restrict__ wb, const __grid_constant__ ForkArgs f,
                double *__restrict__ scratch) {
-  typedef typename RotV<R>::type V;
+  typedef typename SweepV<R>::type V;
   V *S = reinterpret_cast<V *>(state), *A = reinterpret_cast<V *>(wa), *B = reinterpret_cast<V *>(wb);
   const uint32_t ph = (f.ny + 3) & 3;  // w = -i (P psi) = i^ph (+-1) psi_partner, as the rotation descriptors say
   const bool swap = ph & 1;
@@ -677,32 +656,17 @@ __global__ void __launch_bounds__(kForkThreads, 4)
 
 // ---- host ----------------------------------------------------------------------------------------------------------
 
-struct SumGroup {
-  uint64_t x = 0;
-  std::vector<uint32_t> terms;
-};
-
 struct SumSweep {
   RotSweep geo;
   std::vector<uint32_t> groups;  // indices into the group list, in order
 };
 
-void plan_sum(uint32_t n, const std::vector<PauliTerm> &terms, std::vector<SumGroup> *groups_out,
+void plan_sum(uint32_t n, const std::vector<PauliTerm> &terms, std::vector<PauliGroup> *groups_out,
               std::vector<SumSweep> *out) {
-  const uint32_t L = std::min(kRotL, n), m = std::min(kGradM, n - L);
+  const uint32_t L = std::min(kSweepL, n), m = std::min(kGradM, n - L);
   const uint64_t low = (1ull << L) - 1;
-  std::vector<SumGroup> &gr = *groups_out;
-  gr.clear();
-  std::map<uint64_t, size_t> where;
-  for (uint32_t t = 0; t < (uint32_t)terms.size(); ++t) {
-    auto it = where.find(terms[t].x);
-    if (it == where.end()) {
-      it = where.emplace(terms[t].x, gr.size()).first;
-      gr.push_back(SumGroup());
-      gr.back().x = terms[t].x;
-    }
-    gr[it->second].terms.push_back(t);
-  }
+  std::vector<PauliGroup> &gr = *groups_out;
+  gr = group_by_x(terms);
   std::vector<SumSweep> &sw = *out;
   sw.clear();
   std::vector<bool> used(gr.size(), false);
@@ -717,7 +681,7 @@ void plan_sum(uint32_t n, const std::vector<PauliTerm> &terms, std::vector<SumGr
       }
     sw.push_back(S);
   }
-  for (SumSweep &S : sw) rot_sweep_fill(&S.geo, n, L, m);
+  for (SumSweep &S : sw) sweep_fill(&S.geo.hi, &S.geo.x_out, n, L, m);
 }
 
 // The walk of pauli_rot.h's planner with kGradM high tile bits over `terms`, a sweep cut after every kAdjMaxTerms
@@ -738,9 +702,9 @@ void plan_walk(uint32_t n, const std::vector<PauliTerm> &terms, std::vector<RotS
 void plan_adjoint(uint32_t n, const std::vector<PauliTerm> &rev, std::vector<RotSweep> *out) {
   plan_walk(n, rev, out);
   if (out->empty()) {  // no terms: one sweep for the energy, on the tile of the lowest bits
-    const uint32_t L = std::min(kRotL, n), m = std::min(kGradM, n - L);
+    const uint32_t L = std::min(kSweepL, n), m = std::min(kGradM, n - L);
     RotSweep S;
-    rot_sweep_fill(&S, n, L, m);
+    sweep_fill(&S.hi, &S.x_out, n, L, m);
     out->push_back(S);
   }
 }
@@ -748,13 +712,13 @@ void plan_adjoint(uint32_t n, const std::vector<PauliTerm> &rev, std::vector<Rot
 template <typename R, bool PAIR, bool EVO>
 cudaError_t launch_sum(void *dst, const void *src, const RotArgs &a, const SumGroupDev *g, const SumTermDev *t,
                        uint32_t accumulate, const EvoSweep &ev, cudaStream_t s) {
-  typedef typename RotV<R>::type V;
+  typedef typename SweepV<R>::type V;
   static_assert(4 * kGradTile * sizeof(double2) <= 113 * 1024, "two CTAs per SM: at most 113 KiB of shared memory each");
   const size_t smem = 4 * kGradTile * sizeof(V);
   cudaError_t e =
       cudaFuncSetAttribute(k_pauli_sum<R, PAIR, EVO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  const int grid = (int)std::min<uint64_t>(a.n_visits, (uint64_t)kAdjGrid);
+  const int grid = (int)std::min<uint64_t>(a.geo.n_visits, (uint64_t)kGradGrid);
   k_pauli_sum<R, PAIR, EVO><<<grid, kGradThreads, smem, s>>>((R *)dst, (const R *)src, a, g, t, accumulate, ev);
   return cudaGetLastError();
 }
@@ -763,10 +727,10 @@ template <bool EVO>
 cudaError_t launch_sum_any(qip_prec prec, void *dst, const void *src, const RotArgs &a, const SumGroupDev *g,
                            const SumTermDev *t, uint32_t accumulate, const EvoSweep &ev, cudaStream_t s) {
   if (prec == QIP_F32)
-    return a.x_out ? launch_sum<float, true, EVO>(dst, src, a, g, t, accumulate, ev, s)
-                   : launch_sum<float, false, EVO>(dst, src, a, g, t, accumulate, ev, s);
-  return a.x_out ? launch_sum<double, true, EVO>(dst, src, a, g, t, accumulate, ev, s)
-                 : launch_sum<double, false, EVO>(dst, src, a, g, t, accumulate, ev, s);
+    return a.geo.x_out ? launch_sum<float, true, EVO>(dst, src, a, g, t, accumulate, ev, s)
+                       : launch_sum<float, false, EVO>(dst, src, a, g, t, accumulate, ev, s);
+  return a.geo.x_out ? launch_sum<double, true, EVO>(dst, src, a, g, t, accumulate, ev, s)
+                     : launch_sum<double, false, EVO>(dst, src, a, g, t, accumulate, ev, s);
 }
 
 // The device tables of plan_sum: args[k] (n_terms = its group count) and the groups of sweep k from (*hg)[(*g_off)[k]]
@@ -775,10 +739,10 @@ cudaError_t launch_sum_any(qip_prec prec, void *dst, const void *src, const RotA
 bool build_sum_tables(uint32_t n, const std::vector<PauliTerm> &terms, const double *coeffs, double scale,
                       std::vector<RotArgs> *args, std::vector<SumGroupDev> *hg, std::vector<SumTermDev> *ht,
                       std::vector<size_t> *g_off) {
-  std::vector<SumGroup> gr;
+  std::vector<PauliGroup> gr;
   std::vector<SumSweep> sw;
   plan_sum(n, terms, &gr, &sw);
-  const uint32_t L = std::min(kRotL, n);
+  const uint32_t L = std::min(kSweepL, n);
   const uint64_t low = (1ull << L) - 1;
   args->assign(sw.size(), RotArgs());
   g_off->assign(sw.size(), 0);
@@ -788,24 +752,23 @@ bool build_sum_tables(uint32_t n, const std::vector<PauliTerm> &terms, const dou
     const SumSweep &S = sw[k];
     RotArgs &a = (*args)[k];
     memset(&a, 0, sizeof(a));
-    std::vector<uint32_t> hi_pos;
-    rot_geometry(n, L, S.geo.hi, S.geo.x_out, &a, &hi_pos);
+    a.geo = sweep_tiles(n, L, S.geo.hi, S.geo.x_out);
     const uint64_t tile = low | S.geo.hi;
     a.n_terms = (uint32_t)S.groups.size();  // groups, for this kernel
     (*g_off)[k] = hg->size();
     for (uint32_t gi : S.groups) {
-      const SumGroup &G = gr[gi];
+      const PauliGroup &G = gr[gi];
       const uint64_t xo = G.x & ~tile;
       if (xo != 0 && xo != S.geo.x_out) return false;
       SumGroupDev gd;
-      gd.x_in = compact_tile_bits(G.x & tile, L, hi_pos);
+      gd.x_in = tile_local(a.geo, G.x & tile);
       gd.pair = xo ? 1u : 0u;
       gd.first = (uint32_t)ht->size();
       for (uint32_t t : G.terms) {
         const PauliTerm &P = terms[t];
         SumTermDev td;
         td.z_out = P.z & ~tile;
-        td.z_in = compact_tile_bits(P.z & tile, L, hi_pos);
+        td.z_in = tile_local(a.geo, P.z & tile);
         td.odd = P.n_y & 1;
         const double c = scale * coeffs[t];
         td.c = ((P.n_y & 3) >= 2) ? -c : c;  // i^nY = 1, i, -1, -i
@@ -821,7 +784,7 @@ bool build_sum_tables(uint32_t n, const std::vector<PauliTerm> &terms, const dou
 template <typename R, bool PAIR, bool QGT>
 cudaError_t launch_adjoint(void *phi, void *lam, const RotArgs &a, const RotTermDev *terms, uint32_t energy,
                            double *scratch, int grid, cudaStream_t s) {
-  typedef typename RotV<R>::type V;
+  typedef typename SweepV<R>::type V;
   static_assert(kGradThreads == 256 && kGradPer == 4, "the diagonal path's sign table assumes e = t + 256 k, k < 4");
   const size_t fixed = 4 * kGradTile * sizeof(V) + kGradWarps * (QGT ? kQgtRows : kAdjRows) * sizeof(double);
   static_assert(4 * kGradTile * sizeof(double2) + kGradWarps * kAdjRows * sizeof(double) +
@@ -842,10 +805,10 @@ template <bool QGT>
 cudaError_t launch_adjoint_any(qip_prec prec, void *phi, void *lam, const RotArgs &a, const RotTermDev *terms,
                                uint32_t energy, double *scratch, int grid, cudaStream_t s) {
   if (prec == QIP_F32)
-    return a.x_out ? launch_adjoint<float, true, QGT>(phi, lam, a, terms, energy, scratch, grid, s)
-                   : launch_adjoint<float, false, QGT>(phi, lam, a, terms, energy, scratch, grid, s);
-  return a.x_out ? launch_adjoint<double, true, QGT>(phi, lam, a, terms, energy, scratch, grid, s)
-                 : launch_adjoint<double, false, QGT>(phi, lam, a, terms, energy, scratch, grid, s);
+    return a.geo.x_out ? launch_adjoint<float, true, QGT>(phi, lam, a, terms, energy, scratch, grid, s)
+                       : launch_adjoint<float, false, QGT>(phi, lam, a, terms, energy, scratch, grid, s);
+  return a.geo.x_out ? launch_adjoint<double, true, QGT>(phi, lam, a, terms, energy, scratch, grid, s)
+                     : launch_adjoint<double, false, QGT>(phi, lam, a, terms, energy, scratch, grid, s);
 }
 
 // The segments of the geometric tensor: for fork i, the walk over terms i + 1 .. T - 1 (sw[i]).
@@ -858,7 +821,7 @@ void plan_segments(uint32_t n, const std::vector<PauliTerm> &ansatz, std::vector
 }  // namespace
 
 uint32_t pauli_sum_sweep_count(uint32_t n, const std::vector<PauliTerm> &terms) {
-  std::vector<SumGroup> gr;
+  std::vector<PauliGroup> gr;
   std::vector<SumSweep> sw;
   plan_sum(n, terms, &gr, &sw);
   return (uint32_t)sw.size();
@@ -968,7 +931,7 @@ cudaError_t run_lanczos_sum(qip_prec prec, void *dst, const void *src, const voi
     e = launch_sum_any<true>(prec, dst, src, args[j], dg + g_off[j], dt, 0, ev, s);
     ++*launches;
   }
-  *dot_grid = (uint32_t)std::min<uint64_t>(args.back().n_visits, (uint64_t)kAdjGrid);
+  *dot_grid = (uint32_t)std::min<uint64_t>(args.back().geo.n_visits, (uint64_t)kGradGrid);
   const cudaError_t ef = cudaFreeAsync(d, s);
   return e != cudaSuccess ? e : ef;
 }
@@ -989,7 +952,7 @@ cudaError_t run_pauli_gradient(qip_prec prec, void *state, void *work, uint32_t 
   std::vector<RotTermDev> ht;
   if (!build_rot_tables(prec, n, rev, rev_angles.data(), true, sw, &args, &ht)) return cudaErrorInvalidValue;
   const size_t tbytes = std::max<size_t>(1, ht.size()) * sizeof(RotTermDev);
-  const size_t sbytes = (size_t)kAdjRows * kAdjGrid * sizeof(double), rbytes = (T + 1) * sizeof(double);
+  const size_t sbytes = (size_t)kAdjRows * kGradGrid * sizeof(double), rbytes = (T + 1) * sizeof(double);
   char *d = nullptr;
   e = cudaMallocAsync((void **)&d, tbytes + sbytes + rbytes, s);
   if (e != cudaSuccess) return e;
@@ -999,7 +962,7 @@ cudaError_t run_pauli_gradient(qip_prec prec, void *state, void *work, uint32_t 
   if (!ht.empty()) e = cudaMemcpyAsync(dt, ht.data(), ht.size() * sizeof(RotTermDev), cudaMemcpyHostToDevice, s);
   for (size_t k = 0; k < sw.size() && e == cudaSuccess; ++k) {
     RotArgs &a = args[k];
-    const uint32_t en = k == 0, g = (uint32_t)std::min<uint64_t>(a.n_visits, (uint64_t)kAdjGrid);
+    const uint32_t en = k == 0, g = (uint32_t)std::min<uint64_t>(a.geo.n_visits, (uint64_t)kGradGrid);
     const RotTermDev *td = dt + sw[k].first;
     e = launch_adjoint_any<false>(prec, state, work, a, td, en, scratch, g, s);
     ++*launches;
@@ -1054,7 +1017,7 @@ cudaError_t run_pauli_qgt(qip_prec prec, void *state, void *work_a, void *work_b
   // one fork grid per call, so that every fork's two rows reduce over the same CTAs at the end
   const uint32_t gf = (uint32_t)std::min<uint64_t>(kForkGrid, std::max<uint64_t>(1, (1ull << (n - 1)) / kForkThreads));
   const size_t tbytes = std::max<size_t>(1, ht.size()) * sizeof(RotTermDev);
-  const size_t sbytes = (size_t)kQgtRows * kAdjGrid * sizeof(double);
+  const size_t sbytes = (size_t)kQgtRows * kGradGrid * sizeof(double);
   const size_t fbytes = (size_t)2 * T * gf * sizeof(double);
   const size_t rcount = (size_t)2 * T * T + 2 * T, rbytes = rcount * sizeof(double);
   char *d = nullptr;
@@ -1090,7 +1053,7 @@ cudaError_t run_pauli_qgt(qip_prec prec, void *state, void *work_a, void *work_b
     ++*launches;
     for (size_t k = 0; k < sw[i].size() && e == cudaSuccess; ++k) {
       const RotArgs &a = args[a_off[i] + k];
-      const uint32_t g = (uint32_t)std::min<uint64_t>(a.n_visits, (uint64_t)kAdjGrid);
+      const uint32_t g = (uint32_t)std::min<uint64_t>(a.geo.n_visits, (uint64_t)kGradGrid);
       e = launch_adjoint_any<true>(prec, work_a, work_b, a, dt + t_off[i] + sw[i][k].first, 0, scratch, g, s);
       ++*launches;
       if (e != cudaSuccess) break;

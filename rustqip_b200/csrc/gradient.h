@@ -27,6 +27,10 @@
 
 namespace qipb200 {
 
+// CTAs of a sum or adjoint sweep (fewer when it has fewer visits): two per SM of a 132-SM H100.  A fixed grid, so the
+// same inputs give the same bits on any device.
+const int kGradGrid = 264;
+
 // Read-write sweeps run_pauli_sum makes for these terms (masks on physical index bits) on an unsharded 2^n state.
 uint32_t pauli_sum_sweep_count(uint32_t n, const std::vector<PauliTerm> &terms);
 

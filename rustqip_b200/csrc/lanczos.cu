@@ -58,7 +58,7 @@
 
 #include "../../include/qipb200.h"
 #include "gradient.h"
-#include "pauli_rot_dev.cuh"
+#include "sweep.cuh"
 
 namespace qipb200 {
 
@@ -68,7 +68,6 @@ const int kLanThreads = 256;
 const int kLanWarps = kLanThreads / 32;
 const uint64_t kLanGrid = 1056;  // 8 CTAs per SM of an H100 SXM
 const int kLanUnroll = 4;        // amplitudes in flight per thread
-const uint32_t kSumGrid = 264;   // the most CTAs a sum sweep uses (gradient.cu)
 
 enum VecMode { kVecNorm, kVecScale, kVecUpdate, kVecResid };
 
@@ -92,7 +91,7 @@ __device__ __forceinline__ double2 narrow_to(double2 a, double2 *) { return a; }
 
 template <typename R, int MODE>
 __global__ void __launch_bounds__(kLanThreads) k_lanczos_vec(const __grid_constant__ VecArgs a) {
-  typedef typename RotV<R>::type V;
+  typedef typename SweepV<R>::type V;
   __shared__ double wsum[3][kLanWarps];
   __shared__ double mu_s;
   const int t = threadIdx.x;
@@ -304,8 +303,8 @@ cudaError_t run_lanczos(qip_prec prec, void *state, void *work_a, void *work_b, 
                         LanczosResult *r) {
   const uint64_t N = 1ull << n;
   const uint32_t vgrid = (uint32_t)std::min<uint64_t>(kLanGrid, (N + kLanThreads - 1) / kLanThreads);
-  double *scratch = nullptr;  // [3][kLanGrid] vector-kernel rows, then kSumGrid dot partials
-  const size_t rows = 3 * kLanGrid + kSumGrid;
+  double *scratch = nullptr;  // [3][kLanGrid] vector-kernel rows, then kGradGrid dot partials
+  const size_t rows = 3 * kLanGrid + kGradGrid;
   cudaError_t e = cudaMallocAsync((void **)&scratch, rows * sizeof(double), s);
   if (e != cudaSuccess) return e;
   double *red = scratch, *dot = scratch + 3 * kLanGrid;

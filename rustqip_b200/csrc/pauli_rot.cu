@@ -10,13 +10,14 @@
 // rounded once from double on the host.  Amplitudes stay in the state's precision between terms, so the result does
 // not depend on how terms are grouped into sweeps, on the tile geometry or on the layout.
 //
-// Sweep = tile geometry + x_out (planner: pauli_rot.h).  A tile is the kRotL lowest index bits plus up to kRotM chosen
-// high bits (2^11 amplitudes, runs of 16 contiguous amplitudes).  Each term's X/Y mask splits as x = x_in ^ x_out with
-// x_in on tile bits and x_out either 0 or the one out-of-tile mask the sweep shares.  With x_out == 0 a CTA stages one
-// tile (double-buffered: the next tile loads with cp.async while the current one is rotated); otherwise it stages the
-// pair (B, B ^ x_out), visited from the side whose lowest x_out bit is clear.  Every amplitude belongs to exactly one
-// CTA visit per sweep, so the tiles are written back in place.  The CTA applies the sweep's terms in order on the staged
-// tile(s) and writes them back once.  Z/Y bits outside the tile give a CTA-uniform sign, popc(base & z_out).
+// Sweep = tile geometry + x_out (planner: pauli_rot.h).  A tile (sweep.cuh) is the kSweepL lowest index bits plus up to
+// kRotM chosen high bits (2^11 amplitudes, runs of 16 contiguous amplitudes).  Each term's X/Y mask splits as
+// x = x_in ^ x_out with x_in on tile bits and x_out either 0 or the one out-of-tile mask the sweep shares.  With
+// x_out == 0 a CTA stages one tile (double-buffered: the next tile loads with cp.async while the current one is
+// rotated); otherwise it stages the pair (B, B ^ x_out), visited from the side whose lowest x_out bit is clear.  Every
+// amplitude belongs to exactly one CTA visit per sweep, so the tiles are written back in place.  The CTA applies the
+// sweep's terms in order on the staged tile(s) and writes them back once.  Z/Y bits outside the tile give a CTA-uniform
+// sign, popc(base & z_out).
 //
 // Ownership: for a term with x_in != 0 on one tile a thread updates the pairs (e, e ^ x_in) it enumerates, for a term
 // that reaches the partner tile the pairs (A[e], B[e ^ x_in]) for its own e, for a diagonal term (x == 0) its own
@@ -39,7 +40,7 @@ namespace qipb200 {
 namespace {
 
 const uint32_t kRotM = 7;   // chosen high bits of a tile
-const uint32_t kRotTile = 1u << (kRotL + kRotM);
+const uint32_t kRotTile = 1u << (kSweepL + kRotM);
 const int kRotThreads = 256;
 const int kRotPer = kRotTile / kRotThreads;  // tile amplitudes per thread
 const uint32_t kRotSmemTerms = 256;          // descriptors staged in shared memory; later ones are read from global
@@ -64,58 +65,48 @@ __device__ __forceinline__ void rot_in_tile(V *X, uint64_t b, const RotTermDev &
 template <typename R, bool PAIR>
 __global__ void __launch_bounds__(kRotThreads, 2)
     k_pauli_rot(R *__restrict__ psi, const __grid_constant__ RotArgs a, const RotTermDev *__restrict__ terms) {
-  typedef typename RotV<R>::type V;
+  typedef typename SweepV<R>::type V;
   extern __shared__ __align__(16) unsigned char smem[];
   V *tiles = reinterpret_cast<V *>(smem);  // [2][kRotTile]: two buffers of one tile, or the tiles A and B of a pair
   RotTermDev *sT = reinterpret_cast<RotTermDev *>(smem + 2 * kRotTile * sizeof(V));
   const int t = threadIdx.x;
   const uint32_t n_smem = min(a.n_terms, kRotSmemTerms);
   for (uint32_t i = t; i < n_smem; i += kRotThreads) sT[i] = terms[i];  // ordered by the first barrier of the loop
-  const uint32_t tsize = 1u << a.tb;
+  const uint32_t tsize = 1u << a.geo.tb;
   uint64_t off[kRotPer];
 #pragma unroll
-  for (int k = 0; k < kRotPer; ++k) {
-    const uint32_t e = t + kRotThreads * k;
-    uint64_t o = e & ((1u << a.L) - 1);
-    for (uint32_t i = 0; i < a.tb - a.L; ++i) o |= (uint64_t)((e >> (a.L + i)) & 1u) << a.hi_pos[i];
-    off[k] = o;
-  }
-  auto base_of = [&](uint64_t v) {
-    uint64_t b = 0;
-    for (uint32_t i = 0; i < a.n_out; ++i) b |= ((v >> i) & 1ull) << a.out_pos[i];
-    return b;
-  };
+  for (int k = 0; k < kRotPer; ++k) off[k] = tile_offset(a.geo, t + kRotThreads * k);
   auto issue = [&](uint64_t v, V *dst) {
-    const uint64_t b = base_of(v);
+    const uint64_t b = visit_base(a.geo, v);
 #pragma unroll
     for (int k = 0; k < kRotPer; ++k) {
       const uint32_t e = t + kRotThreads * k;
       if (e >= tsize) continue;
       cp_async<sizeof(V)>(dst + e, psi + 2 * (b | off[k]));
-      if (PAIR) cp_async<sizeof(V)>(dst + kRotTile + e, psi + 2 * ((b ^ a.x_out) | off[k]));
+      if (PAIR) cp_async<sizeof(V)>(dst + kRotTile + e, psi + 2 * ((b ^ a.geo.x_out) | off[k]));
     }
   };
   uint64_t v = blockIdx.x;
   if (!PAIR) {
-    if (v < a.n_visits) issue(v, tiles);
+    if (v < a.geo.n_visits) issue(v, tiles);
     cp_async_commit();
   }
   int cur = 0;
-  for (; v < a.n_visits; v += gridDim.x) {
+  for (; v < a.geo.n_visits; v += gridDim.x) {
     if (PAIR) {
       issue(v, tiles);
       cp_async_commit();
       cp_async_wait<0>();
     } else {  // the next tile into the other buffer, then wait for the current one only
       const uint64_t nv = v + gridDim.x;
-      if (nv < a.n_visits) issue(nv, tiles + (cur ^ 1) * kRotTile);
+      if (nv < a.geo.n_visits) issue(nv, tiles + (cur ^ 1) * kRotTile);
       cp_async_commit();
       cp_async_wait<1>();
     }
     __syncthreads();
     V *A = tiles + (PAIR ? 0 : cur) * kRotTile;
     V *Bt = A + kRotTile;  // PAIR only
-    const uint64_t bA = base_of(v), bB = bA ^ a.x_out;
+    const uint64_t bA = visit_base(a.geo, v), bB = bA ^ a.geo.x_out;
     for (uint32_t i = 0; i < a.n_terms;) {
       const RotTermDev T = i < kRotSmemTerms ? sT[i] : terms[i];
       if (T.flags & kRotBarrier) __syncthreads();
@@ -193,7 +184,7 @@ __global__ void __launch_bounds__(kRotThreads, 2)
 
 template <typename R, bool PAIR>
 cudaError_t launch_rot(void *psi, const RotArgs &a, const RotTermDev *terms, int grid, cudaStream_t s) {
-  typedef typename RotV<R>::type V;
+  typedef typename SweepV<R>::type V;
   static_assert(kRotThreads == 256 && kRotPer == 8, "the diagonal path's sign table assumes e = t + 256 k, k < 8");
   static_assert(2 * kRotTile * sizeof(double2) + kRotSmemTerms * sizeof(RotTermDev) <= 113 * 1024,
                 "two CTAs per SM: at most 113 KiB of shared memory each");
@@ -223,17 +214,8 @@ bool rot_sweep_join(RotSweep *S, uint64_t x, uint64_t low, uint32_t m) {
   return false;
 }
 
-void rot_sweep_fill(RotSweep *S, uint32_t n, uint32_t L, uint32_t m) {
-  for (uint32_t b = 0; b < n && (uint32_t)__builtin_popcountll(S->hi) < m; ++b)
-    if ((S->x_out >> b) & 1) {
-      S->hi |= 1ull << b;
-      S->x_out &= ~(1ull << b);
-    }
-  for (uint32_t b = L; b < n && (uint32_t)__builtin_popcountll(S->hi) < m; ++b) S->hi |= 1ull << b;
-}
-
 void plan_rot_sweeps(uint32_t n, uint32_t m_max, const std::vector<PauliTerm> &terms, std::vector<RotSweep> *out) {
-  const uint32_t L = std::min(kRotL, n), m = std::min(m_max, n - L);
+  const uint32_t L = std::min(kSweepL, n), m = std::min(m_max, n - L);
   const uint64_t low = (1ull << L) - 1;
   std::vector<RotSweep> &sw = *out;
   sw.clear();
@@ -247,35 +229,13 @@ void plan_rot_sweeps(uint32_t n, uint32_t m_max, const std::vector<PauliTerm> &t
     rot_sweep_join(&sw.back(), terms[t].x, low, m);  // always joins an empty sweep
   }
   sw.back().end = (uint32_t)terms.size();
-  for (RotSweep &S : sw) rot_sweep_fill(&S, n, L, m);
-}
-
-uint32_t compact_tile_bits(uint64_t v, uint32_t L, const std::vector<uint32_t> &hi_pos) {
-  uint32_t r = (uint32_t)(v & ((1ull << L) - 1));
-  for (size_t i = 0; i < hi_pos.size(); ++i) r |= (uint32_t)((v >> hi_pos[i]) & 1ull) << (L + i);
-  return r;
-}
-
-void rot_geometry(uint32_t n, uint32_t L, uint64_t hi, uint64_t x_out, RotArgs *a, std::vector<uint32_t> *hi_pos) {
-  hi_pos->clear();
-  for (uint32_t b = 0; b < n; ++b)
-    if ((hi >> b) & 1) hi_pos->push_back(b);
-  const uint64_t tile = ((1ull << L) - 1) | hi;
-  a->x_out = x_out;
-  a->L = L;
-  a->tb = L + (uint32_t)hi_pos->size();
-  for (size_t i = 0; i < hi_pos->size(); ++i) a->hi_pos[i] = (uint8_t)(*hi_pos)[i];
-  const int pair_bit = x_out ? __builtin_ctzll(x_out) : -1;
-  a->n_out = 0;
-  for (uint32_t b = 0; b < n; ++b)
-    if (!((tile >> b) & 1) && (int)b != pair_bit) a->out_pos[a->n_out++] = (uint8_t)b;
-  a->n_visits = 1ull << a->n_out;
+  for (RotSweep &S : sw) sweep_fill(&S.hi, &S.x_out, n, L, m);
 }
 
 bool build_rot_tables(qip_prec prec, uint32_t n, const std::vector<PauliTerm> &terms, const double *angles,
                       bool negate_s, const std::vector<RotSweep> &sw, std::vector<RotArgs> *args_out,
                       std::vector<RotTermDev> *ht_out) {
-  const uint32_t L = std::min(kRotL, n);
+  const uint32_t L = std::min(kSweepL, n);
   const uint64_t low = (1ull << L) - 1;
   std::vector<RotArgs> &args = *args_out;
   std::vector<RotTermDev> &ht = *ht_out;
@@ -285,8 +245,7 @@ bool build_rot_tables(qip_prec prec, uint32_t n, const std::vector<PauliTerm> &t
     const RotSweep &S = sw[k];
     RotArgs &a = args[k];
     memset(&a, 0, sizeof(a));
-    std::vector<uint32_t> hi_pos;
-    rot_geometry(n, L, S.hi, S.x_out, &a, &hi_pos);
+    a.geo = sweep_tiles(n, L, S.hi, S.x_out);
     const uint64_t tile = low | S.hi;
     a.n_terms = S.end - S.first;
     uint64_t prev_key = ~0ull;  // ownership of the previous term: (x_in, pair), diagonal terms (0, 0)
@@ -297,8 +256,8 @@ bool build_rot_tables(qip_prec prec, uint32_t n, const std::vector<PauliTerm> &t
       const uint64_t xo = P.x & ~tile;
       if (xo != 0 && xo != S.x_out) return false;  // the planner's invariant
       d.z_out = P.z & ~tile;
-      d.x_in = compact_tile_bits(P.x & tile, L, hi_pos);
-      d.z_in = compact_tile_bits(P.z & tile, L, hi_pos);
+      d.x_in = tile_local(a.geo, P.x & tile);
+      d.z_in = tile_local(a.geo, P.z & tile);
       double c = cos(angles[t] / 2), sn = sin(angles[t] / 2);
       if (prec == QIP_F32) {
         c = (double)(float)c;
@@ -353,13 +312,14 @@ cudaError_t run_pauli_rotations(qip_prec prec, void *psi, uint32_t n, const std:
   // pageable source: the copy is staged before cudaMemcpyAsync returns, so ht may go when this function does
   e = cudaMemcpyAsync(d, ht.data(), ht.size() * sizeof(RotTermDev), cudaMemcpyHostToDevice, s);
   for (size_t k = 0; k < sw.size() && e == cudaSuccess; ++k) {
-    const int g = (int)std::min<uint64_t>(args[k].n_visits, (uint64_t)std::max(grid, 1));
+    const int g = (int)std::min<uint64_t>(args[k].geo.n_visits, (uint64_t)std::max(grid, 1));
     const RotTermDev *td = d + sw[k].first;
     if (prec == QIP_F32)
-      e = args[k].x_out ? launch_rot<float, true>(psi, args[k], td, g, s) : launch_rot<float, false>(psi, args[k], td, g, s);
+      e = args[k].geo.x_out ? launch_rot<float, true>(psi, args[k], td, g, s)
+                            : launch_rot<float, false>(psi, args[k], td, g, s);
     else
-      e = args[k].x_out ? launch_rot<double, true>(psi, args[k], td, g, s)
-                        : launch_rot<double, false>(psi, args[k], td, g, s);
+      e = args[k].geo.x_out ? launch_rot<double, true>(psi, args[k], td, g, s)
+                            : launch_rot<double, false>(psi, args[k], td, g, s);
     ++*launches;
   }
   const cudaError_t ef = cudaFreeAsync(d, s);

@@ -1,7 +1,7 @@
 // pauli_rot_dev.cuh -- what pauli_rot.cu (qipb200_state_apply_pauli_rotations) and gradient.cu (the adjoint
-// gradient and qipb200_state_apply_pauli_sum) share: the tile geometry and term descriptors of a sweep, the sweep
-// planner parameterised by the number of high tile bits, the descriptor builder and the device arithmetic of one
-// rotation.  See pauli_rot.cu for the arithmetic and pauli_rot.h for the planner policy.
+// gradient and qipb200_state_apply_pauli_sum) share: the term descriptors of a rotation sweep, the sweep planner
+// parameterised by the number of high tile bits, the descriptor builder and the device arithmetic of one rotation.  The
+// tile geometry is sweep.cuh's.  See pauli_rot.cu for the arithmetic and pauli_rot.h for the planner policy.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -11,11 +11,12 @@
 
 #include "../../include/qip_op.h"
 #include "expect.h"
+#include "sweep.cuh"
 
 namespace qipb200 {
 
-const uint32_t kRotL = 4;     // low index bits of a tile (runs of 16 amplitudes)
 const uint32_t kRotMaxM = 7;  // the most chosen high tile bits any sweep geometry uses
+static_assert(kRotMaxM <= kSweepMaxHi, "the high tile bits fit SweepTiles::hi_pos");
 
 enum : uint32_t {
   kRotPhase = 3u,     // w = i^phase (+-1) psi_partner
@@ -34,13 +35,8 @@ struct RotTermDev {
 };
 
 struct RotArgs {
-  uint64_t x_out;     // 0, or the out-of-tile X/Y mask shared by the sweep
-  uint64_t n_visits;  // tiles (x_out == 0) or tile pairs
-  uint32_t L, tb;     // low bits, tile bits
-  uint32_t n_out;     // bits of the visit index, spread over out_pos
+  SweepTiles geo;
   uint32_t n_terms;
-  uint8_t hi_pos[kRotMaxM];
-  uint8_t out_pos[64];
 };
 
 struct RotSweep {
@@ -55,19 +51,9 @@ struct RotSweep {
 // true when a term or group of X/Y mask x fits S, after growing S.hi or setting S.x_out as the rule says; false leaves S
 // as it was.
 bool rot_sweep_join(RotSweep *S, uint64_t x, uint64_t low, uint32_t m);
-// Fill the free high tile bits of a planned sweep up to m: first x_out bits (fewer tile pairs), then the lowest free
-// bits from L up (longer contiguous runs).
-void rot_sweep_fill(RotSweep *S, uint32_t n, uint32_t L, uint32_t m);
 
 // The policy of pauli_rot.h with at most m (<= kRotMaxM) chosen high tile bits: consecutive terms per sweep.
 void plan_rot_sweeps(uint32_t n, uint32_t m, const std::vector<PauliTerm> &terms, std::vector<RotSweep> *out);
-
-// Index bits of v on the tile (the L low bits, then hi_pos in order) packed into a tile-local index.
-uint32_t compact_tile_bits(uint64_t v, uint32_t L, const std::vector<uint32_t> &hi_pos);
-
-// The geometry of a sweep with tile bits low(L) | hi and out-of-tile mask x_out: a.L, a.tb, a.hi_pos, a.out_pos,
-// a.n_out, a.n_visits, a.x_out (a.n_terms untouched); hi_pos gets the chosen high bits in increasing order.
-void rot_geometry(uint32_t n, uint32_t L, uint64_t hi, uint64_t x_out, RotArgs *a, std::vector<uint32_t> *hi_pos);
 
 // Geometry and term descriptors of every sweep: args[k] for sw[k], ht[t] for terms[t].  c and s come from the host's
 // cos and sin of angles[t]/2, rounded once to the state's precision; negate_s stores -s (the inverse rotation).
@@ -79,24 +65,6 @@ bool build_rot_tables(qip_prec prec, uint32_t n, const std::vector<PauliTerm> &t
 // ---- device --------------------------------------------------------------------------------------------------------
 
 namespace {
-
-template <typename R>
-struct RotV;
-template <>
-struct RotV<float> {
-  typedef float2 type;
-};
-template <>
-struct RotV<double> {
-  typedef double2 type;
-};
-
-__device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
-__device__ __forceinline__ double mul_rn(double a, double b) { return __dmul_rn(a, b); }
-__device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }
-__device__ __forceinline__ double add_rn(double a, double b) { return __dadd_rn(a, b); }
-
-__device__ __forceinline__ bool parity(uint64_t v) { return __popcll(v) & 1; }
 
 __device__ __forceinline__ float flip_sign(float v, uint32_t bit) {
   return __int_as_float(__float_as_int(v) ^ (int)(bit << 31));
@@ -118,20 +86,6 @@ __device__ __forceinline__ V rot1(V a, V p, R c, R s, bool swap) {
     o.y = add_rn(mul_rn(c, a.y), mul_rn(s, p.y));
   }
   return o;
-}
-
-template <int B>
-__device__ __forceinline__ void cp_async(void *sdst, const void *gsrc) {
-  const uint32_t d = (uint32_t)__cvta_generic_to_shared(sdst);
-  if (B == 16)
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(d), "l"(gsrc) : "memory");
-  else
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;\n" ::"r"(d), "l"(gsrc) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-  asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory");
 }
 
 }  // namespace

@@ -2,7 +2,7 @@
 //
 //   rho[a][b] = sum_r psi(r, a) conj(psi(r, b))     (partial trace over every index bit not kept)
 //
-// Tile geometry as in expect.cu: the kRdmL lowest index bits plus up to kRdmM chosen high bits, 2^11 amplitudes.  Up to
+// Tile geometry of sweep.cuh: the kSweepL lowest index bits plus up to kRdmM chosen high bits, 2^11 amplitudes.  Up to
 // six kept bits ("columns") are tile bits; the other tile bits and the visit index are the traced-out rows r.  A tile is
 // then a block X of rows x C entries (C = 2^min(k, 6)), and a CTA accumulates X_I^T conj(X_J) over the tiles it visits.
 //   - k <= 6: every kept bit is a column, I = J, one read sweep gives all of rho.
@@ -31,54 +31,27 @@
 #include <cstring>
 #include <vector>
 
+#include "sweep.cuh"
+
 namespace qipb200 {
 
 namespace {
 
-const uint32_t kRdmL = 4;          // low index bits of a tile (runs of 16 amplitudes)
 const uint32_t kRdmM = 7;          // chosen high bits of a tile
-const uint32_t kRdmTileLog2 = kRdmL + kRdmM;
+const uint32_t kRdmTileLog2 = kSweepL + kRdmM;
 const uint32_t kRdmTile = 1u << kRdmTileLog2;
 const uint32_t kRdmColsLog2 = 6;   // kept bits inside the tile
 const int kRdmThreads = 256;
 const int kRdmPer = kRdmTile / kRdmThreads;  // tile amplitudes staged per thread
 const int kRdmGrid = 264;          // CTAs per sweep: two per SM of a 132-SM H100
+static_assert(kRdmM <= kSweepMaxHi, "the high tile bits fit SweepTiles::hi_pos");
 
 struct RdmArgs {
+  SweepTiles geo;         // x_out = 0; the block bits are skipped
   uint64_t off_i, off_j;  // block bits of the tiles I and J
-  uint64_t n_visits;      // tiles (or tile pairs) per sweep
-  uint32_t L, tb;         // low bits, tile bits
   uint32_t rows;          // rows per tile: 2^tb / C
-  uint32_t n_out;         // bits of the visit index, spread over out_pos
-  uint8_t hi_pos[kRdmM];
   uint8_t slot[kRdmTileLog2];  // tile slot -> 0x80 | column bit, or row bit
-  uint8_t out_pos[64];
 };
-
-template <typename R>
-struct RdmV;
-template <>
-struct RdmV<float> {
-  typedef float2 type;
-};
-template <>
-struct RdmV<double> {
-  typedef double2 type;
-};
-
-template <int B>
-__device__ __forceinline__ void cp_async(void *sdst, const void *gsrc) {
-  const uint32_t d = (uint32_t)__cvta_generic_to_shared(sdst);
-  if (B == 16)
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(d), "l"(gsrc) : "memory");
-  else
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;\n" ::"r"(d), "l"(gsrc) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-  asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory");
-}
 
 // Register blocks: RB x RB entries per thread, Q x Q blocks, S threads per block splitting the rows.
 template <int C>
@@ -96,7 +69,7 @@ struct RdmShape {
 template <typename R, int C, bool SAME>
 __global__ void __launch_bounds__(kRdmThreads, 2)
     k_rdm(const R *__restrict__ psi, const __grid_constant__ RdmArgs a, double2 *__restrict__ partials) {
-  typedef typename RdmV<R>::type V;
+  typedef typename SweepV<R>::type V;
   typedef RdmShape<C> SH;
   constexpr int RB = SH::RB, Q = SH::Q, NB = SH::NB, S = SH::S;
   constexpr bool ROWMAJOR = SH::ROWMAJOR;
@@ -104,7 +77,7 @@ __global__ void __launch_bounds__(kRdmThreads, 2)
   extern __shared__ __align__(16) unsigned char smem[];
   V *tiles = reinterpret_cast<V *>(smem);
   const int t = threadIdx.x;
-  const uint32_t tsize = 1u << a.tb, rows = a.rows;
+  const uint32_t tsize = 1u << a.geo.tb, rows = a.rows;
   const int blk = ROWMAJOR ? t % NB : t / S, split = ROWMAJOR ? t / NB : t % S;
   const int ablk = blk / Q, bblk = blk % Q;
   // global offset and shared-memory slot of the tile elements this thread stages
@@ -113,11 +86,14 @@ __global__ void __launch_bounds__(kRdmThreads, 2)
 #pragma unroll
   for (int k = 0; k < kRdmPer; ++k) {
     const uint32_t e = t + kRdmThreads * k;
-    uint64_t o = e & ((1u << a.L) - 1);
+    // tile_offset(a.geo, e), fused with the slot loop: written as tile_offset plus a separate slot loop, each k_rdm
+    // instantiation compiles to 96-112 more SASS instructions (e.g. k_rdm<double, 64, true>: 2000 -> 2096) and its
+    // register count moves by -12..+8 (sm_90a, CUDA 12.9)
+    uint64_t o = e & ((1u << a.geo.L) - 1);
     uint32_t c = 0, r = 0;
-    for (uint32_t sl = 0; sl < a.tb; ++sl) {
+    for (uint32_t sl = 0; sl < a.geo.tb; ++sl) {
       const uint32_t bit = (e >> sl) & 1u;
-      if (sl >= a.L) o |= (uint64_t)bit << a.hi_pos[sl - a.L];
+      if (sl >= a.geo.L) o |= (uint64_t)bit << a.geo.hi_pos[sl - a.geo.L];
       const uint32_t code = a.slot[sl];
       if (code & 0x80)
         c |= bit << (code & 0x7f);
@@ -128,8 +104,7 @@ __global__ void __launch_bounds__(kRdmThreads, 2)
     dst[k] = ROWMAJOR ? r * C + c : c * rows + r;
   }
   auto issue = [&](uint64_t v, int b) {
-    uint64_t base = 0;
-    for (uint32_t i = 0; i < a.n_out; ++i) base |= ((v >> i) & 1ull) << a.out_pos[i];
+    const uint64_t base = visit_base(a.geo, v);
     V *sI = tiles + (size_t)b * tsize;
     V *sJ = sI + tsize;
 #pragma unroll
@@ -145,13 +120,13 @@ __global__ void __launch_bounds__(kRdmThreads, 2)
 #pragma unroll
     for (int j = 0; j < RB; ++j) acc[i][j] = make_double2(0.0, 0.0);
   uint64_t v = blockIdx.x;
-  if (v < a.n_visits) issue(v, 0);
+  if (v < a.geo.n_visits) issue(v, 0);
   cp_async_commit();
   int cur = 0;
-  for (; v < a.n_visits; v += gridDim.x) {
+  for (; v < a.geo.n_visits; v += gridDim.x) {
     const uint64_t nv = v + gridDim.x;
     if (SAME) {  // the next tile into the other buffer, then wait for the current one only
-      if (nv < a.n_visits) issue(nv, cur ^ 1);
+      if (nv < a.geo.n_visits) issue(nv, cur ^ 1);
       cp_async_commit();
       cp_async_wait<1>();
     } else {
@@ -188,7 +163,7 @@ __global__ void __launch_bounds__(kRdmThreads, 2)
     if (SAME) {
       cur ^= 1;
     } else {
-      if (nv < a.n_visits) issue(nv, 0);
+      if (nv < a.geo.n_visits) issue(nv, 0);
       cp_async_commit();
     }
   }
@@ -239,11 +214,11 @@ __global__ void __launch_bounds__(256) k_rdm_reduce(const double2 *__restrict__ 
 
 template <typename R, int C, bool SAME>
 cudaError_t launch_rdm(const void *psi, const RdmArgs &a, double2 *partials, cudaStream_t s) {
-  typedef typename RdmV<R>::type V;
+  typedef typename SweepV<R>::type V;
   typedef RdmShape<C> SH;
   static_assert(2 * kRdmTile * sizeof(double2) <= 113 * 1024 && SH::RED_BYTES <= 113 * 1024,
                 "two CTAs per SM: at most 113 KiB of shared memory each");
-  const size_t smem = std::max(((size_t)2 << a.tb) * sizeof(V), SH::RED_BYTES);
+  const size_t smem = std::max(((size_t)2 << a.geo.tb) * sizeof(V), SH::RED_BYTES);
   const size_t smem_max = std::max((size_t)2 * kRdmTile * sizeof(V), SH::RED_BYTES);
   cudaError_t e = cudaFuncSetAttribute(k_rdm<R, C, SAME>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
   if (e != cudaSuccess) return e;
@@ -273,7 +248,7 @@ uint64_t rdm_launch_count(uint32_t k) {
 
 cudaError_t run_reduced_density(qip_prec prec, const void *psi, uint32_t n, const uint32_t *pos, uint32_t k,
                                 double *out, cudaStream_t s, uint64_t *launches) {
-  const uint32_t L = std::min(kRdmL, n);
+  const uint32_t L = std::min(kSweepL, n);
   const uint32_t k_in = std::min(k, kRdmColsLog2), C = 1u << k_in, nB = 1u << (k - k_in), K = 1u << k;
   // columns: the kept bits among the L low bits (always in the tile) first, then the others in the given order; the
   // kept bits left over are block bits, all above the low bits
@@ -286,33 +261,25 @@ cudaError_t run_reduced_density(qip_prec prec, const void *psi, uint32_t n, cons
   for (uint32_t i = 0; i < k; ++i)
     if (pos[i] >= L) (col.size() < k_in ? col : blk).push_back(i);
   // high tile bits: the columns above the low bits, then the lowest bits that are not kept
-  std::vector<uint32_t> hi;
+  uint64_t hi = 0, blk_mask = 0;
   for (uint32_t i : col)
-    if (pos[i] >= L) hi.push_back(pos[i]);
+    if (pos[i] >= L) hi |= 1ull << pos[i];
   const uint32_t m = std::min(kRdmM, n - L - (uint32_t)blk.size());
-  for (uint32_t b = L; b < n && hi.size() < m; ++b)
-    if (!((kept >> b) & 1)) hi.push_back(b);
-  std::sort(hi.begin(), hi.end());
-  uint64_t tile = (1ull << L) - 1, blk_mask = 0;
-  for (uint32_t b : hi) tile |= 1ull << b;
+  for (uint32_t b = L; b < n && (uint32_t)__builtin_popcountll(hi) < m; ++b)
+    if (!((kept >> b) & 1)) hi |= 1ull << b;
   for (uint32_t i : blk) blk_mask |= 1ull << pos[i];
   RdmArgs a;
   memset(&a, 0, sizeof(a));
-  a.L = L;
-  a.tb = L + (uint32_t)hi.size();
-  for (size_t h = 0; h < hi.size(); ++h) a.hi_pos[h] = (uint8_t)hi[h];
+  a.geo = sweep_tiles(n, L, hi, 0, blk_mask);
   uint32_t n_rows_bits = 0;
-  for (uint32_t sl = 0; sl < a.tb; ++sl) {
-    const uint32_t p = sl < L ? sl : hi[sl - L];
+  for (uint32_t sl = 0; sl < a.geo.tb; ++sl) {
+    const uint32_t p = sl < L ? sl : a.geo.hi_pos[sl - L];
     uint32_t code = 0xff;
     for (uint32_t ci = 0; ci < k_in; ++ci)
       if (pos[col[ci]] == p) code = 0x80 | ci;
     a.slot[sl] = (uint8_t)(code == 0xff ? n_rows_bits++ : code);
   }
   a.rows = 1u << n_rows_bits;
-  for (uint32_t b = 0; b < n; ++b)
-    if (!((tile >> b) & 1) && !((blk_mask >> b) & 1)) a.out_pos[a.n_out++] = (uint8_t)b;
-  a.n_visits = 1ull << a.n_out;
 
   const size_t part_bytes = (size_t)kRdmGrid * C * C * sizeof(double2);
   const size_t rho_bytes = (size_t)K * K * sizeof(double2);
