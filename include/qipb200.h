@@ -374,6 +374,54 @@ int qipb200_state_apply_function(qipb200_state *state, const qipb200_function *f
  * give QIPB200_ERR_INVALID_ARG; n_in and n_out are checked as function_new checks them, the qubits as the call does. */
 int qipb200_function_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *in_qubits, uint32_t n_in, const uint64_t *out_qubits, uint32_t n_out, uint32_t *out2);
 
+/* Functions given as CUDA source (absent in the reference): the same op U |x>|y> = e^{i theta(x)} |x>|y XOR f(x)> with f
+ * and theta evaluated on the device, so no table is built or uploaded and n_in may span the whole state.  `source` is
+ * CUDA C++ that defines
+ *   __device__ uint64_t qip_f(uint64_t x)                   when n_out > 0, and
+ *   __device__ double qip_theta(uint64_t x, const double *p) with QIPB200_FN_CODE_THETA,
+ * where p holds the handle's n_params parameters (set by function_set_params, all 0 at creation); the bit convention
+ * is that of function_new.  The source is compiled with NVRTC for sm_90a together with the kernels of the table path
+ * (--fmad=false, the options of the generated pass kernels), through the same process cache and QIPB200_JIT_CACHE_DIR
+ * on-disk cache.  Before the handle is returned, one kernel evaluates f over every x < 2^n_in and one evaluates theta
+ * with the zero parameters: f(x) >= 2^n_out or a non-finite theta(x) refuses the handle, naming the first such x.
+ * Errors: NULL ctx or out, NULL or empty source, n_in == 0, unknown flags, n_out == 0 without THETA (nothing to apply),
+ * n_params > 16, an NVRTC compile error (the NVRTC log goes to `log`, when log_len > 0, and to last_error) and the
+ * refusals above give QIPB200_ERR_INVALID_ARG; n_out > 32, n_in + n_out > 34, multi-device contexts, and a process
+ * without NVRTC or the driver API (the reason in `log`) QIPB200_ERR_UNSUPPORTED.  Synchronises.
+ * A code handle applies with qipb200_state_apply_function exactly as a table does (same checks, path plan, one kernel
+ * and one read-write sweep), with c = RN(cos theta(x)) and s = RN(sin theta(x)) from sincos evaluated in double on the
+ * device.  function_free of a code handle waits for the context's stream before it unloads the program. */
+enum { QIPB200_FN_CODE_THETA = 1u /* the source defines qip_theta */ };
+int qipb200_function_new_code(qipb200_ctx *ctx, uint32_t n_in, uint32_t n_out, const char *source, uint32_t flags, uint32_t n_params, char *log, size_t log_len, qipb200_function **out);
+/* Set the n_params parameters theta is evaluated with (n_params must equal the handle's).  With THETA, one kernel first
+ * evaluates theta(x, params) for every x < 2^n_in; a non-finite value gives QIPB200_ERR_INVALID_ARG naming the first
+ * such x and keeps the previous parameters.  NULL fn, or NULL params with n_params > 0, QIPB200_ERR_INVALID_ARG; a
+ * table handle QIPB200_ERR_UNSUPPORTED.  Synchronises.  Applies queued before keep the parameters they were queued
+ * with. */
+int qipb200_function_set_params(qipb200_function *fn, const double *params, uint32_t n_params);
+/* Host-only (no GPU, ctx-free): build and compile the program of function_new_code, as qipb200_jit_precompile does for
+ * passes, so that code can be checked without a GPU.  Same argument checks and codes as function_new_code; the NVRTC
+ * log (errors, or warnings) goes to `log`. */
+int qipb200_function_code_compile(uint32_t n_in, uint32_t n_out, const char *source, uint32_t flags, uint32_t n_params, char *log, size_t log_len);
+/* f(x) into f_out[i] and (cos theta(x), sin theta(x)) in double into cs_out[2i], cs_out[2i + 1], for x = x0 + i,
+ * i < count, evaluated ON THE DEVICE by the functions the apply kernels use (the table lookups, or the compiled code
+ * with the current parameters): the apply rounds these (c, s) once to the state's precision.  Either output may be
+ * NULL; without a phase cs_out gets (1, 0) and without an out register f_out gets 0.  x0 + count > 2^n_in or NULL fn
+ * give QIPB200_ERR_INVALID_ARG.  Synchronises. */
+int qipb200_function_tabulate(const qipb200_function *fn, uint64_t x0, uint64_t count, uint64_t *f_out, double *cs_out);
+/* *out = sum_j |psi_j|^2 theta(x(j), p) = <psi|D|psi> for D = diag theta, x(j) the value of in_qubits in index j: the
+ * diagonal expectation value of a code handle with THETA (e.g. the QAOA energy <C> of any cost C), on the state AS IT
+ * IS (not renormalised, like expect_paulis).  One kernel, one read sweep.  Accumulated in double for both precisions
+ * (f32 amplitudes are widened before use) over a fixed grid with per-CTA partials summed on the host in a fixed order,
+ * no floating-point atomics: the same state and parameters give bit-identical out.  The order and the first-order
+ * rounding bound are documented in rustqip_b200/csrc/function.cu.  Synchronises.  Errors, all before any device work (a
+ * refused call leaves the state and a pending collapse as they were): NULL state, fn or out QIPB200_ERR_INVALID_ARG; a
+ * table handle or a code handle without THETA QIPB200_ERR_UNSUPPORTED (a table keeps cos theta and sin theta, not
+ * theta); in_qubits checked as apply_function checks them; sharded and multi-device states QIPB200_ERR_UNSUPPORTED; fn
+ * made on another context QIPB200_ERR_INVALID_ARG.  A pending collapse is applied first (one more kernel); a permuted
+ * layout is read where it is. */
+int qipb200_state_expect_function(qipb200_state *state, const qipb200_function *fn, const uint64_t *in_qubits, double *out);
+
 /* dst <- sum_h coeffs[h] P_h src, out of place: H|psi> for a Hamiltonian given as a real Pauli sum (absent in the
  * reference).  Terms are encoded and validated as for qipb200_state_expect_paulis (same codes and messages); an empty
  * term is coeffs[h] times the identity.  NULL coeffs with n_terms > 0, a non-finite coefficient or dst == src give

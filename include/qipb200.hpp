@@ -195,16 +195,24 @@ void apply_op_overwrite(Context &ctx, size_t n, const MatrixOp<P> &op, const std
 // U|x>|y> = e^{i theta(x)} |x>|y ^ f(x)> for a table of 2^n_in entries, checked and uploaded once; bit i of x is qubit
 // in_qubits[i], bit i of f(x) goes to out_qubits[i] (B200State::apply_function).  f may be empty when n_out == 0,
 // theta empty for a pure permutation.
+//
+// B200Function::from_code: the same op for f and theta given as CUDA source (qipb200_function_new_code), compiled with
+// NVRTC and evaluated on the device, so n_in may cover the whole state.  A compile error throws with the NVRTC log.
 class B200Function {
  public:
   B200Function(Context &ctx, uint32_t n_in, uint32_t n_out, const std::vector<uint64_t> &f,
                const std::vector<double> &theta = {})
-      : n_in_(n_in), n_out_(n_out) {
+      : ctx_(ctx), n_in_(n_in), n_out_(n_out) {
     const size_t size = n_in < 64 ? size_t(1) << n_in : 0;
     if ((!f.empty() && f.size() != size) || (!theta.empty() && theta.size() != size))
       throw CircuitError("B200Function: f and theta need 2^n_in = " + std::to_string(size) + " entries each");
     ctx.check(qipb200_function_new(ctx.get(), n_in, n_out, f.empty() ? nullptr : f.data(),
                                    theta.empty() ? nullptr : theta.data(), &fn_));
+  }
+  // source defines qip_f (n_out > 0) and, with theta, qip_theta(x, p) over n_params parameters (0 until set_params)
+  static B200Function from_code(Context &ctx, uint32_t n_in, uint32_t n_out, const std::string &source,
+                                bool theta = false, uint32_t n_params = 0) {
+    return B200Function(ctx, n_in, n_out, source, theta, n_params);
   }
   ~B200Function() { qipb200_function_free(fn_); }
   B200Function(const B200Function &) = delete;
@@ -212,8 +220,25 @@ class B200Function {
   uint32_t n_in() const { return n_in_; }
   uint32_t n_out() const { return n_out_; }
   const qipb200_function *get() const { return fn_; }
+  // code functions: the parameters theta is evaluated with (checked finite for every x; refused: the old ones stay)
+  void set_params(const std::vector<double> &params) {
+    ctx_.check(qipb200_function_set_params(fn_, params.empty() ? nullptr : params.data(), (uint32_t)params.size()));
+  }
+  // f(x) and (cos theta(x), sin theta(x)) (interleaved) for x in [x0, x0 + count), evaluated on the device
+  void tabulate(uint64_t x0, uint64_t count, std::vector<uint64_t> *f, std::vector<double> *cs) const {
+    if (f) f->assign(count, 0);
+    if (cs) cs->assign(2 * count, 0.0);
+    ctx_.check(qipb200_function_tabulate(fn_, x0, count, f ? f->data() : nullptr, cs ? cs->data() : nullptr));
+  }
 
  private:
+  B200Function(Context &ctx, uint32_t n_in, uint32_t n_out, const std::string &source, bool theta, uint32_t n_params)
+      : ctx_(ctx), n_in_(n_in), n_out_(n_out) {
+    // the NVRTC log of a compile error is in the last error, which check() throws
+    ctx.check(qipb200_function_new_code(ctx.get(), n_in, n_out, source.c_str(), theta ? QIPB200_FN_CODE_THETA : 0u,
+                                        n_params, nullptr, 0, &fn_));
+  }
+  Context &ctx_;
   uint32_t n_in_, n_out_;
   qipb200_function *fn_ = nullptr;
 };
@@ -347,6 +372,14 @@ class B200State {
                          std::to_string(fn.n_out()) + " output qubits");
     ctx_.check(qipb200_state_apply_function(st_, fn.get(), in_qubits.empty() ? nullptr : in_qubits.data(),
                                             out_qubits.empty() ? nullptr : out_qubits.data()));
+  }
+  // <psi|D|psi> = sum_j |psi_j|^2 theta(x(j)) for D = diag theta of a code function with theta, x on in_qubits
+  double expect_function(const B200Function &fn, const std::vector<uint64_t> &in_qubits) {
+    if (in_qubits.size() != fn.n_in())
+      throw CircuitError("expect_function: the function takes " + std::to_string(fn.n_in()) + " input qubits");
+    double out = 0.0;
+    ctx_.check(qipb200_state_expect_function(st_, fn.get(), in_qubits.data(), &out));
+    return out;
   }
   // this state <- H src for H = sum_h coeffs[h] P_h, Pauli strings encoded as in expect_paulis; src is another state
   // of the same context, precision and size, and this state takes its layout (absent in the reference)

@@ -34,7 +34,9 @@ EXPORTS = [
     "qipb200_state_measure", "qipb200_state_expect_paulis", "qipb200_expect_plan", "qipb200_state_transition_paulis",
     "qipb200_transition_plan", "qipb200_state_reduced_density",
     "qipb200_state_apply_pauli_rotations", "qipb200_pauli_rotation_plan", "qipb200_function_new",
-    "qipb200_function_free", "qipb200_state_apply_function", "qipb200_function_plan", "qipb200_state_apply_pauli_sum",
+    "qipb200_function_free", "qipb200_state_apply_function", "qipb200_function_plan", "qipb200_function_new_code",
+    "qipb200_function_set_params", "qipb200_function_code_compile", "qipb200_function_tabulate",
+    "qipb200_state_expect_function", "qipb200_state_apply_pauli_sum",
     "qipb200_pauli_sum_plan", "qipb200_state_pauli_energy_gradient", "qipb200_pauli_gradient_plan",
     "qipb200_state_pauli_geometric_tensor", "qipb200_pauli_geometric_tensor_plan",
     "qipb200_state_evolve_pauli_sum", "qipb200_pauli_evolution_plan", "qipb200_state_lanczos_pauli_sum",
@@ -126,6 +128,17 @@ def lib():
     L.qipb200_state_apply_function.argtypes = [vp, vp, vp, vp]
     L.qipb200_function_plan.restype = i32
     L.qipb200_function_plan.argtypes = [i32, u32, vp, u32, vp, u32, vp]
+    L.qipb200_function_new_code.restype = i32
+    L.qipb200_function_new_code.argtypes = [vp, u32, u32, C.c_char_p, u32, u32, C.c_char_p, C.c_size_t,
+                                            C.POINTER(vp)]
+    L.qipb200_function_set_params.restype = i32
+    L.qipb200_function_set_params.argtypes = [vp, vp, u32]
+    L.qipb200_function_code_compile.restype = i32
+    L.qipb200_function_code_compile.argtypes = [u32, u32, C.c_char_p, u32, u32, C.c_char_p, C.c_size_t]
+    L.qipb200_function_tabulate.restype = i32
+    L.qipb200_function_tabulate.argtypes = [vp, u64, u64, vp, vp]
+    L.qipb200_state_expect_function.restype = i32
+    L.qipb200_state_expect_function.argtypes = [vp, vp, vp, vp]
     L.qipb200_state_apply_pauli_sum.restype = i32
     L.qipb200_state_apply_pauli_sum.argtypes = [vp, vp, vp, vp, vp, C.c_size_t, vp]
     L.qipb200_pauli_sum_plan.restype = i32

@@ -2138,6 +2138,68 @@ void free_function_tables(qipb200_function *fn) {
   fn->d_cs = nullptr;
 }
 
+// A code function's module cannot be unloaded in stream order: the context's stream is drained first.
+void free_function_code(qipb200_function *fn) {
+  if (!fn->code && !fn->d_scratch) return;
+  cudaSetDevice(fn->ctx->device);
+  cudaStreamSynchronize(fn->ctx->stream);
+  function_code_free(fn->code);
+  if (fn->d_scratch) cudaFreeAsync(fn->d_scratch, fn->ctx->stream);
+  fn->code = nullptr;
+  fn->d_scratch = nullptr;
+}
+
+// n_in, n_out, flags, n_params and source of a code function: the checks function_new_code and function_code_compile
+// share.
+int check_code_args(const qipb200_ctx *ctx, const std::string &who, uint32_t n_in, uint32_t n_out, const char *source,
+                    uint32_t flags, uint32_t n_params) {
+  if (!source || !*source) return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL or empty source");
+  if (n_in == 0) return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": n_in must be at least 1");
+  if (flags & ~(uint32_t)QIPB200_FN_CODE_THETA)
+    return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": unknown flags " + std::to_string(flags));
+  const bool theta = flags & QIPB200_FN_CODE_THETA;
+  if (!n_out && !theta)
+    return set_err(ctx, QIPB200_ERR_INVALID_ARG,
+                   who + ": no output qubits and no QIPB200_FN_CODE_THETA: nothing to apply");
+  if (n_params > kFnCodeMaxParams)
+    return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": at most 16 parameters, got " + std::to_string(n_params));
+  if (n_out > kFnMaxOut) return set_err(ctx, QIPB200_ERR_UNSUPPORTED, who + ": at most 32 output qubits");
+  if (n_in + n_out > kFnCodeMaxBits)
+    return set_err(ctx, QIPB200_ERR_UNSUPPORTED,
+                   who + ": n_in + n_out = " + std::to_string(n_in + n_out) +
+                       " exceeds 34 (no state on one device is larger)");
+  return QIPB200_OK;
+}
+
+void copy_log(char *log, size_t log_len, const std::string &msg) {
+  if (log && log_len) snprintf(log, log_len, "%s", msg.c_str());
+}
+
+// A code function's status with msg (the NVRTC log for a compile error) in the last error and in log.
+int code_fail(const qipb200_ctx *ctx, const std::string &who, int st, const std::string &msg, char *log,
+              size_t log_len) {
+  copy_log(log, log_len, msg);
+  const char *what = st == QIPB200_ERR_INVALID_ARG    ? ": the source does not compile:\n"
+                     : st == QIPB200_ERR_UNSUPPORTED ? ": code functions need NVRTC and the driver API: "
+                                                      : ": ";
+  return set_err(ctx, st, who + what + msg);
+}
+
+// theta(x, params) is finite for every x < 2^n_in, or the error that names the first x where it is not.
+int check_code_theta(qipb200_function *fn, const double *params, const std::string &who) {
+  qipb200_ctx *ctx = fn->ctx;
+  uint64_t first = 0;
+  std::string err;
+  cudaError_t e = function_code_first_bad(fn->code, false, fn->n_in, fn->n_out, params, (uint64_t *)fn->d_scratch,
+                                          ctx->sm_count, ctx->stream, &first, &err);
+  ++ctx->launches;
+  if (e != cudaSuccess)
+    return err.empty() ? cuda_fail(ctx, e, "function_code_first_bad") : set_err(ctx, QIPB200_ERR_CUDA, who + ": " + err);
+  if (first != ~0ull)
+    return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": theta(" + std::to_string(first) + ") is not finite");
+  return QIPB200_OK;
+}
+
 }  // namespace
 
 extern "C" int qipb200_function_new(qipb200_ctx *ctx, uint32_t n_in, uint32_t n_out, const uint64_t *f,
@@ -2205,6 +2267,7 @@ extern "C" int qipb200_function_new(qipb200_ctx *ctx, uint32_t n_in, uint32_t n_
 extern "C" void qipb200_function_free(qipb200_function *fn) {
   if (!fn) return;
   free_function_tables(fn);  // stream-ordered: an apply queued before runs first
+  free_function_code(fn);
   delete fn;
 }
 
@@ -2224,9 +2287,16 @@ extern "C" int qipb200_state_apply_function(qipb200_state *s, const qipb200_func
     CU(ctx, cudaSetDevice(ctx->device));
     if ((st = materialise_collapse(s)) != QIPB200_OK) return st;
     // A permuted layout (QIPB200_ROTATE) needs no restore: the registers are read and written where their qubits are.
-    uint32_t in_pos[kFnMaxIn], out_pos[kFnMaxOut];
+    uint32_t in_pos[kFnCodeMaxBits], out_pos[kFnMaxOut];
     for (uint32_t i = 0; i < fn->n_in; ++i) in_pos[i] = s->phys_of_logical[s->n - 1 - (uint32_t)in_qubits[i]];
     for (uint32_t i = 0; i < fn->n_out; ++i) out_pos[i] = s->phys_of_logical[s->n - 1 - (uint32_t)out_qubits[i]];
+    if (fn->code) {
+      std::string err;
+      const cudaError_t e = run_function_code(s->prec, s->buf, s->n_local, in_pos, fn->n_in, out_pos, fn->n_out,
+                                              fn->code, fn->params, ctx->sm_count, ctx->stream, &ctx->launches, &err);
+      if (e != cudaSuccess) return err.empty() ? cuda_fail(ctx, e, "run_function_code") : set_err(ctx, QIPB200_ERR_CUDA, who + ": " + err);
+      return (int)QIPB200_OK;
+    }
     CU(ctx, run_function(s->prec, s->buf, s->n_local, in_pos, fn->n_in, out_pos, fn->n_out, fn->d_f, fn->d_cs,
                          ctx->sm_count, ctx->stream, &ctx->launches));
     return (int)QIPB200_OK;
@@ -2248,6 +2318,161 @@ extern "C" int qipb200_function_plan(qip_prec prec, uint32_t n_qubits, const uin
     const FnPlan p = plan_function(prec, n_qubits, out_pos, n_out);
     out2[0] = p.path;
     out2[1] = p.tile_bits;
+    return (int)QIPB200_OK;
+  });
+}
+
+extern "C" int qipb200_function_code_compile(uint32_t n_in, uint32_t n_out, const char *source, uint32_t flags,
+                                             uint32_t n_params, char *log, size_t log_len) {
+  const std::string who = "function_code_compile";
+  copy_log(log, log_len, std::string());
+  return guarded(nullptr, [&]() -> int {
+    int st = check_code_args(nullptr, who, n_in, n_out, source, flags, n_params);
+    if (st != QIPB200_OK) return st;
+    std::string msg;
+    if ((st = function_code_compile(n_out, source, flags & QIPB200_FN_CODE_THETA, &msg)) != QIPB200_OK)
+      return code_fail(nullptr, who, st, msg, log, log_len);
+    copy_log(log, log_len, msg);  // warnings, if any
+    return (int)QIPB200_OK;
+  });
+}
+
+extern "C" int qipb200_function_new_code(qipb200_ctx *ctx, uint32_t n_in, uint32_t n_out, const char *source,
+                                         uint32_t flags, uint32_t n_params, char *log, size_t log_len,
+                                         qipb200_function **out) {
+  const std::string who = "function_new_code";
+  copy_log(log, log_len, std::string());
+  if (!ctx || !out) return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL context or out-pointer");
+  *out = nullptr;
+  return guarded(ctx, [&]() -> int {
+    int st = check_code_args(ctx, who, n_in, n_out, source, flags, n_params);
+    if (st != QIPB200_OK) return st;
+    if (!ctx->children.empty())
+      return set_err(ctx, QIPB200_ERR_UNSUPPORTED, who + ": multi-device contexts are not supported");
+    CU(ctx, cudaSetDevice(ctx->device));
+    const bool theta = flags & QIPB200_FN_CODE_THETA;
+    std::string msg;
+    FnCode *code = nullptr;
+    if ((st = function_code_load(n_out, source, theta, &code, &msg)) != QIPB200_OK)
+      return code_fail(ctx, who, st, msg, log, log_len);
+    copy_log(log, log_len, msg);
+    qipb200_function *fn = new qipb200_function();
+    fn->ctx = ctx;
+    fn->n_in = n_in;
+    fn->n_out = n_out;
+    fn->code = code;
+    fn->theta = theta;
+    fn->n_params = n_params;
+    auto refuse = [&](int code_st) {
+      free_function_code(fn);
+      delete fn;
+      return code_st;
+    };
+    cudaError_t e = cudaMallocAsync(&fn->d_scratch, (1 + kFnExpPartials) * sizeof(double), ctx->stream);
+    if (e != cudaSuccess) return refuse(cuda_fail(ctx, e, "cudaMallocAsync(function scratch)"));
+    std::string err;
+    if (n_out) {  // every f(x) fits the out register
+      uint64_t first = 0;
+      e = function_code_first_bad(code, true, n_in, n_out, fn->params, (uint64_t *)fn->d_scratch, ctx->sm_count,
+                                  ctx->stream, &first, &err);
+      ++ctx->launches;
+      uint64_t fx = 0;
+      if (e == cudaSuccess && first != ~0ull)
+        e = tabulate_function(code, fn->params, nullptr, nullptr, first, 1, &fx, nullptr, ctx->sm_count, ctx->stream,
+                              &err);
+      if (e != cudaSuccess)
+        return refuse(err.empty() ? cuda_fail(ctx, e, "function_code_first_bad")
+                                  : set_err(ctx, QIPB200_ERR_CUDA, who + ": " + err));
+      if (first != ~0ull)
+        return refuse(set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": f(" + std::to_string(first) + ") = " +
+                                                                std::to_string(fx) + " does not fit in " +
+                                                                std::to_string(n_out) + " output bits"));
+    }
+    if (theta && (st = check_code_theta(fn, fn->params, who)) != QIPB200_OK) return refuse(st);
+    *out = fn;
+    return (int)QIPB200_OK;
+  });
+}
+
+extern "C" int qipb200_function_set_params(qipb200_function *fn, const double *params, uint32_t n_params) {
+  const std::string who = "function_set_params";
+  if (!fn) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, who + ": NULL function");
+  qipb200_ctx *ctx = fn->ctx;
+  return guarded(ctx, [&]() -> int {
+    if (!fn->code)
+      return set_err(ctx, QIPB200_ERR_UNSUPPORTED, who + ": a table function has no parameters");
+    if (n_params != fn->n_params)
+      return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": the function takes " + std::to_string(fn->n_params) +
+                                                       " parameters, got " + std::to_string(n_params));
+    if (n_params && !params) return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL params");
+    double p[kFnCodeMaxParams] = {};
+    for (uint32_t i = 0; i < n_params; ++i) p[i] = params[i];
+    if (fn->theta) {
+      CU(ctx, cudaSetDevice(ctx->device));
+      const int st = check_code_theta(fn, p, who);
+      if (st != QIPB200_OK) return st;  // the previous parameters stay
+    }
+    memcpy(fn->params, p, sizeof(p));
+    return (int)QIPB200_OK;
+  });
+}
+
+extern "C" int qipb200_function_tabulate(const qipb200_function *fn, uint64_t x0, uint64_t count, uint64_t *f_out,
+                                         double *cs_out) {
+  const std::string who = "function_tabulate";
+  if (!fn) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, who + ": NULL function");
+  qipb200_ctx *ctx = fn->ctx;
+  return guarded(ctx, [&]() -> int {
+    const uint64_t N = 1ull << fn->n_in;
+    if (x0 > N || count > N - x0)
+      return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": [x0, x0 + count) exceeds 2^n_in = " + std::to_string(N));
+    if (!count) return (int)QIPB200_OK;
+    const bool phase = fn->code ? fn->theta : fn->d_cs != nullptr;
+    if (cs_out && !phase)  // no phase: e^{i 0}
+      for (uint64_t i = 0; i < count; ++i) {
+        cs_out[2 * i] = 1.0;
+        cs_out[2 * i + 1] = 0.0;
+      }
+    if (!f_out && !(cs_out && phase)) return (int)QIPB200_OK;
+    CU(ctx, cudaSetDevice(ctx->device));
+    std::string err;
+    const cudaError_t e = tabulate_function(fn->code, fn->params, fn->d_f, fn->d_cs, x0, count, f_out,
+                                            phase ? cs_out : nullptr, ctx->sm_count, ctx->stream, &err);
+    ++ctx->launches;
+    if (e != cudaSuccess)
+      return err.empty() ? cuda_fail(ctx, e, "tabulate_function") : set_err(ctx, QIPB200_ERR_CUDA, who + ": " + err);
+    return (int)QIPB200_OK;
+  });
+}
+
+extern "C" int qipb200_state_expect_function(qipb200_state *s, const qipb200_function *fn, const uint64_t *in_qubits,
+                                             double *out) {
+  const std::string who = "expect_function";
+  if (!s || !fn || !out)
+    return set_err(s ? s->ctx : nullptr, QIPB200_ERR_INVALID_ARG, who + ": NULL state, function or out");
+  return guarded(s->ctx, [&]() -> int {
+    // every check runs before any device work: a refused call leaves the state (and a pending collapse) as it was
+    if (!fn->code)
+      return set_err(s->ctx, QIPB200_ERR_UNSUPPORTED,
+                     who + ": a table function keeps cos theta and sin theta, not theta: make it from code");
+    if (!fn->theta)
+      return set_err(s->ctx, QIPB200_ERR_UNSUPPORTED, who + ": the function has no theta (QIPB200_FN_CODE_THETA)");
+    int st = check_function_registers(s->ctx, who, s->n, in_qubits, fn->n_in, nullptr, 0);
+    if (st != QIPB200_OK) return st;
+    if (s->world > 1 || !s->shards.empty())
+      return set_err(s->ctx, QIPB200_ERR_UNSUPPORTED, who + ": sharded states are not supported");
+    if (fn->ctx != s->ctx)
+      return set_err(s->ctx, QIPB200_ERR_INVALID_ARG, who + ": the function was made on another context");
+    qipb200_ctx *ctx = s->ctx;
+    CU(ctx, cudaSetDevice(ctx->device));
+    if ((st = materialise_collapse(s)) != QIPB200_OK) return st;
+    uint32_t in_pos[kFnCodeMaxBits];
+    for (uint32_t i = 0; i < fn->n_in; ++i) in_pos[i] = s->phys_of_logical[s->n - 1 - (uint32_t)in_qubits[i]];
+    std::string err;
+    const cudaError_t e = expect_function_code(s->prec, s->buf, s->n_local, in_pos, fn->n_in, fn->code, fn->params,
+                                               (double *)fn->d_scratch + 1, ctx->stream, &ctx->launches, out, &err);
+    if (e != cudaSuccess)
+      return err.empty() ? cuda_fail(ctx, e, "expect_function_code") : set_err(ctx, QIPB200_ERR_CUDA, who + ": " + err);
     return (int)QIPB200_OK;
   });
 }

@@ -409,6 +409,47 @@ void jit_unload(std::vector<std::pair<const JitCubin *, JitLoaded>> *loaded) {
   loaded->clear();
 }
 
+namespace {
+
+cudaError_t driver_fail(CUresult r, const char *what, std::string *err) {
+  const char *nm = nullptr;
+  driver().err_name(r, &nm);
+  if (err) *err = std::string(what) + ": " + (nm ? nm : "?");
+  return cudaErrorUnknown;
+}
+
+}  // namespace
+
+cudaError_t jit_module_load(const JitCubin &cubin, CUmodule *mod, std::string *err) {
+  Driver &d = driver();
+  if (!d.ok || !cubin.ok) {
+    if (err) *err = !d.ok ? d.why : "no cubin";
+    return cudaErrorNotSupported;
+  }
+  const CUresult r = d.module_load(mod, cubin.image.data());
+  return r == CUDA_SUCCESS ? cudaSuccess : driver_fail(r, "cuModuleLoadData", err);
+}
+
+cudaError_t jit_module_kernel(CUmodule mod, const char *name, unsigned max_dyn_smem, CUfunction *fn, std::string *err) {
+  Driver &d = driver();
+  CUresult r = d.module_get(fn, mod, name);
+  if (r != CUDA_SUCCESS) return driver_fail(r, "cuModuleGetFunction", err);
+  if (max_dyn_smem && (r = d.func_set_attr(*fn, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)max_dyn_smem)) !=
+                          CUDA_SUCCESS)
+    return driver_fail(r, "cuFuncSetAttribute(max dynamic shared memory)", err);
+  return cudaSuccess;
+}
+
+cudaError_t jit_kernel_launch(CUfunction fn, unsigned grid, unsigned threads, unsigned smem, cudaStream_t stream,
+                              void **args, std::string *err) {
+  const CUresult r = driver().launch(fn, grid, 1, 1, threads, 1, 1, smem, (CUstream)stream, args, nullptr);
+  return r == CUDA_SUCCESS ? cudaSuccess : driver_fail(r, "cuLaunchKernel", err);
+}
+
+void jit_module_unload(CUmodule mod) {
+  if (mod && driver().ok) driver().module_unload(mod);
+}
+
 JitMode jit_mode_from_env(uint32_t n_local) {
   if (const char *e = getenv("QIPB200_JIT")) {
     if (!strcmp(e, "off") || !strcmp(e, "0")) return JIT_OFF;

@@ -65,6 +65,16 @@ cudaError_t jit_launch(const std::shared_ptr<const JitCubin> &cubin, std::vector
 
 void jit_unload(std::vector<std::pair<const JitCubin *, JitLoaded>> *loaded);
 
+// A compiled program as a module of the current device's context whose kernels are looked up by name and launched on
+// runtime streams (the code functions of function.cu).  The calls fail with cudaErrorNotSupported when the driver entry
+// points are missing, with cudaErrorUnknown on a driver error; *err then says which.
+cudaError_t jit_module_load(const JitCubin &cubin, CUmodule *mod, std::string *err);
+// Kernel `name` of mod, allowed max_dyn_smem bytes of dynamic shared memory (0: the default).
+cudaError_t jit_module_kernel(CUmodule mod, const char *name, unsigned max_dyn_smem, CUfunction *fn, std::string *err);
+cudaError_t jit_kernel_launch(CUfunction fn, unsigned grid, unsigned threads, unsigned smem, cudaStream_t stream,
+                              void **args, std::string *err);
+void jit_module_unload(CUmodule mod);
+
 JitMode jit_mode_from_env(uint32_t n_local);
 
 }  // namespace qipb200

@@ -93,13 +93,23 @@ struct qipb200_state {
   double pend_p_mult = 1.0;
 };
 
-// A classical function of an n_in-bit register (qipb200_function_new): its tables live on ctx's device and are freed
-// on ctx's stream.
+namespace qipb200 {
+struct FnCode;
+}
+
+// A classical function of an n_in-bit register, given as tables (qipb200_function_new: they live on ctx's device and
+// are freed on ctx's stream) or as code (qipb200_function_new_code: a compiled program loaded on ctx's device).
 struct qipb200_function {
   qipb200_ctx *ctx = nullptr;
   uint32_t n_in = 0, n_out = 0;
   uint32_t *d_f = nullptr;    // f[x] for x < 2^n_in, NULL when n_out == 0
   double2 *d_cs = nullptr;    // (cos, sin) of theta[x] in double, NULL without phases
+  // code functions only
+  qipb200::FnCode *code = nullptr;
+  bool theta = false;         // the source defines qip_theta
+  uint32_t n_params = 0;
+  double params[16] = {};     // the parameters theta is evaluated with (unused entries 0)
+  void *d_scratch = nullptr;  // one u64 for the checks, then the expect partials
 };
 
 namespace qipb200 {

@@ -340,6 +340,18 @@ class State:
         self._chk(_lib.lib().qipb200_state_apply_function(self._h, fn.handle, _ptr(ia) if ia.shape[0] else None,
                                                           _ptr(oa) if oa.shape[0] else None))
 
+    def expect_function(self, fn: "Function", in_qubits: Sequence[int]) -> float:
+        """<psi|D|psi> = sum_j |psi_j|^2 theta(x(j), p) for D = diag theta of a code function made with
+        ``theta=True`` (e.g. the QAOA energy <C> of a cost C), on the state as it is (not renormalised), computed on
+        the device in one read sweep; bit i of x is the value of qubit ``in_qubits[i]``.  Accumulated in double in a
+        fixed order (bit-identical on repeated calls); synchronises."""
+        ia = np.ascontiguousarray(np.asarray(list(in_qubits), dtype=np.uint64))
+        if ia.shape[0] != fn.n_in:
+            raise ValueError("expect_function: the function takes %d input qubits, got %d" % (fn.n_in, ia.shape[0]))
+        out = C.c_double()
+        self._chk(_lib.lib().qipb200_state_expect_function(self._h, fn.handle, _ptr(ia), C.byref(out)))
+        return float(out.value)
+
     def apply_pauli_sum(self, src: "State", terms, coeffs):
         """Set this state to H|src> for H = sum_h coeffs[h] P_h, a real Pauli sum, on the device (out of place).
 
@@ -525,12 +537,53 @@ class Function:
                                                    None if fa is None else _ptr(fa), None if ta is None else _ptr(ta),
                                                    C.byref(self._h)), ctx.handle)
 
+    @classmethod
+    def from_code(cls, ctx: Context, n_in: int, n_out: int, source: str, theta: bool = False,
+                  n_params: int = 0) -> "Function":
+        """A function given as CUDA source (qipb200_function_new_code), evaluated on the device: no table, so
+        ``n_in`` may cover the whole state (n_in + n_out <= 34, n_out <= 32).
+
+        ``source`` defines ``__device__ uint64_t qip_f(uint64_t x)`` when ``n_out > 0`` and, with ``theta=True``,
+        ``__device__ double qip_theta(uint64_t x, const double *p)`` where ``p`` holds the ``n_params`` (<= 16)
+        parameters of ``set_params`` (all 0 at first).  It is compiled with NVRTC for sm_90a (cached in the process
+        and in ``QIPB200_JIT_CACHE_DIR``); a compile error raises ``CircuitError`` with the NVRTC log.  f is checked
+        over every x (f(x) < 2^n_out) and theta with the zero parameters (finite) before the handle is returned."""
+        self = cls.__new__(cls)
+        self.ctx, self.n_in, self.n_out, self.n_params = ctx, int(n_in), int(n_out), int(n_params)
+        self._h = C.c_void_p()
+        log = C.create_string_buffer(1 << 16)
+        _lib.check(_lib.lib().qipb200_function_new_code(ctx.handle, self.n_in, self.n_out, source.encode("utf-8"),
+                                                        FN_CODE_THETA if theta else 0, self.n_params, log,
+                                                        len(log), C.byref(self._h)), ctx.handle)
+        return self
+
+    def set_params(self, params):
+        """Set the parameters theta(x, p) of a code function is evaluated with; theta is checked finite for every x
+        first (a refused vector raises ``CircuitError`` and keeps the previous parameters).  Later applies use the
+        new values; applies already queued keep theirs.  Synchronises."""
+        pa = np.ascontiguousarray(np.asarray(params, dtype=np.float64).reshape(-1))
+        _lib.check(_lib.lib().qipb200_function_set_params(self._h, _ptr(pa) if pa.shape[0] else None, pa.shape[0]),
+                   self.ctx.handle)
+
+    def tabulate(self, x0: int = 0, count: int = None):
+        """(f, cs) for x in [x0, x0 + count), evaluated on the device by the functions the apply kernels use:
+        f (uint64) and cs (float64, shape (count, 2)) = (cos theta(x), sin theta(x)) in double, which the apply rounds
+        once to the state's precision.  Without a phase cs is (1, 0); without an out register f is 0."""
+        if count is None:
+            count = (1 << self.n_in) - int(x0)
+        f = np.zeros(max(1, int(count)), dtype=np.uint64)
+        cs = np.zeros((max(1, int(count)), 2), dtype=np.float64)
+        _lib.check(_lib.lib().qipb200_function_tabulate(self._h, int(x0), int(count), _ptr(f), _ptr(cs)),
+                   self.ctx.handle)
+        return f[: int(count)], cs[: int(count)]
+
     @property
     def handle(self):
         return self._h
 
     def free(self):
-        """Release the device tables (stream-ordered: safe straight after an apply)."""
+        """Release the device tables (stream-ordered: safe straight after an apply); a code function waits for the
+        context's stream, then unloads its program."""
         if self._h:
             _lib.lib().qipb200_function_free(self._h)
             self._h = C.c_void_p()
@@ -549,6 +602,17 @@ class Function:
 
 
 FUNCTION_TILE, FUNCTION_PAIR = 0, 1
+FN_CODE_THETA = 1  # QIPB200_FN_CODE_THETA
+
+
+def function_code_compile(n_in: int, n_out: int, source: str, theta: bool = False, n_params: int = 0) -> str:
+    """Compile the program of ``Function.from_code`` with NVRTC without a context or GPU; returns the NVRTC log
+    (warnings, if any) and raises ``CircuitError`` (with the log) on a compile error or refused sizes."""
+    log = C.create_string_buffer(1 << 16)
+    _lib.check(_lib.lib().qipb200_function_code_compile(int(n_in), int(n_out), source.encode("utf-8"),
+                                                        FN_CODE_THETA if theta else 0, int(n_params), log, len(log)),
+               None)
+    return log.value.decode("utf-8", "replace")
 
 
 def function_plan(n: int, dtype, in_qubits: Sequence[int], out_qubits: Sequence[int] = ()):
