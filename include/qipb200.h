@@ -316,6 +316,26 @@ int qipb200_transition_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qu
  * Sharded and multi-device states: QIPB200_ERR_UNSUPPORTED. */
 int qipb200_state_reduced_density(qipb200_state *state, const uint64_t *qubits, uint32_t n_qubits_kept, double *out);
 
+/* out2[0] = Tr rho_A^2 = sum_{a,b} |rho_ab|^2, out2[1] = Tr rho_A = sum_j |psi_j|^2, for rho_A the reduced density
+ * matrix of the k qubits `qubits` (as qipb200_state_reduced_density defines it), on the state AS IT IS (not
+ * renormalised): purity = out2[0] / out2[1]^2 and the Renyi-2 entropy is -ln of it; absent in the reference.  With
+ * s = min(k, n - k), the smaller side, the route depends on s only: s = 0 (k = n) is one norm2 sweep (out2 = {norm2^2,
+ * norm2}); 1 <= s <= 10 is qipb200_state_reduced_density of the side's qubits, with ||rho||_F^2 summed on the host in a
+ * fixed order; s >= 11 is a Gram product G = M M^dagger on the FP64 tensor pipe over the side (M: the state reshaped
+ * to 2^s x 2^(n-s)), two kernels, documented with its summation order and error bound in rustqip_b200/csrc/purity.cu.
+ * Double for f32 and f64 states (f32 amplitudes are widened before they are multiplied), deterministic (same state and
+ * qubits -> bit-identical out2), no floating-point atomics, synchronises.  Errors, all before any device work: NULL
+ * state, NULL qubits, NULL out2, k == 0 or k > n give QIPB200_ERR_INVALID_ARG, a qubit >= n or repeated
+ * QIPB200_ERR_BAD_INDEX, sharded and multi-device states QIPB200_ERR_UNSUPPORTED.  A pending collapse is applied first;
+ * a permuted layout is read as it is. */
+int qipb200_state_purity(qipb200_state *state, const uint64_t *qubits, uint32_t k, double *out2);
+/* Host-only (no GPU, ctx-free): out4 = {route (0 norm2, 1 reduced_density, 2 Gram), s, kernels, Gram blocks} of the
+ * call above on an unsharded n-qubit state with nothing pending.  Kernels: 1, 2^m (2^m + 1) with m = max(0, s - 6), or
+ * 2; Gram blocks (128 x 64 entries of G, those touching its upper triangle): 2^(s-7) (2^(s-7) + 1) on route 2, else 0.
+ * Validates the qubits as the call above does; NULL out4, a bad precision or n_qubits not in 1..40 give
+ * QIPB200_ERR_INVALID_ARG. */
+int qipb200_purity_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, uint32_t k, uint32_t *out4);
+
 /* psi <- exp(-i angles[T-1]/2 P_{T-1}) ... exp(-i angles[0]/2 P_0) psi: Pauli-string rotations, term 0 first; absent in
  * the reference.  Terms are encoded and validated as for qipb200_state_expect_paulis (same codes and messages), with
  * P = i^nY X^x Z^z, so a single 'Z' term is rz(q, angle) and a single 'X' term is Rx(angle); an empty term is the

@@ -485,6 +485,13 @@ class B200State {
                                              reinterpret_cast<double *>(out.data())));
     return out;
   }
+  // {Tr rho_A^2, Tr rho_A} of the qubits `qubits` on the state as it is; purity = first / second^2 (absent in the
+  // reference)
+  std::pair<double, double> purity(const std::vector<uint64_t> &qubits) {
+    double out2[2] = {0.0, 0.0};
+    ctx_.check(qipb200_state_purity(st_, qubits.data(), (uint32_t)qubits.size(), out2));
+    return std::make_pair(out2[0], out2[1]);
+  }
   // a schedule parsed from the QIPS wire format (owned by the library): builder.rs:423-514 on foreign circuits
   void apply_parsed(const qip_op *ops, size_t n_ops, bool fusion = true) {
     ctx_.check(qipb200_state_apply_schedule(st_, ops, n_ops, fusion ? QIPB200_SCHED_DEFAULT : QIPB200_SCHED_NO_FUSION));

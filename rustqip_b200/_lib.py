@@ -32,7 +32,7 @@ EXPORTS = [
     "qipb200_state_sync", "qipb200_state_max_abs_diff", "qipb200_calculate_state", "qipb200_state_measure_probs",
     "qipb200_state_measure_prob", "qipb200_state_soft_measure", "qipb200_state_sample", "qipb200_state_collapse",
     "qipb200_state_measure", "qipb200_state_expect_paulis", "qipb200_expect_plan", "qipb200_state_transition_paulis",
-    "qipb200_transition_plan", "qipb200_state_reduced_density",
+    "qipb200_transition_plan", "qipb200_state_reduced_density", "qipb200_state_purity", "qipb200_purity_plan",
     "qipb200_state_apply_pauli_rotations", "qipb200_pauli_rotation_plan", "qipb200_function_new",
     "qipb200_function_free", "qipb200_state_apply_function", "qipb200_function_plan", "qipb200_function_new_code",
     "qipb200_function_set_params", "qipb200_function_code_compile", "qipb200_function_tabulate",
@@ -117,6 +117,10 @@ def lib():
     L.qipb200_transition_plan.argtypes = [i32, u32, vp, vp, vp, C.c_size_t, vp]
     L.qipb200_state_reduced_density.restype = i32
     L.qipb200_state_reduced_density.argtypes = [vp, vp, u32, vp]
+    L.qipb200_state_purity.restype = i32
+    L.qipb200_state_purity.argtypes = [vp, vp, u32, vp]
+    L.qipb200_purity_plan.restype = i32
+    L.qipb200_purity_plan.argtypes = [i32, u32, vp, u32, vp]
     L.qipb200_state_apply_pauli_rotations.restype = i32
     L.qipb200_state_apply_pauli_rotations.argtypes = [vp, vp, vp, vp, C.c_size_t, vp]
     L.qipb200_pauli_rotation_plan.restype = i32

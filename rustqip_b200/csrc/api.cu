@@ -27,6 +27,7 @@
 #include "function.h"
 #include "gradient.h"
 #include "pauli_rot.h"
+#include "purity.h"
 #include "rdm.h"
 #include "schedule.h"
 #include "tile.cuh"
@@ -2033,6 +2034,107 @@ extern "C" int qipb200_state_reduced_density(qipb200_state *s, const uint64_t *q
     if (s->world > 1 || !s->shards.empty())
       return set_err(s->ctx, QIPB200_ERR_UNSUPPORTED, "reduced_density: sharded states are not supported");
     return rdm_impl(s, qubits, n_qubits_kept, out);
+  });
+}
+
+// ===================================================================================
+// purity of a bipartition (purity.cu)
+// ===================================================================================
+
+namespace {
+
+// The side of the cut: the kept qubits if they are at most half, else their complement (Tr rho_A^2 = Tr rho_B^2).
+std::vector<uint64_t> purity_side(uint32_t n, const uint64_t *qubits, uint32_t k) {
+  std::vector<uint64_t> side;
+  if (k <= n - k) return std::vector<uint64_t>(qubits, qubits + k);
+  uint64_t kept = 0;
+  for (uint32_t i = 0; i < k; ++i) kept |= 1ull << qubits[i];
+  for (uint32_t q = 0; q < n; ++q)
+    if (!((kept >> q) & 1)) side.push_back(q);
+  return side;
+}
+
+int purity_impl(qipb200_state *s, const uint64_t *qubits, uint32_t k, double *out2) {
+  qipb200_ctx *ctx = s->ctx;
+  CU(ctx, cudaSetDevice(ctx->device));
+  int st = materialise_collapse(s);
+  if (st != QIPB200_OK) return st;
+  // A state left permuted (QIPB200_ROTATE) is read where it is, as by reduced_density.
+  const std::vector<uint64_t> side = purity_side(s->n, qubits, k);
+  const uint32_t sb = (uint32_t)side.size();
+  std::vector<uint32_t> pos(sb);
+  uint64_t mask = 0;
+  for (uint32_t i = 0; i < sb; ++i) {
+    pos[i] = s->phys_of_logical[s->n - 1 - (uint32_t)side[i]];
+    mask |= 1ull << pos[i];
+  }
+  switch (purity_route(sb)) {
+    case 0: {
+      double v = 0.0;
+      CU(ctx, run_purity_norm2(s->prec, s->buf, s->n_local, &v, ctx->stream, &ctx->launches));
+      out2[0] = v * v;
+      out2[1] = v;
+      return QIPB200_OK;
+    }
+    case 1: {
+      // ||rho||_F^2 in a fixed order: each row's |rho_ab|^2 in column order, then the rows in order
+      const size_t K = (size_t)1 << sb;
+      std::vector<double> rho(2 * K * K);
+      CU(ctx, run_reduced_density(s->prec, s->buf, s->n_local, pos.data(), sb, rho.data(), ctx->stream,
+                                  &ctx->launches));
+      double p = 0.0, tr = 0.0;
+      for (size_t a = 0; a < K; ++a) {
+        double row = 0.0;
+        for (size_t b = 0; b < K; ++b) {
+          row = std::fma(rho[2 * (a * K + b)], rho[2 * (a * K + b)], row);
+          row = std::fma(rho[2 * (a * K + b) + 1], rho[2 * (a * K + b) + 1], row);
+        }
+        p += row;
+        tr += rho[2 * (a * K + a)];
+      }
+      out2[0] = p;
+      out2[1] = tr;
+      return QIPB200_OK;
+    }
+    default:
+      CU(ctx, run_purity_gram(s->prec, s->buf, s->n_local, mask, out2, ctx->stream, &ctx->launches));
+      return QIPB200_OK;
+  }
+}
+
+}  // namespace
+
+extern "C" int qipb200_state_purity(qipb200_state *s, const uint64_t *qubits, uint32_t k, double *out2) {
+  if (!s) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, "purity: NULL state");
+  return guarded(s->ctx, [&]() -> int {
+    if (!out2) return set_err(s->ctx, QIPB200_ERR_INVALID_ARG, "purity: NULL out2");
+    int st = check_indices(s, qubits, k);
+    if (st != QIPB200_OK) return st;
+    if (s->world > 1 || !s->shards.empty())
+      return set_err(s->ctx, QIPB200_ERR_UNSUPPORTED, "purity: sharded states are not supported");
+    return purity_impl(s, qubits, k, out2);
+  });
+}
+
+extern "C" int qipb200_purity_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, uint32_t k,
+                                   uint32_t *out4) {
+  if (!out4 || (prec != QIP_F32 && prec != QIP_F64) || n_qubits == 0 || n_qubits > 40)
+    return set_err(nullptr, QIPB200_ERR_INVALID_ARG, "purity_plan: NULL out4, bad precision or n_qubits not in 1..40");
+  if (!qubits || k == 0 || k > n_qubits)
+    return set_err(nullptr, QIPB200_ERR_INVALID_ARG, "purity_plan: bad qubit list");
+  return guarded(nullptr, [&]() -> int {
+    uint64_t seen = 0;
+    for (uint32_t i = 0; i < k; ++i) {
+      if (qubits[i] >= n_qubits) return set_err(nullptr, QIPB200_ERR_BAD_INDEX, "purity_plan: qubit index out of range");
+      if ((seen >> qubits[i]) & 1) return set_err(nullptr, QIPB200_ERR_BAD_INDEX, "purity_plan: repeated qubit index");
+      seen |= 1ull << qubits[i];
+    }
+    const uint32_t sb = std::min(k, n_qubits - k);
+    out4[0] = purity_route(sb);
+    out4[1] = sb;
+    out4[2] = (uint32_t)purity_launch_count(sb);
+    out4[3] = out4[0] == 2 ? (uint32_t)purity_gram_blocks(sb) : 0;
+    return (int)QIPB200_OK;
   });
 }
 

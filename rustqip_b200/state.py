@@ -488,6 +488,26 @@ class State:
         self._chk(_lib.lib().qipb200_state_reduced_density(self._h, _ptr(idx) if k else None, k, _ptr(out)))
         return out.reshape(1 << k, 1 << k)
 
+    def _purity2(self, qubits):
+        idx = np.ascontiguousarray(np.asarray(list(qubits), dtype=np.uint64))
+        out2 = np.zeros(2)
+        self._chk(_lib.lib().qipb200_state_purity(self._h, _ptr(idx) if len(idx) else None, len(idx), _ptr(out2)))
+        return float(out2[0]), float(out2[1])
+
+    def purity(self, qubits: Sequence[int]) -> float:
+        """Tr rho_A^2 = sum_{a,b} |rho_ab|^2 of the reduced density matrix of ``qubits`` on the state as it is (not
+        renormalised: divide by ``norm2()**2`` for a state that is not a unit vector), computed on the device.
+
+        The route depends on s = min(k, n - k): one norm2 sweep for k = n, ``reduced_density`` of the smaller side for
+        s <= 10, and a Gram product on the FP64 tensor pipe above (``purity_plan`` reports it).  Deterministic."""
+        return self._purity2(qubits)[0]
+
+    def renyi2_entropy(self, qubits: Sequence[int]) -> float:
+        """S_2 = -ln(Tr rho_A^2 / (Tr rho_A)^2) of ``qubits``: the Renyi-2 entanglement entropy across the cut, with
+        the state normalised on the fly (one device call)."""
+        p, tr = self._purity2(qubits)
+        return -float(np.log(p / (tr * tr)))
+
     # -- multi-GPU --------------------------------------------------------------
     def ipc_export(self):
         a = (C.c_ubyte * _lib.IPC_HANDLE_BYTES)()
@@ -667,6 +687,16 @@ def transition_plan(n: int, dtype, terms):
     _lib.check(_lib.lib().qipb200_transition_plan(prec_of(dtype), int(n), _ptr(qs), ls, _ptr(lens), lens.shape[0], v),
                None)
     return int(v[0]), int(v[1])
+
+
+def purity_plan(n: int, dtype, qubits):
+    """(route, s, kernels, Gram blocks) of State.purity for these qubits on an unsharded n-qubit state (needs no GPU):
+    route 0 is norm2 (k = n), 1 reduced_density (s <= 10), 2 the Gram kernel; s = min(k, n - k)."""
+    idx = np.ascontiguousarray(np.asarray(list(qubits), dtype=np.uint64))
+    v = (C.c_uint32 * 4)()
+    _lib.check(_lib.lib().qipb200_purity_plan(prec_of(dtype), int(n), _ptr(idx) if len(idx) else None, len(idx), v),
+               None)
+    return tuple(int(x) for x in v)
 
 
 def pauli_rotation_plan(n: int, dtype, terms) -> int:
