@@ -549,15 +549,21 @@ double collapse_multiplier(qip_prec prec, double measured_prob) {
   return 1.0 / sqrt(measured_prob);
 }
 
+// The index bit of s that holds each of k qubits under the current layout: qubit q is logical bit n - 1 - q.
+void phys_positions(const qipb200_state *s, const uint64_t *qubits, uint32_t k, uint32_t *pos) {
+  for (uint32_t i = 0; i < k; ++i) pos[i] = s->phys_of_logical[s->n - 1 - (uint32_t)qubits[i]];
+}
+
 // measure_state with a known multiplier over this rank's amplitudes, under the current layout.
 int launch_collapse_on(qipb200_state *s, const uint64_t *qubits, uint32_t n_qubits, uint64_t measured, double p_mult) {
   qipb200_ctx *ctx = s->ctx;
   CU(ctx, cudaSetDevice(ctx->device));
+  uint32_t pos[64];  // distinct qubits of at most 40
+  phys_positions(s, qubits, n_qubits, pos);
   uint64_t row_mask = 0, measured_mask = 0;
   for (uint32_t i = 0; i < n_qubits; ++i) {
-    const uint32_t bit = s->phys_of_logical[s->n - 1 - (uint32_t)qubits[i]];
-    row_mask |= 1ull << bit;
-    measured_mask |= ((measured >> i) & 1ull) << bit;
+    row_mask |= 1ull << pos[i];
+    measured_mask |= ((measured >> i) & 1ull) << pos[i];
   }
   CU(ctx, launch_collapse(s->prec, s->buf, 1ull << s->n_local, (uint64_t)s->rank << s->n_local, row_mask,
                           measured_mask, p_mult, ctx->stream, &ctx->launches));
@@ -570,6 +576,12 @@ int materialise_collapse(qipb200_state *s) {
   s->collapse_pending = false;
   return launch_collapse_on(s, s->pend_qubits.data(), (uint32_t)s->pend_qubits.size(), s->pend_measured,
                             s->pend_p_mult);
+}
+
+// s's device made current and its pending collapse applied: the start of every call that reads s.
+int begin_device_work(qipb200_state *s) {
+  CU(s->ctx, cudaSetDevice(s->ctx->device));
+  return materialise_collapse(s);
 }
 
 int check_barrier_error(qipb200_state *s) {
@@ -1211,8 +1223,7 @@ static int transfer_impl(qipb200_state *s, void *host, uint64_t offset, uint64_t
   if (!host && len) return set_err(ctx, QIPB200_ERR_INVALID_ARG, std::string(what) + ": host pointer is NULL");
   if (len > (1ull << s->n_local) || offset > (1ull << s->n_local) - len)
     return set_err(ctx, QIPB200_ERR_SIZE_MISMATCH, std::string(what) + ": range exceeds the local state");
-  CU(ctx, cudaSetDevice(ctx->device));
-  int st = materialise_collapse(s);  // a partial upload keeps the other amplitudes
+  int st = begin_device_work(s);  // a partial upload keeps the other amplitudes
   if (st != QIPB200_OK) return st;
   if (!layout_is_identity(s)) {
     st = restore_layout(s);
@@ -1262,8 +1273,7 @@ extern "C" int qipb200_state_download(qipb200_state *s, void *host, uint64_t off
 }
 
 static int apply_op_impl(qipb200_state *s, const qip_op *op) {
-  CU(s->ctx, cudaSetDevice(s->ctx->device));
-  int st = materialise_collapse(s);
+  int st = begin_device_work(s);
   if (st != QIPB200_OK) return st;
   FlatOp f;
   st = compile_and_localize(s, op, &f, nullptr);
@@ -1324,8 +1334,7 @@ extern "C" int qipb200_state_apply_schedule(qipb200_state *s, const qip_op *ops,
 // sum |a|^2 of the WHOLE state: on a sharded state the per-rank sums are all-reduced (collective call).
 static int norm2_impl(qipb200_state *s, double *out) {
   qipb200_ctx *ctx = s->ctx;
-  CU(ctx, cudaSetDevice(ctx->device));
-  int st = materialise_collapse(s);
+  int st = begin_device_work(s);
   if (st != QIPB200_OK) return st;
   CU(ctx, launch_norm2(s->prec, s->buf, 1ull << s->n_local, ctx->d_scalar, ctx->stream, &ctx->launches));
   st = allreduce_sum(s, ctx->d_scalar, 1);
@@ -1354,8 +1363,7 @@ static int max_abs_diff_impl(qipb200_state *a, qipb200_state *b, double *out) {
     return set_err(ctx, QIPB200_ERR_SIZE_MISMATCH, "max_abs_diff: the two states differ in context, precision or shape");
   if (a->phys_of_logical != b->phys_of_logical)
     return set_err(ctx, QIPB200_ERR_UNSUPPORTED, "max_abs_diff: the two sharded states hold different qubit layouts");
-  CU(ctx, cudaSetDevice(ctx->device));
-  int st = materialise_collapse(a);
+  int st = begin_device_work(a);
   if (st == QIPB200_OK) st = materialise_collapse(b);
   if (st != QIPB200_OK) return st;
   CU(ctx, launch_max_abs_diff(a->prec, a->buf, b->buf, 1ull << a->n_local, ctx->d_scalar, ctx->stream, &ctx->launches));
@@ -1568,11 +1576,10 @@ int measure_probs_impl(qipb200_state *s, const uint64_t *indices, uint32_t n_ind
   if (n_indices > 26) return set_err(ctx, QIPB200_ERR_UNSUPPORTED, "measure_probs: more than 26 measured qubits");
   if (s->world > 1 && (1u << n_indices) > (uint32_t)kCommDoubles)
     return set_err(ctx, QIPB200_ERR_UNSUPPORTED, "measure_probs on a sharded state: more than 16 measured qubits");
-  CU(ctx, cudaSetDevice(ctx->device));
-  int st = materialise_collapse(s);
+  int st = begin_device_work(s);
   if (st != QIPB200_OK) return st;
   uint32_t bitpos[32];
-  for (uint32_t i = 0; i < n_indices; ++i) bitpos[i] = s->phys_of_logical[s->n - 1 - (uint32_t)indices[i]];
+  phys_positions(s, indices, n_indices, bitpos);
   double *d_hist = nullptr;
   CU(ctx, cudaMallocAsync((void **)&d_hist, sizeof(double) << n_indices, ctx->stream));
   CU(ctx, launch_measure_probs(s->prec, s->buf, 1ull << s->n_local, (uint64_t)s->rank << s->n_local, bitpos,
@@ -1636,8 +1643,7 @@ int local_scan(qipb200_state *s, double rem, bool *crossed, uint64_t *idx_out) {
 
 int soft_measure_impl(qipb200_state *s, const uint64_t *indices, uint32_t n_indices, double r, uint64_t *measured) {
   qipb200_ctx *ctx = s->ctx;
-  CU(ctx, cudaSetDevice(ctx->device));
-  int st0 = materialise_collapse(s);
+  int st0 = begin_device_work(s);
   if (st0 != QIPB200_OK) return st0;
   uint64_t idx = 0;  // the reference leaves measured_indx = 0 when the scan never crosses
   if (s->world == 1) {
@@ -1705,8 +1711,7 @@ int sample_impl(qipb200_state *s, const uint64_t *indices, uint32_t n_indices, c
                 uint64_t *measured) {
   qipb200_ctx *ctx = s->ctx;
   if (n_draws > 0xffffffffull) return set_err(ctx, QIPB200_ERR_UNSUPPORTED, "sample: more than 2^32-1 draws in one call");
-  CU(ctx, cudaSetDevice(ctx->device));
-  int st = materialise_collapse(s);
+  int st = begin_device_work(s);
   if (st != QIPB200_OK) return st;
   if (!layout_is_identity(s)) {
     st = restore_layout(s);
@@ -1733,8 +1738,7 @@ int sample_impl(qipb200_state *s, const uint64_t *indices, uint32_t n_indices, c
 }
 
 int collapse_impl(qipb200_state *s, const uint64_t *indices, uint32_t n_indices, uint64_t measured, double measured_prob) {
-  CU(s->ctx, cudaSetDevice(s->ctx->device));
-  int st = materialise_collapse(s);
+  int st = begin_device_work(s);
   if (st != QIPB200_OK) return st;
   if (measured_prob == 0.0) return QIPB200_OK;  // measurement_ops.rs:230: untouched
   return launch_collapse_on(s, indices, n_indices, measured, collapse_multiplier(s->prec, measured_prob));
@@ -1745,8 +1749,7 @@ int collapse_impl(qipb200_state *s, const uint64_t *indices, uint32_t n_indices,
 int measure_impl(qipb200_state *s, const uint64_t *indices, uint32_t n_indices, double r, uint32_t flags,
                  uint64_t *measured, double *prob) {
   qipb200_ctx *ctx = s->ctx;
-  CU(ctx, cudaSetDevice(ctx->device));
-  int st = materialise_collapse(s);
+  int st = begin_device_work(s);
   if (st != QIPB200_OK) return st;
   MeasureRecord rec = {(flags & QIPB200_MEASURE_FORCED) ? *measured : 0, 0.0};
   if (flags & QIPB200_MEASURE_FORCED_PROB) {
@@ -1895,6 +1898,76 @@ extern "C" int qipb200_state_collapse(qipb200_state *s, const uint64_t *indices,
 
 namespace {
 
+// The checks the feature entries below share: each returns QIPB200_OK or the status of the refusal it reported.
+
+// The Pauli term list of an n-qubit state, or parse_pauli_terms' refusal reported on ctx.
+int parse_terms(const qipb200_ctx *ctx, uint32_t n, const uint64_t *qubits, const char *paulis, const uint32_t *term_len,
+                size_t n_terms, std::vector<PauliTerm> *terms) {
+  std::string err;
+  const int st = parse_pauli_terms(n, qubits, paulis, term_len, n_terms, terms, &err);
+  return st == QIPB200_OK ? st : set_err(ctx, st, err);
+}
+
+// The preconditions of every host-only plan: its outputs (named outs) given, a known precision and 1..40 qubits.
+int check_plan_args(const std::string &who, qip_prec prec, uint32_t n_qubits, bool outs_present, const char *outs) {
+  if (outs_present && (prec == QIP_F32 || prec == QIP_F64) && n_qubits >= 1 && n_qubits <= 40) return QIPB200_OK;
+  return set_err(nullptr, QIPB200_ERR_INVALID_ARG, who + ": NULL " + outs + ", bad precision or n_qubits not in 1..40");
+}
+
+int require_unsharded(const qipb200_state *s, const std::string &who) {
+  if (s->world > 1 || !s->shards.empty())
+    return set_err(s->ctx, QIPB200_ERR_UNSUPPORTED, who + ": sharded states are not supported");
+  return QIPB200_OK;
+}
+
+// Context, precision and size, then sharding: the checks every call on two states makes.
+int check_compatible(const qipb200_state *a, const qipb200_state *b, const std::string &who) {
+  if (a->ctx != b->ctx || a->prec != b->prec || a->n != b->n)
+    return set_err(a->ctx, QIPB200_ERR_SIZE_MISMATCH, who + ": the states differ in context, precision or size");
+  int st = require_unsharded(a, who);
+  if (st == QIPB200_OK) st = require_unsharded(b, who);
+  return st;
+}
+
+// dst == src first: an out-of-place call cannot read the state it writes.
+int check_state_pair(const qipb200_state *dst, const qipb200_state *src, const std::string &who) {
+  if (dst == src) return set_err(dst->ctx, QIPB200_ERR_INVALID_ARG, who + ": the two states must differ");
+  return check_compatible(dst, src, who);
+}
+
+// A state and the two work states it is evolved through.
+int check_three_states(const qipb200_state *state, const qipb200_state *work_a, const qipb200_state *work_b,
+                       const std::string &who) {
+  if (state == work_a || state == work_b || work_a == work_b)
+    return set_err(state->ctx, QIPB200_ERR_INVALID_ARG, who + ": the three states must differ");
+  int st = check_compatible(work_a, state, who);
+  if (st == QIPB200_OK) st = check_compatible(work_b, state, who);
+  return st;
+}
+
+int check_finite(qipb200_ctx *ctx, const double *v, size_t n, const std::string &who, const char *what) {
+  if (n && !v) return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL " + what + "s");
+  for (size_t t = 0; t < n; ++t)
+    if (!std::isfinite(v[t]))
+      return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": " + what + " " + std::to_string(t) + " is not finite");
+  return QIPB200_OK;
+}
+
+// src's pending collapse runs, dst's is dropped (dst is overwritten), and dst takes src's layout.
+int prepare_out_of_place(qipb200_state *dst, qipb200_state *src) {
+  int st = materialise_collapse(src);
+  if (st != QIPB200_OK) return st;
+  dst->collapse_pending = false;
+  dst->phys_of_logical = src->phys_of_logical;
+  return QIPB200_OK;
+}
+
+int prepare_work_states(qipb200_state *state, qipb200_state *work_a, qipb200_state *work_b) {
+  int st = prepare_out_of_place(work_a, state);
+  if (st == QIPB200_OK) st = prepare_out_of_place(work_b, state);
+  return st;
+}
+
 // Logical masks -> physical index bits of s (a permuted layout needs no restore sweep: Pauli masks permute with bits).
 std::vector<PauliTerm> phys_terms(const qipb200_state *s, const std::vector<PauliTerm> &terms) {
   std::vector<PauliTerm> phys(terms.size());
@@ -1911,8 +1984,7 @@ std::vector<PauliTerm> phys_terms(const qipb200_state *s, const std::vector<Paul
 
 int expect_impl(qipb200_state *s, const std::vector<PauliTerm> &terms, double *out) {
   qipb200_ctx *ctx = s->ctx;
-  CU(ctx, cudaSetDevice(ctx->device));
-  int st = materialise_collapse(s);
+  int st = begin_device_work(s);
   if (st != QIPB200_OK) return st;
   // A state left permuted (QIPB200_ROTATE) needs no restore_layout sweep: Pauli masks permute with the bits.
   const std::vector<PauliTerm> phys = phys_terms(s, terms);
@@ -1927,11 +1999,9 @@ extern "C" int qipb200_state_expect_paulis(qipb200_state *s, const uint64_t *qub
   if (!s) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, "expect_paulis: NULL state");
   return guarded(s->ctx, [&]() -> int {
     std::vector<PauliTerm> terms;
-    std::string err;
-    int st = parse_pauli_terms(s->n, qubits, paulis, term_len, n_terms, &terms, &err);
-    if (st != QIPB200_OK) return set_err(s->ctx, st, err);
-    if (s->world > 1 || !s->shards.empty())
-      return set_err(s->ctx, QIPB200_ERR_UNSUPPORTED, "expect_paulis: sharded states are not supported");
+    int st = parse_terms(s->ctx, s->n, qubits, paulis, term_len, n_terms, &terms);
+    if (st == QIPB200_OK) st = require_unsharded(s, "expect_paulis");
+    if (st != QIPB200_OK) return st;
     if (n_terms == 0) return (int)QIPB200_OK;
     if (!out) return set_err(s->ctx, QIPB200_ERR_INVALID_ARG, "expect_paulis: NULL out");
     return expect_impl(s, terms, out);
@@ -1940,13 +2010,11 @@ extern "C" int qipb200_state_expect_paulis(qipb200_state *s, const uint64_t *qub
 
 extern "C" int qipb200_expect_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, const char *paulis,
                                    const uint32_t *term_len, size_t n_terms, uint32_t *sweeps) {
-  if (!sweeps || (prec != QIP_F32 && prec != QIP_F64) || n_qubits == 0 || n_qubits > 40)
-    return set_err(nullptr, QIPB200_ERR_INVALID_ARG, "expect_plan: NULL sweeps, bad precision or n_qubits not in 1..40");
   return guarded(nullptr, [&]() -> int {
     std::vector<PauliTerm> terms;
-    std::string err;
-    int st = parse_pauli_terms(n_qubits, qubits, paulis, term_len, n_terms, &terms, &err);
-    if (st != QIPB200_OK) return set_err(nullptr, st, err);
+    int st = check_plan_args("expect_plan", prec, n_qubits, sweeps, "sweeps");
+    if (st == QIPB200_OK) st = parse_terms(nullptr, n_qubits, qubits, paulis, term_len, n_terms, &terms);
+    if (st != QIPB200_OK) return st;
     *sweeps = expect_sweep_count(n_qubits, terms);
     return (int)QIPB200_OK;
   });
@@ -1960,18 +2028,13 @@ extern "C" int qipb200_state_transition_paulis(qipb200_state *bra, qipb200_state
   return guarded(bra->ctx, [&]() -> int {
     // every check runs before any device work: a refused call leaves both states (and a pending collapse) as they were
     std::vector<PauliTerm> terms;
-    std::string err;
-    int st = parse_pauli_terms(bra->n, qubits, paulis, term_len, n_terms, &terms, &err);
-    if (st != QIPB200_OK) return set_err(bra->ctx, st, err);
-    if (bra->ctx != ket->ctx || bra->prec != ket->prec || bra->n != ket->n)
-      return set_err(bra->ctx, QIPB200_ERR_SIZE_MISMATCH, who + ": the states differ in context, precision or size");
-    if (bra->world > 1 || !bra->shards.empty() || ket->world > 1 || !ket->shards.empty())
-      return set_err(bra->ctx, QIPB200_ERR_UNSUPPORTED, who + ": sharded states are not supported");
+    int st = parse_terms(bra->ctx, bra->n, qubits, paulis, term_len, n_terms, &terms);
+    if (st == QIPB200_OK) st = check_compatible(bra, ket, who);  // bra == ket is allowed
+    if (st != QIPB200_OK) return st;
     if (n_terms == 0) return (int)QIPB200_OK;
     if (!out) return set_err(bra->ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL out");
     qipb200_ctx *ctx = bra->ctx;
-    CU(ctx, cudaSetDevice(ctx->device));
-    if ((st = materialise_collapse(bra)) != QIPB200_OK) return st;
+    if ((st = begin_device_work(bra)) != QIPB200_OK) return st;
     if ((st = materialise_collapse(ket)) != QIPB200_OK) return st;
     // One qubit map: the states are read where they are (Pauli masks permute with the bits).  Two maps: each permuted
     // state goes back to the canonical layout first, as before a download.
@@ -1987,14 +2050,11 @@ extern "C" int qipb200_state_transition_paulis(qipb200_state *bra, qipb200_state
 
 extern "C" int qipb200_transition_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, const char *paulis,
                                        const uint32_t *term_len, size_t n_terms, uint32_t *out2) {
-  if (!out2 || (prec != QIP_F32 && prec != QIP_F64) || n_qubits == 0 || n_qubits > 40)
-    return set_err(nullptr, QIPB200_ERR_INVALID_ARG,
-                   "transition_plan: NULL out2, bad precision or n_qubits not in 1..40");
   return guarded(nullptr, [&]() -> int {
     std::vector<PauliTerm> terms;
-    std::string err;
-    int st = parse_pauli_terms(n_qubits, qubits, paulis, term_len, n_terms, &terms, &err);
-    if (st != QIPB200_OK) return set_err(nullptr, st, err);
+    int st = check_plan_args("transition_plan", prec, n_qubits, out2, "out2");
+    if (st == QIPB200_OK) st = parse_terms(nullptr, n_qubits, qubits, paulis, term_len, n_terms, &terms);
+    if (st != QIPB200_OK) return st;
     out2[0] = out2[1] = 0;
     if (!terms.empty()) transition_plan_counts(n_qubits, terms, out2);
     return (int)QIPB200_OK;
@@ -2009,12 +2069,11 @@ namespace {
 
 int rdm_impl(qipb200_state *s, const uint64_t *qubits, uint32_t k, double *out) {
   qipb200_ctx *ctx = s->ctx;
-  CU(ctx, cudaSetDevice(ctx->device));
-  int st = materialise_collapse(s);
+  int st = begin_device_work(s);
   if (st != QIPB200_OK) return st;
   // A state left permuted (QIPB200_ROTATE) needs no restore_layout sweep: the kept qubits are read where they are.
   uint32_t pos[kRdmMaxKept];
-  for (uint32_t i = 0; i < k; ++i) pos[i] = s->phys_of_logical[s->n - 1 - (uint32_t)qubits[i]];
+  phys_positions(s, qubits, k, pos);
   CU(ctx, run_reduced_density(s->prec, s->buf, s->n_local, pos, k, out, ctx->stream, &ctx->launches));
   return QIPB200_OK;
 }
@@ -2031,8 +2090,7 @@ extern "C" int qipb200_state_reduced_density(qipb200_state *s, const uint64_t *q
     if (n_qubits_kept > kRdmMaxKept)
       return set_err(s->ctx, QIPB200_ERR_UNSUPPORTED,
                      "reduced_density: at most 10 kept qubits (the output at 10 is already 16 MiB)");
-    if (s->world > 1 || !s->shards.empty())
-      return set_err(s->ctx, QIPB200_ERR_UNSUPPORTED, "reduced_density: sharded states are not supported");
+    if ((st = require_unsharded(s, "reduced_density")) != QIPB200_OK) return st;
     return rdm_impl(s, qubits, n_qubits_kept, out);
   });
 }
@@ -2056,18 +2114,15 @@ std::vector<uint64_t> purity_side(uint32_t n, const uint64_t *qubits, uint32_t k
 
 int purity_impl(qipb200_state *s, const uint64_t *qubits, uint32_t k, double *out2) {
   qipb200_ctx *ctx = s->ctx;
-  CU(ctx, cudaSetDevice(ctx->device));
-  int st = materialise_collapse(s);
+  int st = begin_device_work(s);
   if (st != QIPB200_OK) return st;
   // A state left permuted (QIPB200_ROTATE) is read where it is, as by reduced_density.
   const std::vector<uint64_t> side = purity_side(s->n, qubits, k);
   const uint32_t sb = (uint32_t)side.size();
   std::vector<uint32_t> pos(sb);
+  phys_positions(s, side.data(), sb, pos.data());
   uint64_t mask = 0;
-  for (uint32_t i = 0; i < sb; ++i) {
-    pos[i] = s->phys_of_logical[s->n - 1 - (uint32_t)side[i]];
-    mask |= 1ull << pos[i];
-  }
+  for (uint32_t i = 0; i < sb; ++i) mask |= 1ull << pos[i];
   switch (purity_route(sb)) {
     case 0: {
       double v = 0.0;
@@ -2109,20 +2164,19 @@ extern "C" int qipb200_state_purity(qipb200_state *s, const uint64_t *qubits, ui
   return guarded(s->ctx, [&]() -> int {
     if (!out2) return set_err(s->ctx, QIPB200_ERR_INVALID_ARG, "purity: NULL out2");
     int st = check_indices(s, qubits, k);
+    if (st == QIPB200_OK) st = require_unsharded(s, "purity");
     if (st != QIPB200_OK) return st;
-    if (s->world > 1 || !s->shards.empty())
-      return set_err(s->ctx, QIPB200_ERR_UNSUPPORTED, "purity: sharded states are not supported");
     return purity_impl(s, qubits, k, out2);
   });
 }
 
 extern "C" int qipb200_purity_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, uint32_t k,
                                    uint32_t *out4) {
-  if (!out4 || (prec != QIP_F32 && prec != QIP_F64) || n_qubits == 0 || n_qubits > 40)
-    return set_err(nullptr, QIPB200_ERR_INVALID_ARG, "purity_plan: NULL out4, bad precision or n_qubits not in 1..40");
-  if (!qubits || k == 0 || k > n_qubits)
-    return set_err(nullptr, QIPB200_ERR_INVALID_ARG, "purity_plan: bad qubit list");
   return guarded(nullptr, [&]() -> int {
+    const int st = check_plan_args("purity_plan", prec, n_qubits, out4, "out4");
+    if (st != QIPB200_OK) return st;
+    if (!qubits || k == 0 || k > n_qubits)
+      return set_err(nullptr, QIPB200_ERR_INVALID_ARG, "purity_plan: bad qubit list");
     uint64_t seen = 0;
     for (uint32_t i = 0; i < k; ++i) {
       if (qubits[i] >= n_qubits) return set_err(nullptr, QIPB200_ERR_BAD_INDEX, "purity_plan: qubit index out of range");
@@ -2146,8 +2200,7 @@ namespace {
 
 int pauli_rot_impl(qipb200_state *s, const std::vector<PauliTerm> &terms, const double *angles) {
   qipb200_ctx *ctx = s->ctx;
-  CU(ctx, cudaSetDevice(ctx->device));
-  int st = materialise_collapse(s);
+  int st = begin_device_work(s);
   if (st != QIPB200_OK) return st;
   // A state left permuted (QIPB200_ROTATE) is rotated where it is: Pauli masks permute with the bits.
   const std::vector<PauliTerm> phys = phys_terms(s, terms);
@@ -2163,17 +2216,12 @@ extern "C" int qipb200_state_apply_pauli_rotations(qipb200_state *s, const uint6
   if (!s) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, "apply_pauli_rotations: NULL state");
   return guarded(s->ctx, [&]() -> int {
     // every term and angle is checked before any device work: a refused call leaves the state as it was
+    const char *who = "apply_pauli_rotations";
     std::vector<PauliTerm> terms;
-    std::string err;
-    int st = parse_pauli_terms(s->n, qubits, paulis, term_len, n_terms, &terms, &err);
-    if (st != QIPB200_OK) return set_err(s->ctx, st, err);
-    if (n_terms && !angles) return set_err(s->ctx, QIPB200_ERR_INVALID_ARG, "apply_pauli_rotations: NULL angles");
-    for (size_t t = 0; t < n_terms; ++t)
-      if (!std::isfinite(angles[t]))
-        return set_err(s->ctx, QIPB200_ERR_INVALID_ARG,
-                       "apply_pauli_rotations: angle " + std::to_string(t) + " is not finite");
-    if (s->world > 1 || !s->shards.empty())
-      return set_err(s->ctx, QIPB200_ERR_UNSUPPORTED, "apply_pauli_rotations: sharded states are not supported");
+    int st = parse_terms(s->ctx, s->n, qubits, paulis, term_len, n_terms, &terms);
+    if (st == QIPB200_OK) st = check_finite(s->ctx, angles, n_terms, who, "angle");
+    if (st == QIPB200_OK) st = require_unsharded(s, who);
+    if (st != QIPB200_OK) return st;
     if (n_terms == 0) return (int)QIPB200_OK;
     return pauli_rot_impl(s, terms, angles);
   });
@@ -2182,14 +2230,11 @@ extern "C" int qipb200_state_apply_pauli_rotations(qipb200_state *s, const uint6
 extern "C" int qipb200_pauli_rotation_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits,
                                            const char *paulis, const uint32_t *term_len, size_t n_terms,
                                            uint32_t *sweeps) {
-  if (!sweeps || (prec != QIP_F32 && prec != QIP_F64) || n_qubits == 0 || n_qubits > 40)
-    return set_err(nullptr, QIPB200_ERR_INVALID_ARG,
-                   "pauli_rotation_plan: NULL sweeps, bad precision or n_qubits not in 1..40");
   return guarded(nullptr, [&]() -> int {
     std::vector<PauliTerm> terms;
-    std::string err;
-    int st = parse_pauli_terms(n_qubits, qubits, paulis, term_len, n_terms, &terms, &err);
-    if (st != QIPB200_OK) return set_err(nullptr, st, err);
+    int st = check_plan_args("pauli_rotation_plan", prec, n_qubits, sweeps, "sweeps");
+    if (st == QIPB200_OK) st = parse_terms(nullptr, n_qubits, qubits, paulis, term_len, n_terms, &terms);
+    if (st != QIPB200_OK) return st;
     *sweeps = pauli_rotation_sweep_count(n_qubits, terms);
     return (int)QIPB200_OK;
   });
@@ -2287,6 +2332,11 @@ int code_fail(const qipb200_ctx *ctx, const std::string &who, int st, const std:
   return set_err(ctx, st, who + what + msg);
 }
 
+// A code-function call that failed with e: the driver's launch error in err when it gave one, else e of what.
+int code_error(const qipb200_ctx *ctx, const std::string &who, cudaError_t e, const std::string &err, const char *what) {
+  return err.empty() ? cuda_fail(ctx, e, what) : set_err(ctx, QIPB200_ERR_CUDA, who + ": " + err);
+}
+
 // theta(x, params) is finite for every x < 2^n_in, or the error that names the first x where it is not.
 int check_code_theta(qipb200_function *fn, const double *params, const std::string &who) {
   qipb200_ctx *ctx = fn->ctx;
@@ -2295,8 +2345,7 @@ int check_code_theta(qipb200_function *fn, const double *params, const std::stri
   cudaError_t e = function_code_first_bad(fn->code, false, fn->n_in, fn->n_out, params, (uint64_t *)fn->d_scratch,
                                           ctx->sm_count, ctx->stream, &first, &err);
   ++ctx->launches;
-  if (e != cudaSuccess)
-    return err.empty() ? cuda_fail(ctx, e, "function_code_first_bad") : set_err(ctx, QIPB200_ERR_CUDA, who + ": " + err);
+  if (e != cudaSuccess) return code_error(ctx, who, e, err, "function_code_first_bad");
   if (first != ~0ull)
     return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": theta(" + std::to_string(first) + ") is not finite");
   return QIPB200_OK;
@@ -2380,23 +2429,21 @@ extern "C" int qipb200_state_apply_function(qipb200_state *s, const qipb200_func
   return guarded(s->ctx, [&]() -> int {
     // every check runs before any device work: a refused call leaves the state (and a pending collapse) as it was
     int st = check_function_registers(s->ctx, who, s->n, in_qubits, fn->n_in, out_qubits, fn->n_out);
+    if (st == QIPB200_OK) st = require_unsharded(s, who);
     if (st != QIPB200_OK) return st;
-    if (s->world > 1 || !s->shards.empty())
-      return set_err(s->ctx, QIPB200_ERR_UNSUPPORTED, who + ": sharded states are not supported");
     if (fn->ctx != s->ctx)
       return set_err(s->ctx, QIPB200_ERR_INVALID_ARG, who + ": the function was made on another context");
     qipb200_ctx *ctx = s->ctx;
-    CU(ctx, cudaSetDevice(ctx->device));
-    if ((st = materialise_collapse(s)) != QIPB200_OK) return st;
+    if ((st = begin_device_work(s)) != QIPB200_OK) return st;
     // A permuted layout (QIPB200_ROTATE) needs no restore: the registers are read and written where their qubits are.
     uint32_t in_pos[kFnCodeMaxBits], out_pos[kFnMaxOut];
-    for (uint32_t i = 0; i < fn->n_in; ++i) in_pos[i] = s->phys_of_logical[s->n - 1 - (uint32_t)in_qubits[i]];
-    for (uint32_t i = 0; i < fn->n_out; ++i) out_pos[i] = s->phys_of_logical[s->n - 1 - (uint32_t)out_qubits[i]];
+    phys_positions(s, in_qubits, fn->n_in, in_pos);
+    phys_positions(s, out_qubits, fn->n_out, out_pos);
     if (fn->code) {
       std::string err;
       const cudaError_t e = run_function_code(s->prec, s->buf, s->n_local, in_pos, fn->n_in, out_pos, fn->n_out,
                                               fn->code, fn->params, ctx->sm_count, ctx->stream, &ctx->launches, &err);
-      if (e != cudaSuccess) return err.empty() ? cuda_fail(ctx, e, "run_function_code") : set_err(ctx, QIPB200_ERR_CUDA, who + ": " + err);
+      if (e != cudaSuccess) return code_error(ctx, who, e, err, "run_function_code");
       return (int)QIPB200_OK;
     }
     CU(ctx, run_function(s->prec, s->buf, s->n_local, in_pos, fn->n_in, out_pos, fn->n_out, fn->d_f, fn->d_cs,
@@ -2408,13 +2455,11 @@ extern "C" int qipb200_state_apply_function(qipb200_state *s, const qipb200_func
 extern "C" int qipb200_function_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *in_qubits, uint32_t n_in,
                                      const uint64_t *out_qubits, uint32_t n_out, uint32_t *out2) {
   const std::string who = "function_plan";
-  if (!out2 || (prec != QIP_F32 && prec != QIP_F64) || n_qubits == 0 || n_qubits > 40)
-    return set_err(nullptr, QIPB200_ERR_INVALID_ARG, who + ": NULL out2, bad precision or n_qubits not in 1..40");
   return guarded(nullptr, [&]() -> int {
-    int st = check_function_sizes(nullptr, who, n_in, n_out);
+    int st = check_plan_args(who, prec, n_qubits, out2, "out2");
+    if (st == QIPB200_OK) st = check_function_sizes(nullptr, who, n_in, n_out);
+    if (st == QIPB200_OK) st = check_function_registers(nullptr, who, n_qubits, in_qubits, n_in, out_qubits, n_out);
     if (st != QIPB200_OK) return st;
-    if ((st = check_function_registers(nullptr, who, n_qubits, in_qubits, n_in, out_qubits, n_out)) != QIPB200_OK)
-      return st;
     uint32_t out_pos[kFnMaxOut];
     for (uint32_t i = 0; i < n_out; ++i) out_pos[i] = n_qubits - 1 - (uint32_t)out_qubits[i];
     const FnPlan p = plan_function(prec, n_qubits, out_pos, n_out);
@@ -2482,9 +2527,7 @@ extern "C" int qipb200_function_new_code(qipb200_ctx *ctx, uint32_t n_in, uint32
       if (e == cudaSuccess && first != ~0ull)
         e = tabulate_function(code, fn->params, nullptr, nullptr, first, 1, &fx, nullptr, ctx->sm_count, ctx->stream,
                               &err);
-      if (e != cudaSuccess)
-        return refuse(err.empty() ? cuda_fail(ctx, e, "function_code_first_bad")
-                                  : set_err(ctx, QIPB200_ERR_CUDA, who + ": " + err));
+      if (e != cudaSuccess) return refuse(code_error(ctx, who, e, err, "function_code_first_bad"));
       if (first != ~0ull)
         return refuse(set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": f(" + std::to_string(first) + ") = " +
                                                                 std::to_string(fx) + " does not fit in " +
@@ -2541,8 +2584,7 @@ extern "C" int qipb200_function_tabulate(const qipb200_function *fn, uint64_t x0
     const cudaError_t e = tabulate_function(fn->code, fn->params, fn->d_f, fn->d_cs, x0, count, f_out,
                                             phase ? cs_out : nullptr, ctx->sm_count, ctx->stream, &err);
     ++ctx->launches;
-    if (e != cudaSuccess)
-      return err.empty() ? cuda_fail(ctx, e, "tabulate_function") : set_err(ctx, QIPB200_ERR_CUDA, who + ": " + err);
+    if (e != cudaSuccess) return code_error(ctx, who, e, err, "tabulate_function");
     return (int)QIPB200_OK;
   });
 }
@@ -2560,21 +2602,18 @@ extern "C" int qipb200_state_expect_function(qipb200_state *s, const qipb200_fun
     if (!fn->theta)
       return set_err(s->ctx, QIPB200_ERR_UNSUPPORTED, who + ": the function has no theta (QIPB200_FN_CODE_THETA)");
     int st = check_function_registers(s->ctx, who, s->n, in_qubits, fn->n_in, nullptr, 0);
+    if (st == QIPB200_OK) st = require_unsharded(s, who);
     if (st != QIPB200_OK) return st;
-    if (s->world > 1 || !s->shards.empty())
-      return set_err(s->ctx, QIPB200_ERR_UNSUPPORTED, who + ": sharded states are not supported");
     if (fn->ctx != s->ctx)
       return set_err(s->ctx, QIPB200_ERR_INVALID_ARG, who + ": the function was made on another context");
     qipb200_ctx *ctx = s->ctx;
-    CU(ctx, cudaSetDevice(ctx->device));
-    if ((st = materialise_collapse(s)) != QIPB200_OK) return st;
+    if ((st = begin_device_work(s)) != QIPB200_OK) return st;
     uint32_t in_pos[kFnCodeMaxBits];
-    for (uint32_t i = 0; i < fn->n_in; ++i) in_pos[i] = s->phys_of_logical[s->n - 1 - (uint32_t)in_qubits[i]];
+    phys_positions(s, in_qubits, fn->n_in, in_pos);
     std::string err;
     const cudaError_t e = expect_function_code(s->prec, s->buf, s->n_local, in_pos, fn->n_in, fn->code, fn->params,
                                                (double *)fn->d_scratch + 1, ctx->stream, &ctx->launches, out, &err);
-    if (e != cudaSuccess)
-      return err.empty() ? cuda_fail(ctx, e, "expect_function_code") : set_err(ctx, QIPB200_ERR_CUDA, who + ": " + err);
+    if (e != cudaSuccess) return code_error(ctx, who, e, err, "expect_function_code");
     return (int)QIPB200_OK;
   });
 }
@@ -2583,50 +2622,17 @@ extern "C" int qipb200_state_expect_function(qipb200_state *s, const qipb200_fun
 // Pauli sums and the adjoint energy gradient (gradient.cu)
 // ===================================================================================
 
-namespace {
-
-// dst == src, then context, precision and size, then sharding: the checks the two-state calls share.
-int check_state_pair(const qipb200_state *dst, const qipb200_state *src, const std::string &who) {
-  if (dst == src) return set_err(dst->ctx, QIPB200_ERR_INVALID_ARG, who + ": the two states must differ");
-  if (dst->ctx != src->ctx || dst->prec != src->prec || dst->n != src->n)
-    return set_err(dst->ctx, QIPB200_ERR_SIZE_MISMATCH, who + ": the states differ in context, precision or size");
-  if (dst->world > 1 || !dst->shards.empty() || src->world > 1 || !src->shards.empty())
-    return set_err(dst->ctx, QIPB200_ERR_UNSUPPORTED, who + ": sharded states are not supported");
-  return QIPB200_OK;
-}
-
-int check_finite(qipb200_ctx *ctx, const double *v, size_t n, const std::string &who, const char *what) {
-  if (n && !v) return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL " + what + "s");
-  for (size_t t = 0; t < n; ++t)
-    if (!std::isfinite(v[t]))
-      return set_err(ctx, QIPB200_ERR_INVALID_ARG, who + ": " + what + " " + std::to_string(t) + " is not finite");
-  return QIPB200_OK;
-}
-
-// src's pending collapse runs, dst's is dropped (dst is overwritten), and dst takes src's layout.
-int prepare_out_of_place(qipb200_state *dst, qipb200_state *src) {
-  int st = materialise_collapse(src);
-  if (st != QIPB200_OK) return st;
-  dst->collapse_pending = false;
-  dst->phys_of_logical = src->phys_of_logical;
-  return QIPB200_OK;
-}
-
-}  // namespace
-
 extern "C" int qipb200_state_apply_pauli_sum(qipb200_state *dst, const qipb200_state *src, const uint64_t *qubits,
                                              const char *paulis, const uint32_t *term_len, size_t n_terms,
                                              const double *coeffs) {
   if (!dst || !src) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, "apply_pauli_sum: NULL state");
   return guarded(dst->ctx, [&]() -> int {
     // every check runs before any device work: a refused call leaves both states as they were
-    int st = check_state_pair(dst, src, "apply_pauli_sum");
-    if (st != QIPB200_OK) return st;
     std::vector<PauliTerm> terms;
-    std::string err;
-    st = parse_pauli_terms(src->n, qubits, paulis, term_len, n_terms, &terms, &err);
-    if (st != QIPB200_OK) return set_err(dst->ctx, st, err);
-    if ((st = check_finite(dst->ctx, coeffs, n_terms, "apply_pauli_sum", "coefficient")) != QIPB200_OK) return st;
+    int st = check_state_pair(dst, src, "apply_pauli_sum");
+    if (st == QIPB200_OK) st = parse_terms(dst->ctx, src->n, qubits, paulis, term_len, n_terms, &terms);
+    if (st == QIPB200_OK) st = check_finite(dst->ctx, coeffs, n_terms, "apply_pauli_sum", "coefficient");
+    if (st != QIPB200_OK) return st;
     qipb200_state *s = const_cast<qipb200_state *>(src);  // a pending collapse is applied: the state it stands for
     qipb200_ctx *ctx = dst->ctx;
     CU(ctx, cudaSetDevice(ctx->device));
@@ -2639,14 +2645,11 @@ extern "C" int qipb200_state_apply_pauli_sum(qipb200_state *dst, const qipb200_s
 
 extern "C" int qipb200_pauli_sum_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, const char *paulis,
                                       const uint32_t *term_len, size_t n_terms, uint32_t *sweeps) {
-  if (!sweeps || (prec != QIP_F32 && prec != QIP_F64) || n_qubits == 0 || n_qubits > 40)
-    return set_err(nullptr, QIPB200_ERR_INVALID_ARG,
-                   "pauli_sum_plan: NULL sweeps, bad precision or n_qubits not in 1..40");
   return guarded(nullptr, [&]() -> int {
     std::vector<PauliTerm> terms;
-    std::string err;
-    int st = parse_pauli_terms(n_qubits, qubits, paulis, term_len, n_terms, &terms, &err);
-    if (st != QIPB200_OK) return set_err(nullptr, st, err);
+    int st = check_plan_args("pauli_sum_plan", prec, n_qubits, sweeps, "sweeps");
+    if (st == QIPB200_OK) st = parse_terms(nullptr, n_qubits, qubits, paulis, term_len, n_terms, &terms);
+    if (st != QIPB200_OK) return st;
     *sweeps = pauli_sum_sweep_count(n_qubits, terms);
     return (int)QIPB200_OK;
   });
@@ -2661,16 +2664,13 @@ extern "C" int qipb200_state_pauli_energy_gradient(qipb200_state *state, qipb200
   if (!state || !work) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, std::string(who) + ": NULL state");
   return guarded(state->ctx, [&]() -> int {
     // every check runs before any device work: a refused call leaves both states as they were
-    int st = check_state_pair(work, state, who);
-    if (st != QIPB200_OK) return st;
     std::vector<PauliTerm> ansatz, ham;
-    std::string err;
-    st = parse_pauli_terms(state->n, qubits, paulis, term_len, n_terms, &ansatz, &err);
-    if (st != QIPB200_OK) return set_err(state->ctx, st, err);
-    st = parse_pauli_terms(state->n, ham_qubits, ham_paulis, ham_term_len, n_ham, &ham, &err);
-    if (st != QIPB200_OK) return set_err(state->ctx, st, err);
-    if ((st = check_finite(state->ctx, angles, n_terms, who, "angle")) != QIPB200_OK) return st;
-    if ((st = check_finite(state->ctx, coeffs, n_ham, who, "coefficient")) != QIPB200_OK) return st;
+    int st = check_state_pair(work, state, who);
+    if (st == QIPB200_OK) st = parse_terms(state->ctx, state->n, qubits, paulis, term_len, n_terms, &ansatz);
+    if (st == QIPB200_OK) st = parse_terms(state->ctx, state->n, ham_qubits, ham_paulis, ham_term_len, n_ham, &ham);
+    if (st == QIPB200_OK) st = check_finite(state->ctx, angles, n_terms, who, "angle");
+    if (st == QIPB200_OK) st = check_finite(state->ctx, coeffs, n_ham, who, "coefficient");
+    if (st != QIPB200_OK) return st;
     if (!energy) return set_err(state->ctx, QIPB200_ERR_INVALID_ARG, std::string(who) + ": NULL energy");
     if (n_terms && !grad) return set_err(state->ctx, QIPB200_ERR_INVALID_ARG, std::string(who) + ": NULL grad");
     qipb200_ctx *ctx = state->ctx;
@@ -2687,16 +2687,12 @@ extern "C" int qipb200_pauli_gradient_plan(qip_prec prec, uint32_t n_qubits, con
                                            const char *paulis, const uint32_t *term_len, size_t n_terms,
                                            const uint64_t *ham_qubits, const char *ham_paulis,
                                            const uint32_t *ham_term_len, size_t n_ham, uint32_t *out3) {
-  if (!out3 || (prec != QIP_F32 && prec != QIP_F64) || n_qubits == 0 || n_qubits > 40)
-    return set_err(nullptr, QIPB200_ERR_INVALID_ARG,
-                   "pauli_gradient_plan: NULL out3, bad precision or n_qubits not in 1..40");
   return guarded(nullptr, [&]() -> int {
     std::vector<PauliTerm> ansatz, ham;
-    std::string err;
-    int st = parse_pauli_terms(n_qubits, qubits, paulis, term_len, n_terms, &ansatz, &err);
-    if (st != QIPB200_OK) return set_err(nullptr, st, err);
-    st = parse_pauli_terms(n_qubits, ham_qubits, ham_paulis, ham_term_len, n_ham, &ham, &err);
-    if (st != QIPB200_OK) return set_err(nullptr, st, err);
+    int st = check_plan_args("pauli_gradient_plan", prec, n_qubits, out3, "out3");
+    if (st == QIPB200_OK) st = parse_terms(nullptr, n_qubits, qubits, paulis, term_len, n_terms, &ansatz);
+    if (st == QIPB200_OK) st = parse_terms(nullptr, n_qubits, ham_qubits, ham_paulis, ham_term_len, n_ham, &ham);
+    if (st != QIPB200_OK) return st;
     out3[0] = pauli_rotation_sweep_count(n_qubits, ansatz);
     out3[1] = pauli_sum_sweep_count(n_qubits, ham);
     out3[2] = pauli_adjoint_sweep_count(n_qubits, ansatz);
@@ -2730,23 +2726,17 @@ extern "C" int qipb200_state_pauli_geometric_tensor(qipb200_state *state, qipb20
   return guarded(state->ctx, [&]() -> int {
     // every check runs before any device work: a refused call leaves the three states (and a pending collapse) as
     // they were
-    if (state == work_a || state == work_b || work_a == work_b)
-      return set_err(state->ctx, QIPB200_ERR_INVALID_ARG, who + ": the three states must differ");
-    int st = check_state_pair(work_a, state, who);
-    if (st == QIPB200_OK) st = check_state_pair(work_b, state, who);
-    if (st != QIPB200_OK) return st;
     std::vector<PauliTerm> ansatz;
-    std::string err;
-    st = parse_pauli_terms(state->n, qubits, paulis, term_len, n_terms, &ansatz, &err);
-    if (st != QIPB200_OK) return set_err(state->ctx, st, err);
-    if ((st = check_finite(state->ctx, angles, n_terms, who, "angle")) != QIPB200_OK) return st;
+    int st = check_three_states(state, work_a, work_b, who);
+    if (st == QIPB200_OK) st = parse_terms(state->ctx, state->n, qubits, paulis, term_len, n_terms, &ansatz);
+    if (st == QIPB200_OK) st = check_finite(state->ctx, angles, n_terms, who, "angle");
+    if (st != QIPB200_OK) return st;
     if (n_terms && !qgt) return set_err(state->ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL qgt");
     if ((st = check_qgt_terms(state->ctx, who, n_terms)) != QIPB200_OK) return st;
     qipb200_ctx *ctx = state->ctx;
+    if (n_terms == 0) return begin_device_work(state);  // the work states are not touched
     CU(ctx, cudaSetDevice(ctx->device));
-    if (n_terms == 0) return materialise_collapse(state);  // the work states are not touched
-    if ((st = prepare_out_of_place(work_a, state)) != QIPB200_OK) return st;
-    if ((st = prepare_out_of_place(work_b, state)) != QIPB200_OK) return st;
+    if ((st = prepare_work_states(state, work_a, work_b)) != QIPB200_OK) return st;
     CU(ctx, run_pauli_qgt(state->prec, state->buf, work_a->buf, work_b->buf, state->n_local,
                           phys_terms(state, ansatz), angles, ctx->stream, &ctx->launches, qgt, expect));
     return (int)QIPB200_OK;
@@ -2757,14 +2747,12 @@ extern "C" int qipb200_pauli_geometric_tensor_plan(qip_prec prec, uint32_t n_qub
                                                    const char *paulis, const uint32_t *term_len, size_t n_terms,
                                                    uint32_t *out3) {
   const std::string who = "pauli_geometric_tensor_plan";
-  if (!out3 || (prec != QIP_F32 && prec != QIP_F64) || n_qubits == 0 || n_qubits > 40)
-    return set_err(nullptr, QIPB200_ERR_INVALID_ARG, who + ": NULL out3, bad precision or n_qubits not in 1..40");
   return guarded(nullptr, [&]() -> int {
     std::vector<PauliTerm> ansatz;
-    std::string err;
-    int st = parse_pauli_terms(n_qubits, qubits, paulis, term_len, n_terms, &ansatz, &err);
-    if (st != QIPB200_OK) return set_err(nullptr, st, err);
-    if ((st = check_qgt_terms(nullptr, who, n_terms)) != QIPB200_OK) return st;
+    int st = check_plan_args(who, prec, n_qubits, out3, "out3");
+    if (st == QIPB200_OK) st = parse_terms(nullptr, n_qubits, qubits, paulis, term_len, n_terms, &ansatz);
+    if (st == QIPB200_OK) st = check_qgt_terms(nullptr, who, n_terms);
+    if (st != QIPB200_OK) return st;
     const uint32_t T = (uint32_t)n_terms, S = pauli_qgt_sweep_count(n_qubits, ansatz);
     out3[0] = T;
     out3[1] = S;
@@ -2800,33 +2788,28 @@ extern "C" int qipb200_state_evolve_pauli_sum(qipb200_state *state, qipb200_stat
   return guarded(state->ctx, [&]() -> int {
     // every check runs before any device work: a refused call leaves the three states (and a pending collapse) as
     // they were
-    if (state == work_a || state == work_b || work_a == work_b)
-      return set_err(state->ctx, QIPB200_ERR_INVALID_ARG, who + ": the three states must differ");
-    int st = check_state_pair(work_a, state, who);
-    if (st == QIPB200_OK) st = check_state_pair(work_b, state, who);
-    if (st != QIPB200_OK) return st;
     std::vector<PauliTerm> terms;
-    std::string err;
-    st = parse_pauli_terms(state->n, qubits, paulis, term_len, n_terms, &terms, &err);
-    if (st != QIPB200_OK) return set_err(state->ctx, st, err);
-    if ((st = check_evolution_args(state->ctx, who, coeffs, n_terms, time, tol)) != QIPB200_OK) return st;
+    int st = check_three_states(state, work_a, work_b, who);
+    if (st == QIPB200_OK) st = parse_terms(state->ctx, state->n, qubits, paulis, term_len, n_terms, &terms);
+    if (st == QIPB200_OK) st = check_evolution_args(state->ctx, who, coeffs, n_terms, time, tol);
+    if (st != QIPB200_OK) return st;
     if (!degree || !tail) return set_err(state->ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL degree or tail");
     EvolutionPlan p;
+    std::string err;
     if ((st = plan_evolution(terms, coeffs, time, tol, &p, &err)) != QIPB200_OK) return set_err(state->ctx, st, err);
     *degree = p.degree;
     *tail = p.tail;
     if (p.kind == EvolutionPlan::kNoop) return (int)QIPB200_OK;
     qipb200_ctx *ctx = state->ctx;
-    CU(ctx, cudaSetDevice(ctx->device));
     if (p.kind == EvolutionPlan::kPhase) {  // e^{-iat}: the empty-term rotation by 2 RN(a t)
-      if ((st = materialise_collapse(state)) != QIPB200_OK) return st;
+      if ((st = begin_device_work(state)) != QIPB200_OK) return st;
       const double angle = 2.0 * (p.a * time);
       CU(ctx, run_pauli_rotations(state->prec, state->buf, state->n_local, std::vector<PauliTerm>(1), &angle,
                                   2 * ctx->sm_count, ctx->stream, &ctx->launches));
       return (int)QIPB200_OK;
     }
-    if ((st = prepare_out_of_place(work_a, state)) != QIPB200_OK) return st;
-    if ((st = prepare_out_of_place(work_b, state)) != QIPB200_OK) return st;
+    CU(ctx, cudaSetDevice(ctx->device));
+    if ((st = prepare_work_states(state, work_a, work_b)) != QIPB200_OK) return st;
     CU(ctx, run_pauli_evolution(state->prec, state->buf, work_a->buf, work_b->buf, state->n_local,
                                 phys_terms(state, p.terms), p.coeffs.data(), p.b, p.C, ctx->stream, &ctx->launches));
     return (int)QIPB200_OK;
@@ -2838,16 +2821,14 @@ extern "C" int qipb200_pauli_evolution_plan(qip_prec prec, uint32_t n_qubits, co
                                             const double *coeffs, double time, double tol, uint32_t *out3,
                                             double *tail, double *coeffs_out, size_t coeffs_cap) {
   const std::string who = "pauli_evolution_plan";
-  if (!out3 || !tail || (prec != QIP_F32 && prec != QIP_F64) || n_qubits == 0 || n_qubits > 40)
-    return set_err(nullptr, QIPB200_ERR_INVALID_ARG,
-                   who + ": NULL out3 or tail, bad precision or n_qubits not in 1..40");
   return guarded(nullptr, [&]() -> int {
     std::vector<PauliTerm> terms;
-    std::string err;
-    int st = parse_pauli_terms(n_qubits, qubits, paulis, term_len, n_terms, &terms, &err);
-    if (st != QIPB200_OK) return set_err(nullptr, st, err);
-    if ((st = check_evolution_args(nullptr, who, coeffs, n_terms, time, tol)) != QIPB200_OK) return st;
+    int st = check_plan_args(who, prec, n_qubits, out3 && tail, "out3 or tail");
+    if (st == QIPB200_OK) st = parse_terms(nullptr, n_qubits, qubits, paulis, term_len, n_terms, &terms);
+    if (st == QIPB200_OK) st = check_evolution_args(nullptr, who, coeffs, n_terms, time, tol);
+    if (st != QIPB200_OK) return st;
     EvolutionPlan p;
+    std::string err;
     if ((st = plan_evolution(terms, coeffs, time, tol, &p, &err)) != QIPB200_OK) return set_err(nullptr, st, err);
     const uint64_t s = p.kind == EvolutionPlan::kSeries ? pauli_sum_sweep_count(n_qubits, p.terms) : 0;
     out3[0] = p.degree;
@@ -2873,16 +2854,11 @@ extern "C" int qipb200_state_lanczos_pauli_sum(qipb200_state *state, qipb200_sta
   return guarded(state->ctx, [&]() -> int {
     // every check runs before any device work: a refused call leaves the three states (and a pending collapse) as
     // they were
-    if (state == work_a || state == work_b || work_a == work_b)
-      return set_err(state->ctx, QIPB200_ERR_INVALID_ARG, who + ": the three states must differ");
-    int st = check_state_pair(work_a, state, who);
-    if (st == QIPB200_OK) st = check_state_pair(work_b, state, who);
-    if (st != QIPB200_OK) return st;
     std::vector<PauliTerm> terms;
-    std::string err;
-    st = parse_pauli_terms(state->n, qubits, paulis, term_len, n_terms, &terms, &err);
-    if (st != QIPB200_OK) return set_err(state->ctx, st, err);
-    if ((st = check_finite(state->ctx, coeffs, n_terms, who, "coefficient")) != QIPB200_OK) return st;
+    int st = check_three_states(state, work_a, work_b, who);
+    if (st == QIPB200_OK) st = parse_terms(state->ctx, state->n, qubits, paulis, term_len, n_terms, &terms);
+    if (st == QIPB200_OK) st = check_finite(state->ctx, coeffs, n_terms, who, "coefficient");
+    if (st != QIPB200_OK) return st;
     if (max_steps == 0 || max_steps > kLanczosMaxSteps)
       return set_err(state->ctx, QIPB200_ERR_INVALID_ARG,
                      who + ": max_steps must be in 1.." + std::to_string(kLanczosMaxSteps));
@@ -2900,8 +2876,7 @@ extern "C" int qipb200_state_lanczos_pauli_sum(qipb200_state *state, qipb200_sta
     }
     qipb200_ctx *ctx = state->ctx;
     CU(ctx, cudaSetDevice(ctx->device));
-    if ((st = prepare_out_of_place(work_a, state)) != QIPB200_OK) return st;
-    if ((st = prepare_out_of_place(work_b, state)) != QIPB200_OK) return st;
+    if ((st = prepare_work_states(state, work_a, work_b)) != QIPB200_OK) return st;
     LanczosResult r;
     CU(ctx, run_lanczos(state->prec, state->buf, work_a->buf, work_b->buf, state->n_local, phys_terms(state, terms),
                         coeffs, a, b, max_steps, tol, (flags & QIPB200_LANCZOS_VECTOR) != 0, ctx->stream,
@@ -2921,14 +2896,11 @@ extern "C" int qipb200_state_lanczos_pauli_sum(qipb200_state *state, qipb200_sta
 
 extern "C" int qipb200_pauli_lanczos_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, const char *paulis,
                                           const uint32_t *term_len, size_t n_terms, uint32_t *out4) {
-  if (!out4 || (prec != QIP_F32 && prec != QIP_F64) || n_qubits == 0 || n_qubits > 40)
-    return set_err(nullptr, QIPB200_ERR_INVALID_ARG,
-                   "pauli_lanczos_plan: NULL out4, bad precision or n_qubits not in 1..40");
   return guarded(nullptr, [&]() -> int {
     std::vector<PauliTerm> terms;
-    std::string err;
-    int st = parse_pauli_terms(n_qubits, qubits, paulis, term_len, n_terms, &terms, &err);
-    if (st != QIPB200_OK) return set_err(nullptr, st, err);
+    int st = check_plan_args("pauli_lanczos_plan", prec, n_qubits, out4, "out4");
+    if (st == QIPB200_OK) st = parse_terms(nullptr, n_qubits, qubits, paulis, term_len, n_terms, &terms);
+    if (st != QIPB200_OK) return st;
     lanczos_plan_counts(n_qubits, terms, out4);
     return (int)QIPB200_OK;
   });

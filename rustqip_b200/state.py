@@ -317,13 +317,8 @@ class State:
         single ``[("X", q)]`` term is Rx(angle).  A read-write sweep of the state carries a run of consecutive terms
         whose X/Y letters fit one tile (``pauli_rotation_plan`` gives the count).  Stream-ordered like
         ``apply_schedule``; the result is the same bits however the terms are split over calls."""
-        a = np.ascontiguousarray(np.asarray(angles, dtype=np.float64).reshape(-1))
-        terms = list(terms)
-        if a.shape[0] != len(terms):
-            raise ValueError("apply_pauli_rotations: %d terms but %d angles" % (len(terms), a.shape[0]))
-        qs, ls, lens = _marshal_paulis(terms)
-        self._chk(_lib.lib().qipb200_state_apply_pauli_rotations(self._h, _ptr(qs), ls, _ptr(lens), lens.shape[0],
-                                                                 _ptr(a) if a.shape[0] else None))
+        args = _pauli_args("apply_pauli_rotations", terms, angles, "angles")
+        self._chk(_lib.lib().qipb200_state_apply_pauli_rotations(self._h, *args))
 
     def apply_function(self, fn: "Function", in_qubits: Sequence[int], out_qubits: Sequence[int] = ()):
         """Apply U|x>|y> = e^{i theta(x)} |x>|y XOR f(x)> of ``fn`` on the device: bit i of x is the value of qubit
@@ -360,13 +355,8 @@ class State:
         this state takes its qubit layout.  Deterministic; stream-ordered like ``apply_schedule``
         (``pauli_sum_plan`` gives the sweep count).  For example ``w.apply_pauli_sum(st, H, c)`` then ``w.norm2()``
         is <psi|H^2|psi>."""
-        c = np.ascontiguousarray(np.asarray(coeffs, dtype=np.float64).reshape(-1))
-        terms = list(terms)
-        if c.shape[0] != len(terms):
-            raise ValueError("apply_pauli_sum: %d terms but %d coefficients" % (len(terms), c.shape[0]))
-        qs, ls, lens = _marshal_paulis(terms)
-        self._chk(_lib.lib().qipb200_state_apply_pauli_sum(self._h, src._h, _ptr(qs), ls, _ptr(lens), lens.shape[0],
-                                                           _ptr(c) if c.shape[0] else None))
+        args = _pauli_args("apply_pauli_sum", terms, coeffs, "coefficients")
+        self._chk(_lib.lib().qipb200_state_apply_pauli_sum(self._h, src._h, *args))
 
     def energy_gradient(self, work: "State", ansatz, angles, hamiltonian, coeffs):
         """Energy and gradient of E(angles) = <psi0|U^dagger H U|psi0> by the adjoint method, on the device.
@@ -377,21 +367,13 @@ class State:
         ``work`` is scratch of the same size and precision: it ends holding U^dagger H U psi0.  This state ends at
         psi0 up to rounding (run forward and back); re-prepare psi0 when it is needed exactly.  Deterministic;
         synchronises (``pauli_gradient_plan`` gives the sweep counts)."""
-        a = np.ascontiguousarray(np.asarray(angles, dtype=np.float64).reshape(-1))
-        c = np.ascontiguousarray(np.asarray(coeffs, dtype=np.float64).reshape(-1))
-        ansatz, hamiltonian = list(ansatz), list(hamiltonian)
-        if a.shape[0] != len(ansatz):
-            raise ValueError("energy_gradient: %d terms but %d angles" % (len(ansatz), a.shape[0]))
-        if c.shape[0] != len(hamiltonian):
-            raise ValueError("energy_gradient: %d Hamiltonian terms but %d coefficients" % (len(hamiltonian), c.shape[0]))
-        qs, ls, lens = _marshal_paulis(ansatz)
-        hq, hl, hlen = _marshal_paulis(hamiltonian)
+        a = _pauli_args("energy_gradient", ansatz, angles, "angles")
+        h = _pauli_args("energy_gradient", hamiltonian, coeffs, "coefficients", kind="Hamiltonian terms")
+        T = a[3]
         energy = np.zeros(1, dtype=np.float64)
-        grad = np.zeros(max(1, len(ansatz)), dtype=np.float64)
-        self._chk(_lib.lib().qipb200_state_pauli_energy_gradient(
-            self._h, work._h, _ptr(qs), ls, _ptr(lens), lens.shape[0], _ptr(a) if a.shape[0] else None,
-            _ptr(hq), hl, _ptr(hlen), hlen.shape[0], _ptr(c) if c.shape[0] else None, _ptr(energy), _ptr(grad)))
-        return float(energy[0]), grad[: len(ansatz)]
+        grad = np.zeros(max(1, T), dtype=np.float64)
+        self._chk(_lib.lib().qipb200_state_pauli_energy_gradient(self._h, work._h, *a, *h, _ptr(energy), _ptr(grad)))
+        return float(energy[0]), grad[:T]
 
     def geometric_tensor(self, work_a: "State", work_b: "State", ansatz, angles):
         """The quantum geometric tensor of the Pauli-rotation circuit U = R_{T-1} ... R_0, R_t = exp(-i angles[t]/2 P_t)
@@ -407,17 +389,12 @@ class State:
         host.  ``work_a`` and ``work_b`` are two more states of the same context, precision and size, used as scratch;
         this state ends at U psi0, bit-identical to ``apply_pauli_rotations``.  Deterministic; synchronises; at most
         2048 terms (``pauli_geometric_tensor_plan`` gives the counts)."""
-        a = np.ascontiguousarray(np.asarray(angles, dtype=np.float64).reshape(-1))
-        ansatz = list(ansatz)
-        T = len(ansatz)
-        if a.shape[0] != T:
-            raise ValueError("geometric_tensor: %d terms but %d angles" % (T, a.shape[0]))
-        qs, ls, lens = _marshal_paulis(ansatz)
+        args = _pauli_args("geometric_tensor", ansatz, angles, "angles")
+        T = args[3]
         g = np.zeros(max(1, 2 * T * T), dtype=np.float64)
         e = np.zeros(max(1, T), dtype=np.float64)
-        self._chk(_lib.lib().qipb200_state_pauli_geometric_tensor(
-            self._h, work_a._h, work_b._h, _ptr(qs), ls, _ptr(lens), lens.shape[0], _ptr(a) if T else None, _ptr(g),
-            _ptr(e)))
+        self._chk(_lib.lib().qipb200_state_pauli_geometric_tensor(self._h, work_a._h, work_b._h, *args, _ptr(g),
+                                                                  _ptr(e)))
         return g[: 2 * T * T].view(np.complex128).reshape(T, T), e[:T]
 
     def evolve_pauli_sum(self, work_a: "State", work_b: "State", terms, coeffs, time: float, tol=None):
@@ -431,15 +408,11 @@ class State:
         steps is one read-write sweep per sweep of ``pauli_sum_plan`` of the non-identity terms
         (``pauli_evolution_plan`` gives the counts); deterministic and stream-ordered.  K above 65536 is refused:
         split the time over several calls."""
-        c = np.ascontiguousarray(np.asarray(coeffs, dtype=np.float64).reshape(-1))
-        terms = list(terms)
-        if c.shape[0] != len(terms):
-            raise ValueError("evolve_pauli_sum: %d terms but %d coefficients" % (len(terms), c.shape[0]))
-        qs, ls, lens = _marshal_paulis(terms)
+        args = _pauli_args("evolve_pauli_sum", terms, coeffs, "coefficients")
         degree, tail = C.c_uint32(), C.c_double()
         self._chk(_lib.lib().qipb200_state_evolve_pauli_sum(
-            self._h, work_a._h, work_b._h, _ptr(qs), ls, _ptr(lens), lens.shape[0], _ptr(c) if c.shape[0] else None,
-            float(time), float(_default_tol(self.dtype) if tol is None else tol), C.byref(degree), C.byref(tail)))
+            self._h, work_a._h, work_b._h, *args, float(time),
+            float(_default_tol(self.dtype) if tol is None else tol), C.byref(degree), C.byref(tail)))
         return int(degree.value), float(tail.value)
 
     def lanczos_pauli_sum(self, work_a: "State", work_b: "State", terms, coeffs, max_steps: int = 300, tol=None,
@@ -459,18 +432,14 @@ class State:
         residual of energy.  ``work_a`` and ``work_b`` are two more states of the same context, precision and size,
         used as scratch.  Deterministic; synchronises once per step (``pauli_lanczos_plan`` gives the kernel
         counts)."""
-        c = np.ascontiguousarray(np.asarray(coeffs, dtype=np.float64).reshape(-1))
-        terms = list(terms)
-        if c.shape[0] != len(terms):
-            raise ValueError("lanczos_pauli_sum: %d terms but %d coefficients" % (len(terms), c.shape[0]))
-        qs, ls, lens = _marshal_paulis(terms)
+        args = _pauli_args("lanczos_pauli_sum", terms, coeffs, "coefficients")
         cap = max(1, min(int(max_steps), 4096))
         alpha, beta, out3 = np.zeros(cap), np.zeros(cap + 1), np.zeros(3)
         steps, conv = C.c_uint32(), C.c_uint32()
         self._chk(_lib.lib().qipb200_state_lanczos_pauli_sum(
-            self._h, work_a._h, work_b._h, _ptr(qs), ls, _ptr(lens), lens.shape[0], _ptr(c) if c.shape[0] else None,
-            int(max_steps), float(_default_lanczos_tol(self.dtype) if tol is None else tol), 1 if vector else 0,
-            C.byref(steps), C.byref(conv), _ptr(alpha), _ptr(beta), _ptr(out3)))
+            self._h, work_a._h, work_b._h, *args, int(max_steps),
+            float(_default_lanczos_tol(self.dtype) if tol is None else tol), 1 if vector else 0, C.byref(steps),
+            C.byref(conv), _ptr(alpha), _ptr(beta), _ptr(out3)))
         m = int(steps.value)
         return LanczosResult(float(out3[0]), float(out3[1]), m, bool(conv.value), alpha[:m].copy(),
                              beta[: m + 1].copy(), float(out3[2]))
@@ -670,23 +639,38 @@ def _marshal_paulis(terms):
     return qa, la, np.ascontiguousarray(np.asarray(lens if lens else [0], dtype=np.uint32))[: len(lens)]
 
 
+def _pauli_term_args(terms):
+    """(qubits, letters, term lengths, term count) C arguments of a term list; the pointers keep their arrays alive."""
+    qs, ls, lens = _marshal_paulis(terms)
+    return qs.ctypes.data_as(C.c_void_p), ls, lens.ctypes.data_as(C.c_void_p), lens.shape[0]
+
+
+def _pauli_args(who, terms, values, what, kind="terms"):
+    """The C arguments of a term list followed by its values (float64, one per term; NULL for no terms)."""
+    v = np.ascontiguousarray(np.asarray(values, dtype=np.float64).reshape(-1))
+    terms = list(terms)
+    if v.shape[0] != len(terms):
+        raise ValueError("%s: %d %s but %d %s" % (who, len(terms), kind, v.shape[0], what))
+    return _pauli_term_args(terms) + (v.ctypes.data_as(C.c_void_p) if v.shape[0] else None,)
+
+
+def _pauli_plan(entry, n, dtype, count, *term_lists):
+    """The count uint32 results of the host-only plan qipb200_<entry> of these term lists."""
+    v = (C.c_uint32 * count)()
+    args = [a for terms in term_lists for a in _pauli_term_args(terms)]
+    _lib.check(getattr(_lib.lib(), "qipb200_" + entry)(prec_of(dtype), int(n), *args, v), None)
+    return tuple(int(x) for x in v)
+
+
 def expect_plan(n: int, dtype, terms) -> int:
     """Read sweeps State.expect_paulis makes for these terms on an unsharded n-qubit state (needs no GPU)."""
-    qs, ls, lens = _marshal_paulis(terms)
-    v = C.c_uint32()
-    _lib.check(_lib.lib().qipb200_expect_plan(prec_of(dtype), int(n), _ptr(qs), ls, _ptr(lens), lens.shape[0],
-                                             C.byref(v)), None)
-    return int(v.value)
+    return _pauli_plan("expect_plan", n, dtype, 1, terms)[0]
 
 
 def transition_plan(n: int, dtype, terms):
     """(read sweeps, kernels) of State.transition_paulis for these terms on unsharded n-qubit states in canonical
     layout with nothing pending (needs no GPU); (0, 0) for no terms."""
-    qs, ls, lens = _marshal_paulis(terms)
-    v = (C.c_uint32 * 2)()
-    _lib.check(_lib.lib().qipb200_transition_plan(prec_of(dtype), int(n), _ptr(qs), ls, _ptr(lens), lens.shape[0], v),
-               None)
-    return int(v[0]), int(v[1])
+    return _pauli_plan("transition_plan", n, dtype, 2, terms)
 
 
 def purity_plan(n: int, dtype, qubits):
@@ -702,41 +686,24 @@ def purity_plan(n: int, dtype, qubits):
 def pauli_rotation_plan(n: int, dtype, terms) -> int:
     """Read-write sweeps State.apply_pauli_rotations makes for these terms on an unsharded n-qubit state (needs no
     GPU)."""
-    qs, ls, lens = _marshal_paulis(terms)
-    v = C.c_uint32()
-    _lib.check(_lib.lib().qipb200_pauli_rotation_plan(prec_of(dtype), int(n), _ptr(qs), ls, _ptr(lens), lens.shape[0],
-                                                      C.byref(v)), None)
-    return int(v.value)
+    return _pauli_plan("pauli_rotation_plan", n, dtype, 1, terms)[0]
 
 
 def pauli_sum_plan(n: int, dtype, terms) -> int:
     """Read-write sweeps State.apply_pauli_sum makes for these terms on an unsharded n-qubit state (needs no GPU)."""
-    qs, ls, lens = _marshal_paulis(terms)
-    v = C.c_uint32()
-    _lib.check(_lib.lib().qipb200_pauli_sum_plan(prec_of(dtype), int(n), _ptr(qs), ls, _ptr(lens), lens.shape[0],
-                                                 C.byref(v)), None)
-    return int(v.value)
+    return _pauli_plan("pauli_sum_plan", n, dtype, 1, terms)[0]
 
 
 def pauli_gradient_plan(n: int, dtype, ansatz, hamiltonian):
     """(forward, sum, backward) sweeps State.energy_gradient makes on an unsharded n-qubit state (needs no GPU); the
     call launches forward + sum + 2 * backward kernels."""
-    qs, ls, lens = _marshal_paulis(ansatz)
-    hq, hl, hlen = _marshal_paulis(hamiltonian)
-    v = (C.c_uint32 * 3)()
-    _lib.check(_lib.lib().qipb200_pauli_gradient_plan(prec_of(dtype), int(n), _ptr(qs), ls, _ptr(lens), lens.shape[0],
-                                                      _ptr(hq), hl, _ptr(hlen), hlen.shape[0], v), None)
-    return int(v[0]), int(v[1]), int(v[2])
+    return _pauli_plan("pauli_gradient_plan", n, dtype, 3, ansatz, hamiltonian)
 
 
 def pauli_geometric_tensor_plan(n: int, dtype, ansatz):
     """(forks, segment sweeps, kernels) of State.geometric_tensor on an unsharded n-qubit state (needs no GPU): one
     fork per term, the sweeps of terms i+1 .. T-1 summed over i, and T + 2 sweeps + 1 kernels (0 for no terms)."""
-    qs, ls, lens = _marshal_paulis(ansatz)
-    v = (C.c_uint32 * 3)()
-    _lib.check(_lib.lib().qipb200_pauli_geometric_tensor_plan(prec_of(dtype), int(n), _ptr(qs), ls, _ptr(lens),
-                                                              lens.shape[0], v), None)
-    return int(v[0]), int(v[1]), int(v[2])
+    return _pauli_plan("pauli_geometric_tensor_plan", n, dtype, 3, ansatz)
 
 
 def _default_tol(dtype):
@@ -746,18 +713,13 @@ def _default_tol(dtype):
 def pauli_evolution_plan(n: int, dtype, terms, coeffs, time: float, tol=None):
     """(degree, sweeps per step, kernels, tail, C) of State.evolve_pauli_sum on an unsharded n-qubit state (needs no
     GPU): C[k] (complex128, K + 1 of them) are the series coefficients (2 - delta_k0) (-i)^k J_k(bt) e^{-iat}."""
-    c = np.ascontiguousarray(np.asarray(coeffs, dtype=np.float64).reshape(-1))
-    terms = list(terms)
-    if c.shape[0] != len(terms):
-        raise ValueError("pauli_evolution_plan: %d terms but %d coefficients" % (len(terms), c.shape[0]))
-    qs, ls, lens = _marshal_paulis(terms)
+    args = _pauli_args("pauli_evolution_plan", terms, coeffs, "coefficients")
     tol = float(_default_tol(dtype) if tol is None else tol)
     v, tail = (C.c_uint32 * 3)(), C.c_double()
 
     def call(out, cap):
-        _lib.check(_lib.lib().qipb200_pauli_evolution_plan(
-            prec_of(dtype), int(n), _ptr(qs), ls, _ptr(lens), lens.shape[0], _ptr(c) if c.shape[0] else None,
-            float(time), tol, v, C.byref(tail), out, cap), None)
+        _lib.check(_lib.lib().qipb200_pauli_evolution_plan(prec_of(dtype), int(n), *args, float(time), tol, v,
+                                                           C.byref(tail), out, cap), None)
 
     call(None, 0)
     out = np.zeros(2 * (int(v[0]) + 1), dtype=np.float64)
@@ -785,11 +747,7 @@ def pauli_lanczos_plan(n: int, dtype, terms):
     vector mode) of State.lanczos_pauli_sum on an unsharded n-qubit state (needs no GPU).  A call of m steps launches
     1 + m k1 kernels without the vector, m k1 + (m - 1) k2 + k0 with it; (0, 0, 0, 2) when every term is the
     identity."""
-    qs, ls, lens = _marshal_paulis(terms)
-    v = (C.c_uint32 * 4)()
-    _lib.check(_lib.lib().qipb200_pauli_lanczos_plan(prec_of(dtype), int(n), _ptr(qs), ls, _ptr(lens), lens.shape[0],
-                                                     v), None)
-    return tuple(int(x) for x in v)
+    return _pauli_plan("pauli_lanczos_plan", n, dtype, 4, terms)
 
 
 def lanczos_ritz(alpha, beta):
