@@ -578,10 +578,33 @@ int materialise_collapse(qipb200_state *s) {
                             s->pend_p_mult);
 }
 
-// s's device made current and its pending collapse applied: the start of every call that reads s.
+}  // namespace
+namespace qipb200 {
+
+// Write the basis state qipb200_state_set_basis left pending: one write sweep, memsets only.  No kernel is launched,
+// so the call that triggers it launches exactly the kernels it launches on a state set_basis wrote at once.
+int materialise_init(qipb200_state *s) {
+  if (!s->init_pending) return QIPB200_OK;
+  qipb200_ctx *ctx = s->ctx;
+  CU(ctx, cudaSetDevice(ctx->device));
+  CU(ctx, write_basis_state(s->prec, s->buf, 1ull << s->n_local, s->init_index, ctx->stream));
+  s->init_pending = false;
+  return QIPB200_OK;
+}
+
+}  // namespace qipb200
+namespace {
+
+// Whatever qipb200_state_set_basis or qipb200_state_measure left pending, applied to the amplitudes.
+int materialise_pending(qipb200_state *s) {
+  int st = qipb200::materialise_init(s);
+  return st != QIPB200_OK ? st : materialise_collapse(s);
+}
+
+// s's device made current and its pending work applied: the start of every call that reads s.
 int begin_device_work(qipb200_state *s) {
   CU(s->ctx, cudaSetDevice(s->ctx->device));
-  return materialise_collapse(s);
+  return materialise_pending(s);
 }
 
 int check_barrier_error(qipb200_state *s) {
@@ -1194,12 +1217,24 @@ extern "C" void qipb200_state_free(qipb200_state *s) {
   delete s;
 }
 
+// QIPB200_NO_INIT_FOLD=1: set_basis writes the state at once (read per call, so one process can compare both paths).
+static bool init_fold_enabled() {
+  const char *e = getenv("QIPB200_NO_INIT_FOLD");
+  return !(e && atoi(e) != 0);
+}
+
 static int set_basis_impl(qipb200_state *s, uint64_t index) {
   qipb200_ctx *ctx = s->ctx;
   if (index >> s->n) return set_err(ctx, QIPB200_ERR_BAD_INDEX, "initial index out of range");
   CU(ctx, cudaSetDevice(ctx->device));
   s->collapse_pending = false;  // every amplitude is overwritten
+  s->init_pending = false;
   for (uint32_t b = 0; b < s->n; ++b) s->phys_of_logical[b] = b;  // a fresh state has the canonical layout
+  if (s->world == 1 && init_fold_enabled()) {  // written by the next schedule's first tile pass, or before the next read
+    s->init_pending = true;
+    s->init_index = index;
+    return QIPB200_OK;
+  }
   const uint64_t len = 1ull << s->n_local;
   const bool owns = (index >> s->n_local) == (uint64_t)s->rank;
   CU(ctx, launch_set_basis(s->prec, s->buf, len, index & (len - 1), owns, ctx->stream, &ctx->launches));
@@ -1223,6 +1258,7 @@ static int transfer_impl(qipb200_state *s, void *host, uint64_t offset, uint64_t
   if (!host && len) return set_err(ctx, QIPB200_ERR_INVALID_ARG, std::string(what) + ": host pointer is NULL");
   if (len > (1ull << s->n_local) || offset > (1ull << s->n_local) - len)
     return set_err(ctx, QIPB200_ERR_SIZE_MISMATCH, std::string(what) + ": range exceeds the local state");
+  if (upload && len == (1ull << s->n_local)) s->init_pending = false;  // every amplitude is overwritten
   int st = begin_device_work(s);  // a partial upload keeps the other amplitudes
   if (st != QIPB200_OK) return st;
   if (!layout_is_identity(s)) {
@@ -1364,7 +1400,7 @@ static int max_abs_diff_impl(qipb200_state *a, qipb200_state *b, double *out) {
   if (a->phys_of_logical != b->phys_of_logical)
     return set_err(ctx, QIPB200_ERR_UNSUPPORTED, "max_abs_diff: the two sharded states hold different qubit layouts");
   int st = begin_device_work(a);
-  if (st == QIPB200_OK) st = materialise_collapse(b);
+  if (st == QIPB200_OK) st = materialise_pending(b);
   if (st != QIPB200_OK) return st;
   CU(ctx, launch_max_abs_diff(a->prec, a->buf, b->buf, 1ull << a->n_local, ctx->d_scalar, ctx->stream, &ctx->launches));
   CU(ctx, cudaMemcpyAsync(out, ctx->d_scalar, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1488,7 +1524,7 @@ int state_file_impl(qipb200_state *s, const char *path, bool save) {
   qipb200_ctx *ctx = s->ctx;
   CU(ctx, cudaSetDevice(ctx->device));
   if (save) {
-    int st = materialise_collapse(s);
+    int st = materialise_pending(s);
     if (st != QIPB200_OK) return st;
   }
   if (!layout_is_identity(s)) {  // files hold the canonical layout (collective on a sharded state)
@@ -1511,7 +1547,7 @@ int state_file_impl(qipb200_state *s, const char *path, bool save) {
     else if (h.prec != (uint32_t)s->prec || h.n_qubits != s->n || h.rank != (uint32_t)s->rank || h.world != (uint32_t)s->world ||
              h.n_amplitudes != len)
       st = set_err(ctx, QIPB200_ERR_SIZE_MISMATCH, "state file does not match the target state (prec/n/rank/world/length)");
-    if (st == QIPB200_OK) s->collapse_pending = false;  // every amplitude is overwritten
+    if (st == QIPB200_OK) s->collapse_pending = s->init_pending = false;  // every amplitude is overwritten
   }
   std::vector<char> bounce;
   if (st == QIPB200_OK) bounce.resize((size_t)std::min<uint64_t>(kFileChunkBytes, len * ab));
@@ -1953,11 +1989,11 @@ int check_finite(qipb200_ctx *ctx, const double *v, size_t n, const std::string 
   return QIPB200_OK;
 }
 
-// src's pending collapse runs, dst's is dropped (dst is overwritten), and dst takes src's layout.
+// src's pending work runs, dst's is dropped (dst is overwritten), and dst takes src's layout.
 int prepare_out_of_place(qipb200_state *dst, qipb200_state *src) {
-  int st = materialise_collapse(src);
+  int st = materialise_pending(src);
   if (st != QIPB200_OK) return st;
-  dst->collapse_pending = false;
+  dst->collapse_pending = dst->init_pending = false;
   dst->phys_of_logical = src->phys_of_logical;
   return QIPB200_OK;
 }
@@ -2035,7 +2071,7 @@ extern "C" int qipb200_state_transition_paulis(qipb200_state *bra, qipb200_state
     if (!out) return set_err(bra->ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL out");
     qipb200_ctx *ctx = bra->ctx;
     if ((st = begin_device_work(bra)) != QIPB200_OK) return st;
-    if ((st = materialise_collapse(ket)) != QIPB200_OK) return st;
+    if ((st = materialise_pending(ket)) != QIPB200_OK) return st;
     // One qubit map: the states are read where they are (Pauli masks permute with the bits).  Two maps: each permuted
     // state goes back to the canonical layout first, as before a download.
     if (bra->phys_of_logical != ket->phys_of_logical) {

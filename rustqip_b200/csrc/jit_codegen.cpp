@@ -181,7 +181,8 @@ uint32_t swz_units(bool f64, uint32_t t) { return f64 ? (t ^ ((t >> 3) & 7u)) : 
 
 }  // namespace
 
-bool jit_generate(const HostPass &pass, qip_prec prec, JitProgram *out, std::string *why, bool paired) {
+bool jit_generate(const HostPass &pass, qip_prec prec, JitProgram *out, std::string *why, bool paired,
+                  const uint64_t *synth_index) {
   std::string dummy;
   if (!why) why = &dummy;
   const PassHeader &h = pass.hdr;
@@ -736,6 +737,8 @@ bool jit_generate(const HostPass &pass, qip_prec prec, JitProgram *out, std::str
   src << "#define OFF_TBL " << off_tbl << "u\n#define OFF_GT " << off_gt << "u\n#define OFF_CONDW " << off_condw << "u\n#define OFF_MBAR "
       << off_mbar << "u\n";
   src << "#define QIP_PAIRED " << (paired ? 1 : 0) << "\n";
+  const bool synth = synth_index != nullptr;
+  src << "#define QIP_SYNTH " << (synth ? 1 : 0) << "\n";
   src << "typedef " << RT << " R;\n";
   src << "struct JP {\n  u64 box_off[NBOX];\n";
   if (NC) src << "  u64 cm[NC], cv[NC];\n";
@@ -747,6 +750,7 @@ bool jit_generate(const HostPass &pass, qip_prec prec, JitProgram *out, std::str
   if (NG) src << "  R gw[2 * NG];\n";
   src << "  unsigned hi_pos[8];\n";
   if (NPH) src << "  unsigned pt_begin[NPH + 1];\n";
+  if (synth) src << "  unsigned init_lo, init_hi;\n";  // the basis index the tiles are built from
   // multi-GPU: tiles whose index bit `send_bit` equals `send_val` are stored to `tmap_out` (the partner's staging
   // area) at the index with that bit flipped -- the push half of a qubit migration; send_bit >= 64: off
   src << "  unsigned send_bit, send_val;\n";
@@ -770,11 +774,13 @@ bool jit_generate(const HostPass &pass, qip_prec prec, JitProgram *out, std::str
 #define QIP_DEV static inline
 #define QFMA(a, b, c) std::fma((a), (b), (c))
 struct alignas(2 * sizeof(R)) QV { R x, y; };
+struct alignas(16) QZ { unsigned x, y, z, w; };
 #else
 #define QIP_DEV __device__ __forceinline__
 #define QFMA(a, b, c) fma((a), (b), (c))
 )";
   src << (f64 ? "typedef double2 QV;\n" : "typedef float2 QV;\n");
+  src << "typedef uint4 QZ;\n";
   src << "#endif\n\n";
   src << fn.str();
 
@@ -810,15 +816,37 @@ struct alignas(2 * sizeof(R)) QV { R x, y; };
   src << "  for (unsigned i = 0; i < TILE_M; ++i) {\n    const unsigned q = p.hi_pos[i];\n";
   src << "    base = ((base >> q) << (q + 1)) | (base & ((1ull << q) - 1ull));\n  }\n  return base;\n}\n\n";
 
+  // synthesised pass: the tile of a basis state, written in the layout the TMA load would leave (128-byte swizzle)
+  if (synth) {
+    src << "QIP_DEV void synth_fill(unsigned char* sm, const unsigned tid, const JP& p, const u64 base) {\n";
+    src << "  const u64 idx = ((u64)p.init_hi << 32) | (u64)p.init_lo;\n";
+    src << "  u64 rest = idx & ~((1ull << TILE_L) - 1ull);\n  unsigned t = (unsigned)(idx & ((1ull << TILE_L) - 1ull));\n";
+    src << "  for (unsigned i = 0; i < TILE_M; ++i) {\n    const u64 b = 1ull << p.hi_pos[i];\n";
+    src << "    if (idx & b) t |= 1u << (TILE_L + i);\n    rest &= ~b;\n  }\n";
+    src << (f64 ? "  t ^= (t >> 3) & 7u;\n" : "  t ^= ((t >> 4) & 7u) << 1;\n");
+    src << "  const unsigned hit = rest == base ? t * (unsigned)sizeof(QV) : 0xffffffffu;  // byte offset of the one\n";
+    src << "#pragma unroll 8\n  for (unsigned o = tid * 16u; o < TILE_BYTES; o += CTA_THREADS * 16u) {\n";
+    src << "    QZ v;\n    v.x = v.y = v.z = v.w = 0u;\n";
+    if (f64)
+      src << "    if (o == hit) v.y = 0x3ff00000u;  // 1.0 + 0i\n";
+    else
+      src << "    if (o == (hit & ~15u)) {  // 1.0f + 0i\n      if (hit & 8u) v.z = 0x3f800000u;\n      else v.x = 0x3f800000u;\n    }\n";
+    src << "    *reinterpret_cast<QZ*>(sm + o) = v;\n  }\n}\n\n";
+  }
+
   // ---- host harness (validation without a GPU) ----
   src << "#ifdef QIP_JIT_HOST\n";
   src << "extern \"C\" void qip_host_pass(R* psi, const JP* pp, unsigned n_local) {\n  const JP& p = *pp;\n";
   src << "  static unsigned char sm[OFF_MBAR + 64];\n  const u64 tiles = 1ull << (n_local - TILE_T);\n";
   src << "  for (u64 tile = 0; tile < tiles; ++tile) {\n    const u64 base = tile_base(p, tile);\n";
-  src << "    for (unsigned t = 0; t < (1u << TILE_T); ++t) {\n      u64 idx = base + (t & ((1u << TILE_L) - 1u));\n";
-  src << "      for (unsigned i = 0; i < TILE_M; ++i) if ((t >> (TILE_L + i)) & 1u) idx |= 1ull << p.hi_pos[i];\n";
-  src << (f64 ? "      const unsigned s = t ^ ((t >> 3) & 7u);\n" : "      const unsigned s = t ^ (((t >> 4) & 7u) << 1);\n");
-  src << "      memcpy(sm + s * sizeof(QV), psi + 2 * idx, sizeof(QV));\n    }\n";
+  if (synth) {
+    src << "    for (unsigned tid = 0; tid < " << kThreads << "u; ++tid) synth_fill(sm, tid, p, base);\n";
+  } else {
+    src << "    for (unsigned t = 0; t < (1u << TILE_T); ++t) {\n      u64 idx = base + (t & ((1u << TILE_L) - 1u));\n";
+    src << "      for (unsigned i = 0; i < TILE_M; ++i) if ((t >> (TILE_L + i)) & 1u) idx |= 1ull << p.hi_pos[i];\n";
+    src << (f64 ? "      const unsigned s = t ^ ((t >> 3) & 7u);\n" : "      const unsigned s = t ^ (((t >> 4) & 7u) << 1);\n");
+    src << "      memcpy(sm + s * sizeof(QV), psi + 2 * idx, sizeof(QV));\n    }\n";
+  }
   src << "    memset(sm + OFF_CONDW, 0, 48);\n";
   src << "    for (unsigned tid = 0; tid < " << kThreads << "u; ++tid) prelude(sm, tid, p, base);\n";
   for (size_t s = 0; s < S; ++s)
@@ -879,6 +907,10 @@ qip_pass(R* __restrict__ psi, const __grid_constant__ JP p, const __grid_constan
   const u64 tt = tile + tile_off;
 #endif
   const u64 base = tile_base(p, tt);
+#if QIP_SYNTH
+  if (tile != (u64)blockIdx.x) __syncthreads();  // the previous tile's stores have read the buffer (thread 0 waited)
+  synth_fill(sm, tid, p, base);
+#else
   if (tid == 0) {  // the tile buffer is free: this thread waited for the previous tile's stores to have read it
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mbar), "r"(TILE_BYTES) : "memory");
 #pragma unroll 1
@@ -903,14 +935,16 @@ qip_pass(R* __restrict__ psi, const __grid_constant__ JP p, const __grid_constan
                    : "memory");
     }
   }
+#endif
 )";
   src << "  prelude(sm, tid, p, base);\n";
   // (always needed with persistent CTAs: the previous tile's super-ops read what the prelude overwrites -- they are
   // all past the barrier before the stores -- and the prelude's results must be visible before the super-ops)
-  if (has_prelude) src << "  __syncthreads();\n";
+  // (a synthesised tile is written by all threads: it must be complete before the super-ops)
+  if (has_prelude || synth) src << "  __syncthreads();\n";
   src << "  const unsigned* condw = reinterpret_cast<const unsigned*>(sm + OFF_CONDW);\n";
   src << "  const R* tbl = reinterpret_cast<const R*>(sm + OFF_TBL);\n  const R* gt = reinterpret_cast<const R*>(sm + OFF_GT);\n";
-  src << "  mbar_wait(mbar, parity);\n";
+  if (!synth) src << "  mbar_wait(mbar, parity);\n";
   src << R"(#if QIP_PAIRED
   const bool pair_give = pair_my != 0ull && ((tt >> p.pair_cbit) & 1ull) == (u64)p.send_val;
   if (pair_give && tid == 0) {  // my copy of the tile is in shared memory: the partner may overwrite the slot
@@ -1041,6 +1075,10 @@ qip_pass(R* __restrict__ psi, const __grid_constant__ JP p, const __grid_constan
     }
     put(&at, 4);
   }
+  if (synth) {
+    const uint32_t w[2] = {(uint32_t)*synth_index, (uint32_t)(*synth_index >> 32)};
+    put(w, 8);
+  }
   out->send_offset = (uint32_t)blob.size();
   {
     const uint32_t off_bit = 64u, val = 0u;
@@ -1058,6 +1096,7 @@ qip_pass(R* __restrict__ psi, const __grid_constant__ JP p, const __grid_constan
 
   out->source = src.str();
   out->params.swap(blob);
+  out->synthesised = synth;
   out->smem_bytes = off_mbar + 64;
   out->threads = kThreads;
   out->tiles_log2_sub = T;

@@ -27,6 +27,7 @@ struct JitProgram {
   uint32_t threads = 256;
   uint32_t tiles_log2_sub = 0;        // grid = 1 << (n_local - T)
   uint32_t send_offset = 0;           // byte offset of JP::send_bit / send_val in `params` (patched per launch)
+  bool synthesised = false;           // the pass builds its tiles from a basis index instead of loading them
   // statistics
   uint32_t n_super = 0, n_elems = 0, n_cta_barriers = 0, n_warp_syncs = 0, n_renamed = 0, n_consts = 0;
 };
@@ -34,6 +35,9 @@ struct JitProgram {
 // Returns false (and says why) when the pass holds something the generator does not cover (wide micro-ops,
 // geometry without TMA boxes, > 256 CTA-uniform conditions ...): the caller then runs the interpreter kernel.
 // `paired`: the kernel can also play the per-tile handshake of a migration fused into the pass (multi-GPU, JP::pair_*).
-bool jit_generate(const HostPass &pass, qip_prec prec, JitProgram *out, std::string *why, bool paired = false);
+// `synth_index`: the pass is the first one on a state that is still the basis state |*synth_index> (unsharded): every
+// CTA fills its shared-memory tile with zeros and, in the tile that holds the index, a one, instead of loading the tile.
+bool jit_generate(const HostPass &pass, qip_prec prec, JitProgram *out, std::string *why, bool paired = false,
+                  const uint64_t *synth_index = nullptr);
 
 }  // namespace qipb200

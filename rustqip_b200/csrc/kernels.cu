@@ -1195,6 +1195,17 @@ cudaError_t launch_set_basis(qip_prec prec, void *psi, uint64_t len, uint64_t in
   return cudaGetLastError();
 }
 
+cudaError_t write_basis_state(qip_prec prec, void *psi, uint64_t len, uint64_t index, cudaStream_t s) {
+  const size_t amp = prec == QIP_F32 ? 8 : 16;
+  cudaError_t e = cudaMemsetAsync(psi, 0, len * amp, s);
+  // the real part is 1.0: its two top bytes (little endian) are 0x3FF0 as a double, 0x3F80 as a float
+  char *re = (char *)psi + index * amp;
+  const size_t top = prec == QIP_F32 ? 2 : 6;
+  if (e == cudaSuccess) e = cudaMemsetAsync(re + top, prec == QIP_F32 ? 0x80 : 0xF0, 1, s);
+  if (e == cudaSuccess) e = cudaMemsetAsync(re + top + 1, 0x3F, 1, s);
+  return e;
+}
+
 // measure_probs (measurement_ops.rs:115-127) as one histogram sweep: every amplitude
 // adds |a|^2 to the bin spelled by its measured bits.  Small histograms live in
 // shared memory per CTA and are flushed with one atomicAdd per bin.

@@ -56,6 +56,8 @@ cudaError_t launch_max_abs_diff(qip_prec prec, const void *a, const void *b, uin
                                 uint64_t *launches);
 cudaError_t launch_set_basis(qip_prec prec, void *psi, uint64_t len, uint64_t index, bool owns_index,
                              cudaStream_t s, uint64_t *launches);
+// The same state written with memsets only (no kernel): psi[index] = 1 + 0i, every other amplitude 0.
+cudaError_t write_basis_state(qip_prec prec, void *psi, uint64_t len, uint64_t index, cudaStream_t s);
 
 // Measurement (qip/src/state_ops/measurement_ops.rs).
 // hist[m] += sum of |a|^2 over amplitudes whose bits at bitpos[i] spell m (bit i of m <-> bitpos[i]).

@@ -80,7 +80,9 @@ int execute_steps(qipb200_state *s, const std::vector<PlanStep> &steps, const st
     for (size_t i = 0; i < steps.size(); ++i) {
       if (!steps[i].is_pass) continue;
       std::string why;
-      if (jit_generate(steps[i].pass, s->prec, &progs[i], &why, send.pair && i + 1 == steps.size())) {
+      // a state still pending as a basis state (unsharded only) is built by its first pass instead of being loaded
+      const uint64_t *synth = i == 0 && s->init_pending && s->world == 1 ? &s->init_index : nullptr;
+      if (jit_generate(steps[i].pass, s->prec, &progs[i], &why, send.pair && i + 1 == steps.size(), synth)) {
         have_prog[i] = 1;
         (void)jit_request(progs[i].source, false);  // all compilations of this schedule start now, in parallel
       } else {
@@ -164,6 +166,7 @@ int execute_steps(qipb200_state *s, const std::vector<PlanStep> &steps, const st
                            pair_here && tmo ? &pair : nullptr);
           }
           if (e == cudaSuccess) {
+            if (progs[i].synthesised) s->init_pending = false;
             if (pair_here && tmo)
               paired_done = true;
             else if (tmo)
@@ -179,6 +182,8 @@ int execute_steps(qipb200_state *s, const std::vector<PlanStep> &steps, const st
         }
       }
     }
+    // a step that reads the amplitudes: a pending basis state is written first (no generated synthesising pass ran)
+    if (s->init_pending && (st = materialise_init(s)) != QIPB200_OK) break;
     if (s->halves_pending && (st = join_halves(s)) != QIPB200_OK) break;  // this step sweeps the whole shard at once
     if (steps[i].is_pass) {
       if (!serialise_pass(steps[i].pass, pp)) {
@@ -357,6 +362,7 @@ static bool run_rotating(qipb200_state *s, const qip_op *ops, size_t n_ops, int 
   RotatePlan plan;
   std::string err;
   std::vector<uint32_t> layout = s->phys_of_logical;
+  if ((*status = materialise_init(s)) != QIPB200_OK) return true;  // the rotating passes always load their tiles
   if (plan_rotating(ops, n_ops, s->prec, s->n_local, cfg, &plan, &err, layout.data(), false) != QIPB200_OK) return false;
   s->phys_of_logical = layout;
   *status = execute_steps(s, plan.steps, plan.singles, cfg);
@@ -405,6 +411,10 @@ int run_schedule(qipb200_state *s, const qip_op *ops, size_t n_ops, uint32_t fla
     const int st = run_fused(s, ops, n_ops, next_use);
     const int stj = join_halves(s);  // whatever follows (download, measurement, the next schedule) sees one stream again
     return st != QIPB200_OK ? st : stj;
+  }
+  if (n_ops) {  // one sweep per entry: the pending basis state is written first
+    const int st = materialise_init(s);
+    if (st != QIPB200_OK) return st;
   }
   for (size_t i = 0; i < n_ops; ++i) {
     FlatOp f;

@@ -32,6 +32,8 @@ bool overlap_exchange_enabled();
 void paired_partner(const qipb200_state *s, uint32_t R, int *partner, int *give);
 int paired_send_standin(qipb200_state *s, uint32_t R, uint32_t l, uint32_t cbit, uint32_t seq, const PassHeader &hdr);
 int finish_paired_exchange(qipb200_state *s, uint32_t R, uint32_t l);
+// write the basis state qipb200_state_set_basis left pending (no-op when there is none)
+int materialise_init(qipb200_state *s);
 
 // qubit rotation (opt-in, QIPB200_ROTATE=1, unsharded states; planner.cpp: plan_rotating): is it on / run swap-only steps
 // that bring the state's layout back to the canonical one (api.cu: restore_layout)

@@ -91,6 +91,12 @@ struct qipb200_state {
   std::vector<uint64_t> pend_qubits;
   uint64_t pend_measured = 0;
   double pend_p_mult = 1.0;
+  // Basis state left pending by qipb200_state_set_basis (unsharded single-device states only): the amplitudes are
+  // |init_index>, but nothing has been written yet.  The next fused schedule whose first step is a generated tile pass
+  // builds its tiles from the index instead of loading them; every other access to the amplitudes writes the basis
+  // state first (api.cu: materialise_init).  Never set together with collapse_pending.
+  bool init_pending = false;
+  uint64_t init_index = 0;
 };
 
 namespace qipb200 {
