@@ -336,6 +336,45 @@ int qipb200_state_purity(qipb200_state *state, const uint64_t *qubits, uint32_t 
  * QIPB200_ERR_INVALID_ARG. */
 int qipb200_purity_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, uint32_t k, uint32_t *out4);
 
+/* Entanglement spectrum and von Neumann entropy of the cut between the k qubits `qubits` and the rest, on the state
+ * AS IT IS (not renormalised); absent in the reference.  The side is taken as by qipb200_state_purity: the qubits
+ * passed when k <= n - k, else their complement; s is its size and G its 2^s x 2^s matrix sum_r psi(r, a)
+ * conj(psi(r, b)) in the convention of qipb200_state_reduced_density (bit i of a row index is the value of side qubit
+ * i).  The nonzero spectra of both sides agree, so the eigenvalues do not depend on which side is passed.
+ *   eigs (HOST, eigs_cap >= 2^s doubles): the 2^s eigenvalues of G in descending order (the solver's values sorted
+ *     on the host: cuSOLVER's own order is ascending only up to rounding among nearly equal ones), not renormalised (the
+ *     squared Schmidt coefficients times the norm); values that come out slightly negative through rounding are
+ *     returned as computed.
+ *   out2[0] = T = sum_a G_aa in index order; out2[1] = -sum p_i ln p_i (nats) over the eigenvalues > 0 in ascending
+ *     order, p_i = lambda_i / T; 0 if T == 0.
+ *   rho (HOST, may be NULL; 2 * 4^s doubles, interleaved re/im, row-major): G.  The lower triangle is the exact
+ *     conjugate of the upper one and the diagonal's imaginary part is +0.0.  For s <= 10 these are the bits
+ *     qipb200_state_reduced_density returns; for s = 11..13 it extends that call.  Needs k <= n - k (rho is the
+ *     matrix of the qubits passed); otherwise QIPB200_ERR_INVALID_ARG asks for the complement.
+ * Routes by s alone, as qipb200_state_purity: s = 0 one norm2 sweep (eigs = {norm2}); 1 <= s <= 10
+ * qipb200_state_reduced_density of the side; 11 <= s <= 13 the purity Gram kernel with a store epilogue (one kernel,
+ * G on the device: 16 * 4^s bytes, 1 GiB at s = 13; order and error bound in rustqip_b200/csrc/purity.cu).  On routes
+ * 1 and 2 G is solved on the device by cuSOLVER (cusolverDnZheevd, eigenvalues only), loaded at run time with dlopen
+ * (libcusolver.so.11, then /usr/local/cuda/lib64); the library does not link it.  cuSOLVER's own kernels are not
+ * counted by qipb200_kernel_launches, which counts this library's kernels only.  Determinism: rho and out2[0] are
+ * bit-identical on repeated calls (fixed-order sums, no atomics); the eigenvalues are whatever cuSOLVER returns, and
+ * were bit-identical on repeated calls on an H100 (CUDA 12.9, cuSOLVER 11.7), which cuSOLVER does not promise.
+ * Synchronises; the state is read only.  A pending collapse is applied first (after the device buffers are
+ * allocated); a pending set_basis state is written first; a permuted layout is read as it is.
+ * Errors, all before any device work (a refused call leaves the state and anything pending on it as they were): NULL
+ * state, qubits, eigs or out2, k == 0 or k > n, eigs_cap < 2^s, and rho with k > n - k give QIPB200_ERR_INVALID_ARG;
+ * a qubit >= n or repeated QIPB200_ERR_BAD_INDEX; s >= 14, sharded and multi-device states, and a cuSOLVER that
+ * cannot be loaded (the message gives the loader's reason) QIPB200_ERR_UNSUPPORTED; G or the solver's workspace not
+ * allocatable QIPB200_ERR_OOM. */
+int qipb200_state_entanglement_spectrum(qipb200_state *state, const uint64_t *qubits, uint32_t k,
+                                        double *eigs, size_t eigs_cap, double *rho, double *out2);
+/* Host-only (no GPU, ctx-free): out5 = {route (0 norm2, 1 reduced_density, 2 Gram store), s, kernels this library
+ * launches (1, 2^m (2^m + 1) with m = max(0, s - 6), or 1), bytes of the device matrix (16 * 4^s; 0 on route 0),
+ * 1 if cuSOLVER loads in this process else 0} of the call above on an unsharded n-qubit state with nothing pending.
+ * Validates as qipb200_purity_plan does; s >= 14 gives QIPB200_ERR_UNSUPPORTED as the call does. */
+int qipb200_entanglement_spectrum_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, uint32_t k,
+                                       uint32_t *out5);
+
 /* psi <- exp(-i angles[T-1]/2 P_{T-1}) ... exp(-i angles[0]/2 P_0) psi: Pauli-string rotations, term 0 first; absent in
  * the reference.  Terms are encoded and validated as for qipb200_state_expect_paulis (same codes and messages), with
  * P = i^nY X^x Z^z, so a single 'Z' term is rz(q, angle) and a single 'X' term is Rx(angle); an empty term is the

@@ -17,6 +17,7 @@
 // P is float or double (trait Precision, qip/src/types.rs:6-13).
 #pragma once
 
+#include <algorithm>
 #include <complex>
 #include <cstdint>
 #include <memory>
@@ -491,6 +492,18 @@ class B200State {
     double out2[2] = {0.0, 0.0};
     ctx_.check(qipb200_state_purity(st_, qubits.data(), (uint32_t)qubits.size(), out2));
     return std::make_pair(out2[0], out2[1]);
+  }
+  // eigenvalues (descending, not renormalised) of the reduced density matrix across the cut of `qubits`, for a smaller
+  // side of s <= 13 qubits; *entropy (if given) gets the von Neumann entropy in nats of the normalised spectrum
+  // (absent in the reference)
+  std::vector<double> entanglement_spectrum(const std::vector<uint64_t> &qubits, double *entropy = nullptr) {
+    const size_t k = qubits.size(), s = std::min(k, n_ >= k ? n_ - k : 0);
+    std::vector<double> eigs((size_t)1 << std::min<size_t>(s, 13));
+    double out2[2] = {0.0, 0.0};
+    ctx_.check(qipb200_state_entanglement_spectrum(st_, qubits.data(), (uint32_t)k, eigs.data(), eigs.size(), nullptr,
+                                                   out2));
+    if (entropy) *entropy = out2[1];
+    return eigs;
   }
   // a schedule parsed from the QIPS wire format (owned by the library): builder.rs:423-514 on foreign circuits
   void apply_parsed(const qip_op *ops, size_t n_ops, bool fusion = true) {

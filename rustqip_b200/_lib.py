@@ -33,6 +33,7 @@ EXPORTS = [
     "qipb200_state_measure_prob", "qipb200_state_soft_measure", "qipb200_state_sample", "qipb200_state_collapse",
     "qipb200_state_measure", "qipb200_state_expect_paulis", "qipb200_expect_plan", "qipb200_state_transition_paulis",
     "qipb200_transition_plan", "qipb200_state_reduced_density", "qipb200_state_purity", "qipb200_purity_plan",
+    "qipb200_state_entanglement_spectrum", "qipb200_entanglement_spectrum_plan",
     "qipb200_state_apply_pauli_rotations", "qipb200_pauli_rotation_plan", "qipb200_function_new",
     "qipb200_function_free", "qipb200_state_apply_function", "qipb200_function_plan", "qipb200_function_new_code",
     "qipb200_function_set_params", "qipb200_function_code_compile", "qipb200_function_tabulate",
@@ -45,6 +46,40 @@ EXPORTS = [
     "qipb200_state_qubit_map", "qipb200_state_exchange_bytes", "qipb200_plan_exchanges",
     "qipb200_state_save", "qipb200_state_load", "qipb200_schedule_parse", "qipb200_schedule_ops", "qipb200_schedule_free", "qipb200_schedule_serialise",
 ]
+
+
+_cusolver_checked = False
+
+
+def preload_cusolver():
+    """Optional, once per process, before the first entanglement-spectrum call: the library loads cuSOLVER with dlopen
+    (libcusolver.so.11 on the loader path, then the CUDA toolkit's lib64).  Where neither exists, the copy that ships
+    with the torch wheel (the nvidia-cusolver-cu12 package) is loaded here with RTLD_GLOBAL, its dependencies first, so
+    that the library's dlopen finds it by name.  Nothing else depends on it; QIPB200_NO_CUSOLVER_PRELOAD=1 skips it."""
+    global _cusolver_checked
+    if _cusolver_checked or os.environ.get("QIPB200_NO_CUSOLVER_PRELOAD") == "1":
+        return
+    _cusolver_checked = True
+    for name in ("libcusolver.so.11", "/usr/local/cuda/lib64/libcusolver.so.11"):
+        try:
+            C.CDLL(name)
+            return
+        except OSError:
+            pass
+    try:
+        import nvidia  # the namespace package of the CUDA wheels torch depends on
+    except ImportError:
+        return
+    for base in nvidia.__path__:
+        for pkg, so in (("nvjitlink", "libnvJitLink.so.12"), ("cublas", "libcublasLt.so.12"),
+                        ("cublas", "libcublas.so.12"), ("cusparse", "libcusparse.so.12"),
+                        ("cusolver", "libcusolver.so.11")):
+            path = os.path.join(base, pkg, "lib", so)
+            if os.path.exists(path):
+                try:
+                    C.CDLL(path, mode=C.RTLD_GLOBAL)
+                except OSError:
+                    return
 
 
 def lib():
@@ -121,6 +156,10 @@ def lib():
     L.qipb200_state_purity.argtypes = [vp, vp, u32, vp]
     L.qipb200_purity_plan.restype = i32
     L.qipb200_purity_plan.argtypes = [i32, u32, vp, u32, vp]
+    L.qipb200_state_entanglement_spectrum.restype = i32
+    L.qipb200_state_entanglement_spectrum.argtypes = [vp, vp, u32, vp, C.c_size_t, vp, vp]
+    L.qipb200_entanglement_spectrum_plan.restype = i32
+    L.qipb200_entanglement_spectrum_plan.argtypes = [i32, u32, vp, u32, vp]
     L.qipb200_state_apply_pauli_rotations.restype = i32
     L.qipb200_state_apply_pauli_rotations.argtypes = [vp, vp, vp, vp, C.c_size_t, vp]
     L.qipb200_pauli_rotation_plan.restype = i32

@@ -12,6 +12,7 @@
 #include <cstdio>
 #include <cstring>
 #include <exception>
+#include <memory>
 #include <new>
 #include <thread>
 #include <string>
@@ -30,6 +31,7 @@
 #include "purity.h"
 #include "rdm.h"
 #include "schedule.h"
+#include "spectrum.h"
 #include "tile.cuh"
 #include "jit_codegen.h"
 #include "state.h"
@@ -248,6 +250,7 @@ extern "C" void qipb200_shutdown(qipb200_ctx *ctx) {
     }
   for (size_t i = 0; i < ctx->prof_pool.size(); ++i) cudaEventDestroy(ctx->prof_pool[i]);
   jit_unload(&ctx->jit_loaded);
+  eig_handle_destroy(ctx->eig_solver);
   for (int i = 0; i < 2; ++i) {
     if (ctx->ev_pass[i]) cudaEventDestroy(ctx->ev_pass[i]);
     if (ctx->ev_exch[i]) cudaEventDestroy(ctx->ev_exch[i]);
@@ -2137,6 +2140,18 @@ extern "C" int qipb200_state_reduced_density(qipb200_state *s, const uint64_t *q
 
 namespace {
 
+// The kept qubits of a host-only plan of a cut: 1..n distinct qubits below n.
+int check_plan_cut(const std::string &who, uint32_t n_qubits, const uint64_t *qubits, uint32_t k) {
+  if (!qubits || k == 0 || k > n_qubits) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, who + ": bad qubit list");
+  uint64_t seen = 0;
+  for (uint32_t i = 0; i < k; ++i) {
+    if (qubits[i] >= n_qubits) return set_err(nullptr, QIPB200_ERR_BAD_INDEX, who + ": qubit index out of range");
+    if ((seen >> qubits[i]) & 1) return set_err(nullptr, QIPB200_ERR_BAD_INDEX, who + ": repeated qubit index");
+    seen |= 1ull << qubits[i];
+  }
+  return QIPB200_OK;
+}
+
 // The side of the cut: the kept qubits if they are at most half, else their complement (Tr rho_A^2 = Tr rho_B^2).
 std::vector<uint64_t> purity_side(uint32_t n, const uint64_t *qubits, uint32_t k) {
   std::vector<uint64_t> side;
@@ -2209,21 +2224,157 @@ extern "C" int qipb200_state_purity(qipb200_state *s, const uint64_t *qubits, ui
 extern "C" int qipb200_purity_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, uint32_t k,
                                    uint32_t *out4) {
   return guarded(nullptr, [&]() -> int {
-    const int st = check_plan_args("purity_plan", prec, n_qubits, out4, "out4");
+    int st = check_plan_args("purity_plan", prec, n_qubits, out4, "out4");
+    if (st == QIPB200_OK) st = check_plan_cut("purity_plan", n_qubits, qubits, k);
     if (st != QIPB200_OK) return st;
-    if (!qubits || k == 0 || k > n_qubits)
-      return set_err(nullptr, QIPB200_ERR_INVALID_ARG, "purity_plan: bad qubit list");
-    uint64_t seen = 0;
-    for (uint32_t i = 0; i < k; ++i) {
-      if (qubits[i] >= n_qubits) return set_err(nullptr, QIPB200_ERR_BAD_INDEX, "purity_plan: qubit index out of range");
-      if ((seen >> qubits[i]) & 1) return set_err(nullptr, QIPB200_ERR_BAD_INDEX, "purity_plan: repeated qubit index");
-      seen |= 1ull << qubits[i];
-    }
     const uint32_t sb = std::min(k, n_qubits - k);
     out4[0] = purity_route(sb);
     out4[1] = sb;
     out4[2] = (uint32_t)purity_launch_count(sb);
     out4[3] = out4[0] == 2 ? (uint32_t)purity_gram_blocks(sb) : 0;
+    return (int)QIPB200_OK;
+  });
+}
+
+// ===================================================================================
+// entanglement spectrum of a bipartition (purity.cu store epilogue + spectrum.cu)
+// ===================================================================================
+
+namespace {
+
+// Device bytes of G for a side of s qubits (0 on the s = 0 route, which needs no matrix).
+uint64_t spectrum_matrix_bytes(uint32_t s) { return s == 0 ? 0 : (16ull << (2 * s)); }
+
+uint64_t spectrum_launch_count(uint32_t s) {
+  switch (purity_route(s)) {
+    case 0: return 1;
+    case 1: return rdm_launch_count(s);
+    default: return 1;
+  }
+}
+
+int spectrum_side_too_large(const qipb200_ctx *ctx, const std::string &who, uint32_t sb) {
+  return set_err(ctx, QIPB200_ERR_UNSUPPORTED,
+                 who + ": the smaller side has " + std::to_string(sb) +
+                     " qubits; at most 13 are supported (the matrix of 14 would be 4 GiB or more)");
+}
+
+// out2[0] = sum of the diagonal in index order; out2[1] = -sum p ln p over the eigenvalues > 0 in ascending order,
+// p = lambda / T; eigs = the eigenvalues in descending order.  cuSOLVER's values are ascending only up to rounding
+// among (nearly) equal ones, so they are sorted here first.
+void spectrum_finish(std::vector<double> asc, double trace, double *eigs, double *out2) {
+  std::sort(asc.begin(), asc.end());
+  const size_t K = asc.size();
+  double h = 0.0;
+  if (trace != 0.0)
+    for (size_t i = 0; i < K; ++i)
+      if (asc[i] > 0.0) {
+        const double p = asc[i] / trace;
+        h -= p * std::log(p);
+      }
+  for (size_t i = 0; i < K; ++i) eigs[i] = asc[K - 1 - i];
+  out2[0] = trace;
+  out2[1] = h;
+}
+
+int spectrum_impl(qipb200_state *s, const uint64_t *qubits, uint32_t k, double *eigs, double *rho, double *out2) {
+  qipb200_ctx *ctx = s->ctx;
+  const std::vector<uint64_t> side = purity_side(s->n, qubits, k);
+  const uint32_t sb = (uint32_t)side.size();
+  const size_t K = (size_t)1 << sb;
+  const uint32_t route = purity_route(sb);
+  // The solver handle and every device buffer come before the state is touched: a refusal for memory leaves the
+  // state and anything pending on it as they were.
+  CU(ctx, cudaSetDevice(ctx->device));
+  EigWork w;
+  if (route != 0) {
+    std::string err;
+    const int st = eig_work_alloc(&ctx->eig_solver, (uint32_t)K, &w, ctx->stream, &err);
+    if (st != QIPB200_OK) return set_err(ctx, st, "entanglement_spectrum: " + err);
+  }
+  struct Release {
+    EigWork *w;
+    cudaStream_t s;
+    ~Release() {
+      eig_work_free(w, s);
+      cudaStreamSynchronize(s);
+    }
+  } release{&w, ctx->stream};
+  int st = begin_device_work(s);
+  if (st != QIPB200_OK) return st;
+  // A state left permuted (QIPB200_ROTATE) is read where it is, as by purity.
+  std::vector<uint32_t> pos(sb);
+  phys_positions(s, side.data(), sb, pos.data());
+  double trace = 0.0;
+  if (route == 0) {
+    CU(ctx, run_purity_norm2(s->prec, s->buf, s->n_local, &trace, ctx->stream, &ctx->launches));
+    spectrum_finish(std::vector<double>(1, trace), trace, eigs, out2);
+    return QIPB200_OK;
+  }
+  std::vector<double> diag(K);
+  if (route == 1) {
+    std::unique_ptr<double[]> own(rho ? nullptr : new double[2 * K * K]);  // rho itself when given
+    double *host = rho ? rho : own.get();
+    CU(ctx, run_reduced_density(s->prec, s->buf, s->n_local, pos.data(), sb, host, ctx->stream, &ctx->launches));
+    for (size_t a = 0; a < K; ++a) diag[a] = host[2 * (a * K + a)];
+    CU(ctx, cudaMemcpyAsync(w.G, host, 16 * K * K, cudaMemcpyHostToDevice, ctx->stream));
+    CU(ctx, cudaStreamSynchronize(ctx->stream));  // own is released when this block ends
+  } else {
+    CU(ctx, run_gram_store(s->prec, s->buf, s->n_local, pos.data(), sb, w.G, ctx->stream, &ctx->launches));
+    if (rho) CU(ctx, cudaMemcpyAsync(rho, w.G, 16 * K * K, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(ctx, cudaMemcpy2DAsync(diag.data(), sizeof(double), w.G, (K + 1) * sizeof(double2), sizeof(double), K,
+                              cudaMemcpyDeviceToHost, ctx->stream));
+    CU(ctx, cudaStreamSynchronize(ctx->stream));
+  }
+  for (size_t a = 0; a < K; ++a) trace += diag[a];
+  std::vector<double> asc(K);
+  std::string err;
+  st = eig_solve(ctx->eig_solver, &w, ctx->stream, asc.data(), &err);
+  if (st != QIPB200_OK) return set_err(ctx, st, "entanglement_spectrum: " + err);
+  spectrum_finish(asc, trace, eigs, out2);
+  return QIPB200_OK;
+}
+
+}  // namespace
+
+extern "C" int qipb200_state_entanglement_spectrum(qipb200_state *s, const uint64_t *qubits, uint32_t k, double *eigs,
+                                                   size_t eigs_cap, double *rho, double *out2) {
+  if (!s) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, "entanglement_spectrum: NULL state");
+  return guarded(s->ctx, [&]() -> int {
+    if (!eigs || !out2) return set_err(s->ctx, QIPB200_ERR_INVALID_ARG, "entanglement_spectrum: NULL eigs or out2");
+    int st = check_indices(s, qubits, k);
+    if (st == QIPB200_OK) st = require_unsharded(s, "entanglement_spectrum");
+    if (st != QIPB200_OK) return st;
+    const uint32_t sb = std::min(k, s->n - k);
+    if (sb > kSpectrumMaxSide) return spectrum_side_too_large(s->ctx, "entanglement_spectrum", sb);
+    if (eigs_cap < ((size_t)1 << sb))
+      return set_err(s->ctx, QIPB200_ERR_INVALID_ARG,
+                     "entanglement_spectrum: eigs_cap " + std::to_string(eigs_cap) + " is below the " +
+                         std::to_string(1ull << sb) + " eigenvalues of the side");
+    if (rho && k > s->n - k)
+      return set_err(s->ctx, QIPB200_ERR_INVALID_ARG,
+                     "entanglement_spectrum: rho is the matrix of the smaller side; k > n - k, so pass the "
+                     "complement of these qubits to get it");
+    std::string why;
+    if (sb > 0 && !eig_solver_available(&why))
+      return set_err(s->ctx, QIPB200_ERR_UNSUPPORTED, "entanglement_spectrum: the eigen-solver is unavailable: " + why);
+    return spectrum_impl(s, qubits, k, eigs, rho, out2);
+  });
+}
+
+extern "C" int qipb200_entanglement_spectrum_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, uint32_t k,
+                                                  uint32_t *out5) {
+  return guarded(nullptr, [&]() -> int {
+    int st = check_plan_args("entanglement_spectrum_plan", prec, n_qubits, out5, "out5");
+    if (st == QIPB200_OK) st = check_plan_cut("entanglement_spectrum_plan", n_qubits, qubits, k);
+    if (st != QIPB200_OK) return st;
+    const uint32_t sb = std::min(k, n_qubits - k);
+    if (sb > kSpectrumMaxSide) return spectrum_side_too_large(nullptr, "entanglement_spectrum_plan", sb);
+    out5[0] = purity_route(sb);
+    out5[1] = sb;
+    out5[2] = (uint32_t)spectrum_launch_count(sb);
+    out5[3] = (uint32_t)spectrum_matrix_bytes(sb);
+    out5[4] = eig_solver_available(nullptr) ? 1 : 0;
     return (int)QIPB200_OK;
   });
 }

@@ -40,6 +40,17 @@
 //   |T_got - T| <= gamma_{D+E} T.
 // By Cauchy-Schwarz sum_{a,b} |G_ab| W_ab <= T^2, which gives a bound from the outputs alone.  tests/purity_ref.py
 // evaluates both forms.
+//
+// The store epilogue (qipb200_state_entanglement_spectrum, sides of 11..13 qubits) runs the same main loop and writes
+// G instead of folding it: k_purity_gram<R, true> stores every accumulator entry of its block that lies on or above
+// the diagonal into a device G of 4^s double2 (1 GiB at s = 13), row-major in the side-qubit convention of
+// reduced_density (bit i of a row index is the value of side qubit i).  The rows' indices in that convention, a' and
+// b', are built with the physical offsets into the same shared-memory tables (sideA / sideB next to rowA / rowB).
+// Entry (a, b) with a < b writes G_a'b' = (Re, Im) and G_b'a' = (Re, -Im), the exact conjugate; a diagonal entry
+// writes (Re, +0.0); entries below the diagonal of a straddling block write nothing (their mirror is written by the
+// block holding (b, a), which also runs).  Each entry is the accumulator of one fixed DMMA sequence, so G is
+// deterministic, and every stored entry is within |dG_ab| <= sqrt(2) gamma_D W_ab of the exact one, hence
+// ||dG||_F <= sqrt(2) gamma_D ||W||_F <= sqrt(2) gamma_D T (W = |M| |M|^T, ||W||_F <= || |M| ||_F^2 = T).  One kernel.
 #include "purity.h"
 
 #include <algorithm>
@@ -70,12 +81,14 @@ struct GramArgs {
 
 // Shared memory per stage: the two panels, column-major (inner index k, then row), each column padded so that the
 // 8 (16-byte) or 16 (8-byte) lanes of a fragment load hit distinct banks.
-template <typename V>
+// The store epilogue adds the rows' side indices (uint32) after the offset tables.
+template <typename V, bool Store>
 struct GramSmem {
   static constexpr int PAD = sizeof(V) == 16 ? 2 : 4;
   static constexpr int LDA = kGramBM + PAD, LDB = kGramBN + PAD;
   static constexpr int STAGE = kGramBK * (LDA + LDB);  // elements of V
-  static constexpr size_t TABLE_BYTES = (kGramBM + kGramBN + kGramBK) * sizeof(uint64_t);
+  static constexpr size_t TABLE_BYTES =
+      (kGramBM + kGramBN + kGramBK) * sizeof(uint64_t) + (Store ? (kGramBM + kGramBN) * sizeof(uint32_t) : 0);
   static constexpr size_t BYTES = TABLE_BYTES + (size_t)kGramStages * STAGE * sizeof(V);
 };
 
@@ -93,15 +106,29 @@ __device__ __forceinline__ void dmma(double (&c)[4], const double (&a)[4], doubl
                : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(b0), "d"(b1));
 }
 
-template <typename R>
+// The row index of G in the side-qubit convention: bit r of x (the r-th lowest bit of S) moves to bit lbits[r], the
+// 4-bit field r of lbits.
+__device__ __forceinline__ uint32_t side_index(uint64_t x, uint64_t lbits) {
+  uint32_t r = 0;
+  for (; x; x >>= 1, lbits >>= 4)
+    if (x & 1) r |= 1u << (lbits & 15);
+  return r;
+}
+
+// Store == false: the purity epilogue, out = the CTA slots, lbits unused.  Store == true: out = G (4^s entries,
+// row-major in the side-qubit convention), lbits as side_index takes it.
+template <typename R, bool Store>
 __global__ void __launch_bounds__(kGramThreads, 1)
-    k_purity_gram(const R *__restrict__ psi, const __grid_constant__ GramArgs g, double2 *__restrict__ slots) {
+    k_purity_gram(const R *__restrict__ psi, const __grid_constant__ GramArgs g, double2 *__restrict__ out,
+                  uint64_t lbits) {
   typedef typename SweepV<R>::type V;
-  typedef GramSmem<V> SM;
+  typedef GramSmem<V, Store> SM;
   extern __shared__ __align__(16) unsigned char smem[];
   uint64_t *rowA = reinterpret_cast<uint64_t *>(smem);
   uint64_t *rowB = rowA + kGramBM;
   uint64_t *koff = rowB + kGramBN;
+  uint32_t *sideA = reinterpret_cast<uint32_t *>(koff + kGramBK);  // Store only: a' of each row of the block
+  uint32_t *sideB = sideA + kGramBM;                                 // and b' of each column
   V *stages = reinterpret_cast<V *>(smem + SM::TABLE_BYTES);
   const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
   const int gid = lane >> 2, tig = lane & 3;
@@ -113,11 +140,13 @@ __global__ void __launch_bounds__(kGramThreads, 1)
   while (b >= 2ull * (g.n_rows - I)) b -= 2ull * (g.n_rows - I++);
   const uint32_t J = 2 * I + (uint32_t)b;
 
-  if (t < kGramBM)
+  if (t < kGramBM) {
     rowA[t] = pdep(((uint64_t)I << kGramBMLog2) + t, g.side);
-  else if (t < kGramBM + kGramBN)
+    if constexpr (Store) sideA[t] = side_index(((uint64_t)I << kGramBMLog2) + t, lbits);
+  } else if (t < kGramBM + kGramBN) {
     rowB[t - kGramBM] = pdep(((uint64_t)J << (kGramBMLog2 - 1)) + (t - kGramBM), g.side);
-  else if (t < kGramBM + kGramBN + kGramBK)
+    if constexpr (Store) sideB[t - kGramBM] = side_index(((uint64_t)J << (kGramBMLog2 - 1)) + (t - kGramBM), lbits);
+  } else if (t < kGramBM + kGramBN + kGramBK)
     koff[t - kGramBM - kGramBN] = pdep(t - kGramBM - kGramBN, g.other);
   __syncthreads();
 
@@ -211,6 +240,27 @@ __global__ void __launch_bounds__(kGramThreads, 1)
   cp_async_wait<0>();
 
   // accumulator c of tile (mt, nt) is entry (gid + 8 (c >> 1), 2 tig + (c & 1)) of the tile
+  if constexpr (Store) {
+    const uint64_t K = (uint64_t)g.n_rows << kGramBMLog2;
+    const int64_t a0 = ((int64_t)I << kGramBMLog2) + wm * 64 + gid, b0 = ((int64_t)J << (kGramBMLog2 - 1)) + wn * 16 + 2 * tig;
+#pragma unroll
+    for (int mt = 0; mt < 4; ++mt)
+#pragma unroll
+      for (int nt = 0; nt < 2; ++nt)
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          const int ra = wm * 64 + mt * 16 + gid + 8 * (c >> 1), rb = wn * 16 + nt * 8 + 2 * tig + (c & 1);
+          const int64_t a = a0 + mt * 16 + 8 * (c >> 1), bb = b0 + nt * 8 + (c & 1);
+          const uint64_t la = sideA[ra], lb = sideB[rb];
+          if (a == bb) {
+            out[la * K + la] = make_double2(re[mt][nt][c], 0.0);
+          } else if (a < bb) {
+            out[la * K + lb] = make_double2(re[mt][nt][c], im[mt][nt][c]);
+            out[lb * K + la] = make_double2(re[mt][nt][c], -im[mt][nt][c]);
+          }
+        }
+    return;
+  }
   double p = 0.0, tr = 0.0;
   const int64_t a0 = ((int64_t)I << kGramBMLog2) + wm * 64 + gid, b0 = ((int64_t)J << (kGramBMLog2 - 1)) + wn * 16 + 2 * tig;
 #pragma unroll
@@ -236,7 +286,7 @@ __global__ void __launch_bounds__(kGramThreads, 1)
     }
     __syncthreads();
   }
-  if (t == 0) slots[blockIdx.x] = red[0];
+  if (t == 0) out[blockIdx.x] = red[0];
 }
 
 // out2 = the sum of the slots in block order, by one CTA: thread t adds slots t, t + 256, ..., then a fixed binary tree.
@@ -304,15 +354,32 @@ __global__ void __launch_bounds__(kGramThreads) k_purity_norm2(const R *__restri
   }
 }
 
-template <typename R>
-cudaError_t launch_gram(const void *psi, const GramArgs &g, uint64_t n_blocks, double2 *slots, cudaStream_t s) {
-  typedef GramSmem<typename SweepV<R>::type> SM;
+template <typename R, bool Store>
+cudaError_t launch_gram(const void *psi, const GramArgs &g, uint64_t n_blocks, double2 *out, uint64_t lbits,
+                        cudaStream_t s) {
+  typedef GramSmem<typename SweepV<R>::type, Store> SM;
   static_assert(SM::BYTES <= 227 * 1024, "one CTA per SM: at most 227 KiB of shared memory");
   static_assert(kGramThreads * sizeof(double2) <= SM::BYTES, "the CTA reduction reuses the stage buffers");
-  cudaError_t e = cudaFuncSetAttribute(k_purity_gram<R>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SM::BYTES);
+  cudaError_t e =
+      cudaFuncSetAttribute(k_purity_gram<R, Store>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SM::BYTES);
   if (e != cudaSuccess) return e;
-  k_purity_gram<R><<<(unsigned)n_blocks, kGramThreads, SM::BYTES, s>>>((const R *)psi, g, slots);
+  k_purity_gram<R, Store><<<(unsigned)n_blocks, kGramThreads, SM::BYTES, s>>>((const R *)psi, g, out, lbits);
   return cudaGetLastError();
+}
+
+// The kernel's arguments for the side side_mask (s = popcount >= 7) of an unsharded 2^n state.
+GramArgs gram_args(uint32_t n, uint64_t side_mask) {
+  const uint32_t sb = (uint32_t)__builtin_popcountll(side_mask);
+  GramArgs g;
+  g.side = side_mask;
+  g.other = ((n >= 64 ? 0ull : 1ull << n) - 1) & ~side_mask;
+  uint64_t low = g.other;
+  for (int i = 0; i < 4; ++i) low &= low - 1;  // clear the 4 lowest bits of O
+  g.other_hi = low;
+  g.n_chunks = 1ull << (n - sb - 4);
+  g.n_rows = 1u << (sb - kGramBMLog2);
+  g.k_fast = g.other & 1;
+  return g;
 }
 
 }  // namespace
@@ -360,21 +427,14 @@ uint64_t purity_launch_count(uint32_t s) {
 cudaError_t run_purity_gram(qip_prec prec, const void *psi, uint32_t n, uint64_t side_mask, double *out2,
                             cudaStream_t s, uint64_t *launches) {
   const uint32_t sb = (uint32_t)__builtin_popcountll(side_mask);
-  GramArgs g;
-  g.side = side_mask;
-  g.other = ((n >= 64 ? 0ull : 1ull << n) - 1) & ~side_mask;
-  uint64_t low = g.other;
-  for (int i = 0; i < 4; ++i) low &= low - 1;  // clear the 4 lowest bits of O
-  g.other_hi = low;
-  g.n_chunks = 1ull << (n - sb - 4);
-  g.n_rows = 1u << (sb - kGramBMLog2);
-  g.k_fast = g.other & 1;
+  const GramArgs g = gram_args(n, side_mask);
   const uint64_t n_blocks = purity_gram_blocks(sb);
   double2 *d = nullptr;
   cudaError_t e = cudaMallocAsync((void **)&d, (n_blocks + 1) * sizeof(double2), s);
   if (e != cudaSuccess) return e;
   double2 *d_out = d + n_blocks;
-  e = prec == QIP_F32 ? launch_gram<float>(psi, g, n_blocks, d, s) : launch_gram<double>(psi, g, n_blocks, d, s);
+  e = prec == QIP_F32 ? launch_gram<float, false>(psi, g, n_blocks, d, 0, s)
+                      : launch_gram<double, false>(psi, g, n_blocks, d, 0, s);
   ++*launches;
   if (e == cudaSuccess) {
     k_purity_reduce<<<1, kGramThreads, 0, s>>>(d, n_blocks, reinterpret_cast<double *>(d_out));
@@ -384,6 +444,23 @@ cudaError_t run_purity_gram(qip_prec prec, const void *psi, uint32_t n, uint64_t
   if (e == cudaSuccess) e = cudaMemcpyAsync(out2, d_out, 2 * sizeof(double), cudaMemcpyDeviceToHost, s);
   const cudaError_t ef = cudaFreeAsync(d, s);
   if (e == cudaSuccess) e = ef;
+  const cudaError_t es = cudaStreamSynchronize(s);
+  return e == cudaSuccess ? es : e;
+}
+
+cudaError_t run_gram_store(qip_prec prec, const void *psi, uint32_t n, const uint32_t *pos, uint32_t sb, double2 *G,
+                           cudaStream_t s, uint64_t *launches) {
+  uint64_t side_mask = 0;
+  for (uint32_t i = 0; i < sb; ++i) side_mask |= 1ull << pos[i];
+  // field r of lbits: the side qubit i whose physical bit pos[i] is the r-th lowest bit of the mask
+  uint64_t lbits = 0;
+  for (uint32_t i = 0; i < sb; ++i)
+    lbits |= (uint64_t)i << (4 * __builtin_popcountll(side_mask & ((1ull << pos[i]) - 1)));
+  const GramArgs g = gram_args(n, side_mask);
+  const uint64_t n_blocks = purity_gram_blocks(sb);
+  const cudaError_t e = prec == QIP_F32 ? launch_gram<float, true>(psi, g, n_blocks, G, lbits, s)
+                                        : launch_gram<double, true>(psi, g, n_blocks, G, lbits, s);
+  ++*launches;
   const cudaError_t es = cudaStreamSynchronize(s);
   return e == cudaSuccess ? es : e;
 }

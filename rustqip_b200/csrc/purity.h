@@ -25,6 +25,13 @@ uint64_t purity_launch_count(uint32_t s);
 cudaError_t run_purity_gram(qip_prec prec, const void *psi, uint32_t n, uint64_t side_mask, double *out2,
                             cudaStream_t s, uint64_t *launches);
 
+// G = M M^dagger of the side qubits at physical bits pos[0..sb) (11 <= sb <= 13, sb <= n - sb) of an unsharded 2^n
+// state into the device array G (4^sb double2, row-major): bit i of a row or column index is the value of physical bit
+// pos[i].  The lower triangle is the exact conjugate of the upper one and the diagonal's imaginary part is +0.0.  One
+// kernel (the store epilogue of the purity Gram kernel).  Synchronises the stream.
+cudaError_t run_gram_store(qip_prec prec, const void *psi, uint32_t n, const uint32_t *pos, uint32_t sb, double2 *G,
+                           cudaStream_t s, uint64_t *launches);
+
 // *out = sum_j |psi_j|^2 of an unsharded 2^n state in a fixed order (one kernel; the s = 0 route).  Synchronises.
 cudaError_t run_purity_norm2(qip_prec prec, const void *psi, uint32_t n, double *out, cudaStream_t s,
                              uint64_t *launches);

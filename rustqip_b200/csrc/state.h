@@ -52,6 +52,7 @@ struct qipb200_ctx {
   void *d_in = nullptr, *d_out = nullptr;
   size_t d_in_bytes = 0, d_out_bytes = 0;
   double *d_scalar = nullptr;   // one device double for reductions
+  void *eig_solver = nullptr;   // cuSOLVER handle of qipb200_state_entanglement_spectrum, created on first use
   void *h_pinned = nullptr;     // pinned bounce buffer for downloads/uploads
   size_t h_pinned_bytes = 0;
 };

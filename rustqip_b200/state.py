@@ -477,6 +477,46 @@ class State:
         p, tr = self._purity2(qubits)
         return -float(np.log(p / (tr * tr)))
 
+    def _spectrum(self, qubits, rho):
+        idx = np.ascontiguousarray(np.asarray(list(qubits), dtype=np.uint64))
+        k = len(idx)
+        s = min(max(0, min(k, self.n - k)), 13)  # larger sides are refused by the call
+        eigs = np.zeros(1 << s)
+        out2 = np.zeros(2)
+        r = np.zeros(1 << (2 * s), dtype=np.complex128) if rho else None
+        _lib.preload_cusolver()
+        self._chk(_lib.lib().qipb200_state_entanglement_spectrum(
+            self._h, _ptr(idx) if k else None, k, _ptr(eigs), eigs.size, _ptr(r) if rho else None, _ptr(out2)))
+        return eigs, (r.reshape(1 << s, 1 << s) if rho else None), float(out2[0]), float(out2[1])
+
+    def entanglement_spectrum(self, qubits: Sequence[int], rho: bool = False):
+        """Eigenvalues of the reduced density matrix across the cut between ``qubits`` and the rest, on the state as
+        it is (not renormalised), in descending order: 2^s values for the smaller side of s = min(k, n - k) <= 13
+        qubits.  They are the squared Schmidt coefficients times ``norm2()``, and the same whichever side is passed.
+
+        With ``rho=True`` returns ``(eigs, rho)``, rho the side's 2^s x 2^s matrix (complex128) in the convention of
+        ``reduced_density`` (which it equals for s <= 10); that needs k <= n - k, so that it is the matrix of the qubits
+        passed.  The matrix is formed on the device (``reduced_density`` for s <= 10, the purity Gram kernel storing G
+        for s = 11..13) and solved there by cuSOLVER; ``entanglement_spectrum_plan`` reports the route."""
+        eigs, r, _, _ = self._spectrum(qubits, rho)
+        return (eigs, r) if rho else eigs
+
+    def entanglement_entropy(self, qubits: Sequence[int], alpha: float = 1.0) -> float:
+        """Entanglement entropy across the cut, in nats, of the normalised spectrum p = lambda / Tr rho.  alpha = 1 is
+        the von Neumann entropy -sum p ln p as the device call sums it; other alpha give the Renyi-alpha entropy
+        ln(sum p^alpha) / (1 - alpha) from the spectrum, and alpha = inf the min-entropy -ln max p.  Eigenvalues that
+        rounding left at or below 0 are dropped."""
+        eigs, _, tr, h = self._spectrum(qubits, False)
+        alpha = float(alpha)
+        if alpha == 1.0:
+            return h
+        if tr == 0.0:
+            return 0.0
+        p = eigs[eigs > 0] / tr
+        if np.isinf(alpha):
+            return -float(np.log(p.max()))
+        return float(np.log(np.sum(p ** alpha)) / (1.0 - alpha))
+
     # -- multi-GPU --------------------------------------------------------------
     def ipc_export(self):
         a = (C.c_ubyte * _lib.IPC_HANDLE_BYTES)()
@@ -680,6 +720,18 @@ def purity_plan(n: int, dtype, qubits):
     v = (C.c_uint32 * 4)()
     _lib.check(_lib.lib().qipb200_purity_plan(prec_of(dtype), int(n), _ptr(idx) if len(idx) else None, len(idx), v),
                None)
+    return tuple(int(x) for x in v)
+
+
+def entanglement_spectrum_plan(n: int, dtype, qubits):
+    """(route, s, kernels, device matrix bytes, solver loads) of State.entanglement_spectrum for these qubits on an
+    unsharded n-qubit state (needs no GPU): the routes of purity_plan, with route 2 one Gram kernel that stores G;
+    the last field is 1 when cuSOLVER loads in this process."""
+    idx = np.ascontiguousarray(np.asarray(list(qubits), dtype=np.uint64))
+    v = (C.c_uint32 * 5)()
+    _lib.preload_cusolver()
+    _lib.check(_lib.lib().qipb200_entanglement_spectrum_plan(prec_of(dtype), int(n), _ptr(idx) if len(idx) else None,
+                                                            len(idx), v), None)
     return tuple(int(x) for x in v)
 
 
