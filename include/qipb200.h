@@ -395,6 +395,51 @@ int qipb200_state_apply_pauli_rotations(qipb200_state *state, const uint64_t *qu
  * n-qubit state in canonical layout (0 for n_terms == 0).  Validates the terms as the call above does. */
 int qipb200_pauli_rotation_plan(qip_prec prec, uint32_t n_qubits, const uint64_t *qubits, const char *paulis, const uint32_t *term_len, size_t n_terms, uint32_t *sweeps);
 
+/* One quantum-trajectory step of n_channels single-qubit channels on distinct qubits (absent in the reference): each
+ * channel applies one of its Kraus operators, drawn with its Born probability, and the state is renormalised.
+ * Averaging the states of many trajectories gives the channels' density matrix.  Channel c acts on qubits[c] and has
+ * n_kraus[c] (1..16) operators that follow those of channel c-1 in `kraus`: 2 x 2 complex matrices of 8 doubles each,
+ * row-major, interleaved re/im, rows as outputs, |0> first (the orientation of a qip_op MAT).  Every operator must be
+ * diagonal (K01 = K10 = 0) or anti-diagonal (K00 = K11 = 0), so that K|b> = d(b)|b ^ flip>: amplitude and generalised
+ * amplitude damping, phase damping, bit and phase flips, depolarizing and any Pauli channel, reset, the Z measurement
+ * and their compositions.  A channel is complete when |sum_i |d_i(b)|^2 - 1| <= 1e-12 for b = 0 and 1 (sum K^dagger K
+ * = I), and state-dependent when some operator has |d_i(0)|^2 != |d_i(1)|^2 (damping and reset, not Pauli channels).
+ * draws (HOST, 1 + n_channels uniforms in [0, 1)) and chosen (HOST, n_channels) are arrays of the caller:
+ *   1. x: when some channel is state-dependent, qipb200_state_sample(state, the state-dependent qubits in channel
+ *      order, draws[0]) by the same kernels, so bit-identical (bit k of x <-> the k-th such channel); it assumes a
+ *      unit-norm state and restores a permuted layout first.  Otherwise no sweep runs and draws[0] is unused.
+ *   2. chosen[c] = the smallest i with draws[1 + c] S_b < sum_{i' <= i} e_{i'}, with e_i = re^2 + im^2 of d_i(b) in
+ *      double, S_b = sum_i e_i in Kraus order, b = x_c (0 for a state-independent channel); when rounding leaves no
+ *      such i, the last i with e_i > 0.  The tuple is then drawn with exactly its probability <psi|(x)_c E_i|psi>.
+ *   3. Chosen operators that are positive real multiples of the identity are dropped (they scale psi and p alike):
+ *      when every chosen operator is one, no further kernel runs and the state is unchanged bit for bit.
+ *   4. q: when a remaining operator has |d(0)|^2 != |d(1)|^2, one read sweep computes S = sum_j |psi_j|^2 prod
+ *      |d(bits of j)|^2 and N = sum_j |psi_j|^2 in a fixed order (per-CTA partials added on the host) and q = S / N;
+ *      otherwise q is the product of the remaining operators' uniform weights, on the host.
+ *   5. *prob = q x (the dropped operators' weights): the probability of the tuple for the normalised state.
+ *   6. Unless q == 0 (a zero state, left untouched), one read-write sweep in place on physical bits (a permuted layout
+ *      keeps its qubit map): psi'_{j ^ F} = W(j) psi_j, F the XOR mask of the anti-diagonal choices, with
+ *      W(j) = RN_prec(((T_0[byte_0(j)] T_1[byte_1(j)]) ...) (1/sqrt q)): T_k are 256-entry complex tables of the
+ *      products of d over the channel bits in physical index byte k (bytes without one skipped), built on the host in
+ *      double in ascending bit order, all complex products in double without FMA; then, for (a, b) = psi_j,
+ *      (RN(RN(Wr a) - RN(Wi b)), RN(RN(Wr b) + RN(Wi a))) in the state's precision without FMA.
+ * Errors, all before any device work (a refused call leaves the state and a pending collapse as they were): NULL
+ * state or prob, NULL arrays with n_channels > 0, n_kraus not in 1..16, a non-finite entry, the zero matrix, an
+ * operator neither diagonal nor anti-diagonal, an incomplete channel (the message names the channel and the
+ * operator), and a draw outside [0, 1) give QIPB200_ERR_INVALID_ARG; a qubit >= n or repeated across channels
+ * QIPB200_ERR_BAD_INDEX; sharded and multi-device states QIPB200_ERR_UNSUPPORTED.  n_channels == 0 is a no-op
+ * (*prob = 1).  A pending collapse is applied first and a pending set_basis state written first.  Synchronises (it
+ * returns chosen and prob).  At most three read sweeps (the sample's two, the second only of the chunk its draw
+ * landed in, and the weight) and one read-write sweep; qipb200_channels_plan gives the counts. */
+int qipb200_state_apply_channels(qipb200_state *state, size_t n_channels, const uint64_t *qubits,
+                                 const uint32_t *n_kraus, const double *kraus, const double *draws,
+                                 uint32_t *chosen, double *prob);
+/* Host-only (no GPU, ctx-free): validates as the call does.  out4 = {state-dependent channels, read sweeps at most,
+ * read-write sweeps at most, kernels at most} on an unsharded n-qubit state with nothing pending.  NULL out4, a bad
+ * precision or n_qubits not in 1..40 give QIPB200_ERR_INVALID_ARG. */
+int qipb200_channels_plan(qip_prec prec, uint32_t n_qubits, size_t n_channels, const uint64_t *qubits,
+                          const uint32_t *n_kraus, const double *kraus, uint32_t *out4);
+
 /* Classical functions applied to a register: U |x>|y> = e^{i theta(x)} |x>|y XOR f(x)> for a function given as a table
  * (the row rule of the reference's FunctionOpIterator, qip-iterators/src/iterators/qubit_iterators.rs:221-271, which
  * no MatrixOp reaches): Grover and Shor oracles, modular arithmetic, cost-table phases.

@@ -364,6 +364,21 @@ class B200State {
                                                    letters.empty() ? &no_letter : letters.data(), lens.data(),
                                                    terms.size(), angles.data()));
   }
+  // One quantum-trajectory step of single-qubit channels on distinct qubits: n_kraus[c] operators of 8 doubles each
+  // for channel c (row-major, re/im interleaved), 1 + qubits.size() draws in [0, 1); returns (chosen, prob).
+  std::pair<std::vector<uint32_t>, double> apply_channels(const std::vector<uint64_t> &qubits,
+                                                          const std::vector<uint32_t> &n_kraus,
+                                                          const std::vector<double> &kraus,
+                                                          const std::vector<double> &draws) {
+    if (n_kraus.size() != qubits.size() || draws.size() != qubits.size() + 1)
+      throw CircuitError("apply_channels: " + std::to_string(qubits.size()) + " qubits need as many n_kraus and " +
+                         std::to_string(qubits.size() + 1) + " draws");
+    std::vector<uint32_t> chosen(qubits.size());
+    double p = 0.0;
+    ctx_.check(qipb200_state_apply_channels(st_, qubits.size(), qubits.data(), n_kraus.data(), kraus.data(),
+                                            draws.data(), chosen.data(), &p));
+    return {chosen, p};
+  }
   // psi <- U psi for U|x>|y> = e^{i theta(x)} |x>|y ^ f(x)>: x on in_qubits, y on out_qubits (absent from the
   // reference's MatrixOp)
   void apply_function(const B200Function &fn, const std::vector<uint64_t> &in_qubits,

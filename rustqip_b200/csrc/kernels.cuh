@@ -81,6 +81,7 @@ size_t sample_scratch_bytes(uint32_t n_local, uint64_t n_draws);
 cudaError_t launch_sample(qip_prec prec, const void *psi, uint32_t n_local, const double *d_draws, uint64_t n_draws,
                           const SampleBits &bits, void *d_scratch, uint64_t *d_out, int sm_count, cudaStream_t s,
                           uint64_t *launches);
+const uint32_t kSampleLaunches = 10;  // the kernels one launch_sample launches, whatever n_draws
 // measure (qipb200_state_measure): the outcome m of one draw and its probability p, as one device record.
 // d_draw != nullptr: m is launch_sample's result for that draw; else m must already be in d_rec (a forced outcome)
 // and one read sweep computes the chunk sums.  p is summed in a fixed order from the chunk sums of the chunks whose

@@ -320,6 +320,36 @@ class State:
         args = _pauli_args("apply_pauli_rotations", terms, angles, "angles")
         self._chk(_lib.lib().qipb200_state_apply_pauli_rotations(self._h, *args))
 
+    def apply_channels(self, channels, qubits: Sequence[int], rng=None, draws=None):
+        """One quantum-trajectory step of single-qubit channels on distinct qubits, computed on the device: each
+        channel applies one of its Kraus operators, drawn with its Born probability, and the state is renormalised.
+        Returns (chosen, prob): chosen[c] indexes the operator of channel c, prob is the probability of that tuple.
+
+        ``channels`` is a ``channels.Channel`` for every qubit or one per qubit.  ``draws`` are 1 + len(qubits)
+        uniforms in [0, 1) (draws[0] samples the state-dependent qubits as ``sample`` does, draws[1 + c] picks channel
+        c's operator); without them they are drawn from ``rng`` (a fresh ``np.random.default_rng()`` when None).  At
+        most three read sweeps and one read-write sweep whatever the number of channels (``channels_plan``);
+        synchronises.  Averaging over trajectories reproduces the channels' density matrix."""
+        from . import channels as _ch
+        qa = np.ascontiguousarray(np.asarray(list(qubits), dtype=np.uint64))
+        chans = [channels] * qa.shape[0] if isinstance(channels, _ch.Channel) else list(channels)
+        if len(chans) != qa.shape[0]:
+            raise ValueError("apply_channels: %d channels but %d qubits" % (len(chans), qa.shape[0]))
+        n_kraus, kraus = _ch.marshal(chans)
+        if draws is None:
+            draws = (rng if rng is not None else np.random.default_rng()).random(1 + qa.shape[0])
+        r = np.ascontiguousarray(np.asarray(draws, dtype=np.float64).reshape(-1))
+        if r.shape[0] != 1 + qa.shape[0]:
+            raise ValueError("apply_channels: %d channels need %d draws, got %d" % (qa.shape[0], 1 + qa.shape[0],
+                                                                                   r.shape[0]))
+        chosen = np.zeros(max(1, qa.shape[0]), dtype=np.uint32)
+        prob = C.c_double()
+        n = qa.shape[0]
+        self._chk(_lib.lib().qipb200_state_apply_channels(self._h, n, _ptr(qa) if n else None,
+                                                          _ptr(n_kraus) if n else None, _ptr(kraus) if n else None,
+                                                          _ptr(r), _ptr(chosen), C.byref(prob)))
+        return chosen[:n], float(prob.value)
+
     def apply_function(self, fn: "Function", in_qubits: Sequence[int], out_qubits: Sequence[int] = ()):
         """Apply U|x>|y> = e^{i theta(x)} |x>|y XOR f(x)> of ``fn`` on the device: bit i of x is the value of qubit
         ``in_qubits[i]`` and bit i of f(x) is XORed into qubit ``out_qubits[i]`` (the convention of
@@ -653,6 +683,23 @@ def function_plan(n: int, dtype, in_qubits: Sequence[int], out_qubits: Sequence[
     _lib.check(_lib.lib().qipb200_function_plan(prec_of(dtype), int(n), _ptr(ia) if ia.shape[0] else None,
                                                 ia.shape[0], _ptr(oa) if oa.shape[0] else None, oa.shape[0], v), None)
     return int(v[0]), int(v[1])
+
+
+def channels_plan(n: int, dtype, channels, qubits: Sequence[int]):
+    """(state-dependent channels, read sweeps at most, read-write sweeps at most, kernels at most) of
+    State.apply_channels on an unsharded n-qubit state with nothing pending (needs no GPU); validates as the call
+    does."""
+    from . import channels as _ch
+    qa = np.ascontiguousarray(np.asarray(list(qubits), dtype=np.uint64))
+    chans = [channels] * qa.shape[0] if isinstance(channels, _ch.Channel) else list(channels)
+    if len(chans) != qa.shape[0]:
+        raise ValueError("channels_plan: %d channels but %d qubits" % (len(chans), qa.shape[0]))
+    n_kraus, kraus = _ch.marshal(chans)
+    v = (C.c_uint32 * 4)()
+    k = qa.shape[0]
+    _lib.check(_lib.lib().qipb200_channels_plan(prec_of(dtype), int(n), k, _ptr(qa) if k else None,
+                                                _ptr(n_kraus) if k else None, _ptr(kraus) if k else None, v), None)
+    return tuple(int(x) for x in v)
 
 
 def validate_op(op: MatrixOp, n: int, dtype=np.complex128):
