@@ -440,6 +440,44 @@ int qipb200_state_apply_channels(qipb200_state *state, size_t n_channels, const 
 int qipb200_channels_plan(qip_prec prec, uint32_t n_qubits, size_t n_channels, const uint64_t *qubits,
                           const uint32_t *n_kraus, const double *kraus, uint32_t *out4);
 
+/* qipb200_state_apply_channels for channels on k = 1..4 qubits each (absent in the reference): two-qubit depolarizing
+ * and any multi-qubit Pauli channel, correlated dephasing, tensor products of the single-qubit channels above, a
+ * multi-qubit reset or Z measurement.  Channel c acts on the arity[c] qubits that follow those of channel c-1 in
+ * `qubits` (no qubit twice in the layer) and has n_kraus[c] (1..256) operators that follow those of channel c-1 in
+ * `kraus`: 2^k x 2^k complex matrices of 2 4^k doubles each, row-major, interleaved re/im, rows as outputs, in the
+ * qip_op MAT sub-index convention: the channel's first qubit is the most significant bit of the row and column index
+ * (for k = 1 exactly the input of qipb200_state_apply_channels).  Every operator must have the form K|b> = d(b)|b ^ f>:
+ * every column at most one nonzero entry, at row b ^ f for one f shared by all nonzero columns (whole zero columns are
+ * allowed: the reset |00><b| is one operator per b), and not the zero matrix.  Complete: |sum_i |d_i(b)|^2 - 1| <= 1e-12
+ * for every b in 0..2^k-1; state-dependent: some operator's |d_i(b)|^2 depends on b.  draws, chosen and prob, and the
+ * six steps, are those of qipb200_state_apply_channels with these changes:
+ *   1. x samples the qubits of the state-dependent channels in channel order and, within a channel, in its qubit order:
+ *      bit i of x is the i-th qubit so listed (the measure_probs convention).  The channel value b_c is the channel's
+ *      bits of x in the matrix convention, so the two run in opposite directions: for a channel whose qubits sit at
+ *      bits s .. s+k-1 of x, b_c = sum_i ((x >> (s + i)) & 1) << (k - 1 - i).
+ *   3. A dropped operator has f = 0 and the same positive real d(b) for every b.
+ *   4. w(j) = prod_c |d_c(b_c(j))|^2 over the remaining operators, b_c(j) the channel's bits of physical index j.
+ *   6. F is the XOR of the chosen masks on their physical bits, and W(j) = RN_prec(((T_0[i_0(j)] T_1[i_1(j)]) ...)
+ *      (1/sqrt q)) with two kinds of table: an operator whose physical bits all lie in one index byte folds into that
+ *      byte's 256-entry table (its factors multiplied in the order of their lowest physical bit, so a layer of
+ *      single-qubit channels gives the tables of qipb200_state_apply_channels), bytes ascending; every other operator
+ *      has a table of its 2^k values d(b), indexed by its physical bits gathered in the matrix convention, in channel
+ *      order after the byte tables.
+ * A layer of single-qubit channels gives the same chosen, prob and state, bit for bit, as qipb200_state_apply_channels.
+ * Errors, all before any device work (a refused call leaves the state and a pending collapse as they were): NULL state
+ * or prob, NULL arrays with n_channels > 0, an arity not in 1..4, n_kraus not in 1..256, a non-finite entry, the zero
+ * matrix, an operator not of the form above (the message names the channel and the operator), an incomplete channel
+ * (it names the channel and b) and a draw outside [0, 1) give QIPB200_ERR_INVALID_ARG; a qubit >= n or repeated
+ * anywhere in the layer QIPB200_ERR_BAD_INDEX; sharded and multi-device states QIPB200_ERR_UNSUPPORTED.  Sweeps as for
+ * qipb200_state_apply_channels; qipb200_multiqubit_channels_plan gives the counts. */
+int qipb200_state_apply_multiqubit_channels(qipb200_state *state, size_t n_channels, const uint32_t *arity,
+                                            const uint64_t *qubits, const uint32_t *n_kraus, const double *kraus,
+                                            const double *draws, uint32_t *chosen, double *prob);
+/* Host-only (no GPU, ctx-free): validates as the call does; out4 as for qipb200_channels_plan. */
+int qipb200_multiqubit_channels_plan(qip_prec prec, uint32_t n_qubits, size_t n_channels, const uint32_t *arity,
+                                     const uint64_t *qubits, const uint32_t *n_kraus, const double *kraus,
+                                     uint32_t *out4);
+
 /* Classical functions applied to a register: U |x>|y> = e^{i theta(x)} |x>|y XOR f(x)> for a function given as a table
  * (the row rule of the reference's FunctionOpIterator, qip-iterators/src/iterators/qubit_iterators.rs:221-271, which
  * no MatrixOp reaches): Grover and Shor oracles, modular arithmetic, cost-table phases.

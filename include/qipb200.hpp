@@ -379,6 +379,22 @@ class B200State {
                                             draws.data(), chosen.data(), &p));
     return {chosen, p};
   }
+  // The same for channels on 1..4 qubits each: channel c acts on the arity[c] qubits that follow channel c-1's in
+  // `qubits` and has n_kraus[c] operators of 2 * 4^arity[c] doubles each; returns (chosen, prob).
+  std::pair<std::vector<uint32_t>, double> apply_multiqubit_channels(const std::vector<uint32_t> &arity,
+                                                                     const std::vector<uint64_t> &qubits,
+                                                                     const std::vector<uint32_t> &n_kraus,
+                                                                     const std::vector<double> &kraus,
+                                                                     const std::vector<double> &draws) {
+    if (n_kraus.size() != arity.size() || draws.size() != arity.size() + 1)
+      throw CircuitError("apply_multiqubit_channels: " + std::to_string(arity.size()) +
+                         " channels need as many n_kraus and " + std::to_string(arity.size() + 1) + " draws");
+    std::vector<uint32_t> chosen(arity.size());
+    double p = 0.0;
+    ctx_.check(qipb200_state_apply_multiqubit_channels(st_, arity.size(), arity.data(), qubits.data(), n_kraus.data(),
+                                                       kraus.data(), draws.data(), chosen.data(), &p));
+    return {chosen, p};
+  }
   // psi <- U psi for U|x>|y> = e^{i theta(x)} |x>|y ^ f(x)>: x on in_qubits, y on out_qubits (absent from the
   // reference's MatrixOp)
   void apply_function(const B200Function &fn, const std::vector<uint64_t> &in_qubits,

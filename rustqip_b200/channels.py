@@ -1,51 +1,80 @@
-"""Single-qubit noise channels for quantum-trajectory simulation (State.apply_channels).
+"""Noise channels on one to four qubits for quantum-trajectory simulation (State.apply_channels,
+State.apply_multiqubit_channels).
 
-A ``Channel`` holds Kraus operators K_i that are each diagonal or anti-diagonal, K|b> = d(b)|b ^ flip>, and complete
-(sum_i K_i^dagger K_i = I to 1e-12).  That covers amplitude and phase damping, Pauli channels, reset, the Z measurement
-and their compositions, and lets a layer of such channels be drawn jointly with one sample of the state
-(include/qipb200.h: qipb200_state_apply_channels)."""
+A ``Channel`` on k qubits holds Kraus operators K_i of the form K|b> = d(b)|b ^ f>, one XOR mask f per operator (every
+column has at most one nonzero entry, on the same shifted diagonal; for k = 1 that is diagonal or anti-diagonal), and
+is complete (sum_i K_i^dagger K_i = I to 1e-12).  That covers amplitude and phase damping, every Pauli channel (the two-
+qubit depolarizing channel included), reset, the Z measurement, and their compositions and tensor products, and lets a
+layer of such channels be drawn jointly with one sample of the state (include/qipb200.h:
+qipb200_state_apply_channels, qipb200_state_apply_multiqubit_channels).  Matrices use the qip_op MAT convention: rows
+as outputs, the channel's first qubit the most significant bit of the index."""
 from __future__ import annotations
 
-from typing import Sequence
+import itertools
+from typing import Mapping, Sequence
 
 import numpy as np
 
-MAX_KRAUS = 16
+MAX_KRAUS = 16          # operators of a single-qubit channel (qipb200_state_apply_channels)
+MAX_KRAUS_MULTI = 256   # operators of a channel on 2 to 4 qubits
+MAX_QUBITS = 4
 COMPLETE_TOL = 1e-12
 
 _I = np.eye(2, dtype=np.complex128)
 _X = np.array([[0, 1], [1, 0]], dtype=np.complex128)
 _Y = np.array([[0, -1j], [1j, 0]], dtype=np.complex128)
 _Z = np.array([[1, 0], [0, -1]], dtype=np.complex128)
+_PAULI = {"I": _I, "X": _X, "Y": _Y, "Z": _Z}
+
+
+def _form(k):
+    """(f, d) with K|b> = d[b] |b ^ f>, or None when K is not of that form (or is zero)."""
+    D = k.shape[0]
+    f = None
+    for c in range(D):
+        for r in np.flatnonzero(k[:, c] != 0):
+            if f is None:
+                f = int(r) ^ c
+            elif int(r) ^ c != f:
+                return None
+    if f is None:
+        return None
+    return f, [k[b ^ f, b] for b in range(D)]
 
 
 def _weights(k):
-    """|d(0)|^2, |d(1)|^2 of a monomial operator, in double as the library computes them (re^2 + im^2)."""
-    flip = k[0, 0] == 0 and k[1, 1] == 0
-    d = (k[1, 0], k[0, 1]) if flip else (k[0, 0], k[1, 1])
-    return [float(np.float64(v.real) * np.float64(v.real) + np.float64(v.imag) * np.float64(v.imag)) for v in d]
+    """|d(b)|^2 for every b of a monomial operator, in double as the library computes them (re^2 + im^2)."""
+    return [float(np.float64(v.real) * np.float64(v.real) + np.float64(v.imag) * np.float64(v.imag))
+            for v in _form(k)[1]]
 
 
 class Channel:
-    """A single-qubit channel given by its Kraus operators (a sequence of 2 x 2 complex matrices, rows as outputs,
-    |0> first).  Raises ValueError unless every operator is finite, nonzero, diagonal or anti-diagonal, there are 1
-    to 16 of them, and sum_i |d_i(b)|^2 is 1 within 1e-12 for b = 0 and 1: the checks the library makes."""
+    """A channel on k = 1..4 qubits given by its Kraus operators (a sequence of 2^k x 2^k complex matrices, rows as
+    outputs, the first qubit the most significant index bit).  Raises ValueError unless every operator is finite,
+    nonzero and of the form K|b> = d(b)|b ^ f>, there are 1 to 16 of them (one qubit) or 1 to 256 (two to four), and
+    sum_i |d_i(b)|^2 is 1 within 1e-12 for every b: the checks the library makes."""
 
     def __init__(self, kraus):
-        ks = np.array([np.asarray(k, dtype=np.complex128) for k in kraus], dtype=np.complex128).reshape(-1, 2, 2)
-        if not 1 <= ks.shape[0] <= MAX_KRAUS:
-            raise ValueError("Channel: 1 to 16 Kraus operators, got %d" % ks.shape[0])
-        total = [0.0, 0.0]
+        mats = [np.asarray(k, dtype=np.complex128) for k in kraus]
+        D = mats[0].shape[-1] if mats else 2
+        if D not in (2, 4, 8, 16):
+            raise ValueError("Channel: operators must be 2^k x 2^k for k = 1..4, got %r" % (mats[0].shape,))
+        ks = np.array(mats, dtype=np.complex128).reshape(-1, D, D)
+        nq = D.bit_length() - 1
+        top = MAX_KRAUS if nq == 1 else MAX_KRAUS_MULTI
+        if not 1 <= ks.shape[0] <= top:
+            raise ValueError("Channel: 1 to %d Kraus operators, got %d" % (top, ks.shape[0]))
+        total = [0.0] * D
         for i, k in enumerate(ks):
             if not np.all(np.isfinite(k.view(np.float64))):
                 raise ValueError("Channel: operator %d has a non-finite entry" % i)
             if not np.any(k != 0):
                 raise ValueError("Channel: operator %d is the zero matrix" % i)
-            if not ((k[0, 1] == 0 and k[1, 0] == 0) or (k[0, 0] == 0 and k[1, 1] == 0)):
-                raise ValueError("Channel: operator %d is neither diagonal nor anti-diagonal" % i)
-            e = _weights(k)
-            total = [total[0] + e[0], total[1] + e[1]]
-        for b in (0, 1):
+            if _form(k) is None:
+                raise ValueError("Channel: operator %d is %s" % (i, "neither diagonal nor anti-diagonal" if nq == 1
+                                                                  else "not of the form d(b)|b ^ f>"))
+            total = [t + e for t, e in zip(total, _weights(k))]
+        for b in range(D):
             if not abs(total[b] - 1.0) <= COMPLETE_TOL:
                 raise ValueError("Channel: the operators are not complete (sum of |d_i(%d)|^2 - 1 = %.3g)"
                                  % (b, total[b] - 1.0))
@@ -55,22 +84,36 @@ class Channel:
         return self.kraus.shape[0]
 
     def __repr__(self):
-        return "Channel(%d Kraus operators)" % len(self)
+        return "Channel(%d qubits, %d Kraus operators)" % (self.n_qubits, len(self)) if self.n_qubits > 1 else \
+            "Channel(%d Kraus operators)" % len(self)
+
+    @property
+    def n_qubits(self) -> int:
+        return self.kraus.shape[1].bit_length() - 1
 
     @property
     def state_dependent(self) -> bool:
-        """Some operator has |d(0)|^2 != |d(1)|^2: the choice depends on the qubit's value (damping, reset)."""
-        return any(e[0] != e[1] for e in map(_weights, self.kraus))
+        """Some operator's |d(b)|^2 depends on b: the choice depends on the qubits' values (damping, reset)."""
+        return any(len(set(e)) > 1 for e in map(_weights, self.kraus))
 
     def compose(self, other: "Channel") -> "Channel":
-        """This channel, then ``other``: the Kraus operators B_j A_i (j major), zero products left out.  Products of
-        diagonal or anti-diagonal matrices are again one or the other, so e.g. T1/T2 relaxation is
+        """This channel, then ``other`` on the same qubits: the Kraus operators B_j A_i (j major), zero products left
+        out.  Products of operators of this form are again of this form, so e.g. T1/T2 relaxation is
         ``amplitude_damping(g).compose(phase_damping(l))``."""
+        if other.n_qubits != self.n_qubits:
+            raise ValueError("compose: channels on %d and %d qubits" % (self.n_qubits, other.n_qubits))
         ks = [b @ a for b in other.kraus for a in self.kraus]
         return Channel([k for k in ks if np.any(k != 0)])
 
+    def tensor(self, other: "Channel") -> "Channel":
+        """This channel on the first qubits and ``other`` on the ones after them: the Kraus operators A_i (x) B_j
+        (i major), on at most four qubits in all."""
+        if self.n_qubits + other.n_qubits > MAX_QUBITS:
+            raise ValueError("tensor: %d + %d qubits, at most 4" % (self.n_qubits, other.n_qubits))
+        return Channel([np.kron(a, b) for a in self.kraus for b in other.kraus])
+
     def superop(self, rho: np.ndarray) -> np.ndarray:
-        """sum_i K_i rho K_i^dagger on a 2 x 2 density matrix (for checks)."""
+        """sum_i K_i rho K_i^dagger on a 2^k x 2^k density matrix (for checks)."""
         return sum(k @ rho @ k.conj().T for k in self.kraus)
 
 
@@ -115,9 +158,36 @@ def reset() -> Channel:
     return Channel([np.diag([1.0, 0.0]), np.array([[0, 1], [0, 0]])])
 
 
+def pauli_string_channel(probs: Mapping[str, float]) -> Channel:
+    """A Pauli channel on k qubits: each Pauli string (e.g. ``"XZ"``: X on the first qubit, Z on the second) with its
+    probability, the identity with the rest.  Strings are non-identity, distinct and all of one length k = 1..4."""
+    probs = {str(s).upper(): float(p) for s, p in probs.items()}
+    ks = {len(s) for s in probs}
+    if len(ks) != 1 or not 1 <= next(iter(ks)) <= MAX_QUBITS:
+        raise ValueError("pauli_string_channel: strings of one length 1..4, got %r" % sorted(probs))
+    k = next(iter(ks))
+    for s in probs:
+        if set(s) - set("IXYZ") or s == "I" * k:
+            raise ValueError("pauli_string_channel: %r is not a non-identity Pauli string" % s)
+    def op(s):
+        m = np.ones((1, 1), dtype=np.complex128)
+        for c in s:
+            m = np.kron(m, _PAULI[c])
+        return m
+    rest = 1.0 - sum(probs.values())
+    return _keep([np.sqrt(rest) * op("I" * k)] + [np.sqrt(p) * op(s) for s, p in probs.items()])
+
+
+def two_qubit_depolarizing(p: float) -> Channel:
+    """rho -> (1 - p) rho + p/15 sum_{P != II} P rho P: each of the 15 two-qubit Pauli errors with probability p/15."""
+    p = float(p)
+    return pauli_string_channel({a + b: p / 15 for a, b in itertools.product("IXYZ", repeat=2) if a + b != "II"})
+
+
 def marshal(channels: Sequence[Channel]):
-    """(n_kraus u32, kraus f64) arrays of the C ABI."""
+    """(arity u32, n_kraus u32, kraus f64) arrays of the C ABI."""
+    arity = np.ascontiguousarray([c.n_qubits for c in channels], dtype=np.uint32)
     n_kraus = np.ascontiguousarray([len(c) for c in channels], dtype=np.uint32)
     kraus = np.ascontiguousarray(np.concatenate([c.kraus.reshape(-1) for c in channels]) if channels else
                                  np.zeros(0, dtype=np.complex128)).view(np.float64)
-    return n_kraus, np.ascontiguousarray(kraus)
+    return arity, n_kraus, np.ascontiguousarray(kraus)

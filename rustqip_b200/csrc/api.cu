@@ -2429,20 +2429,23 @@ extern "C" int qipb200_pauli_rotation_plan(qip_prec prec, uint32_t n_qubits, con
 }
 
 // ===================================================================================
-// single-qubit noise channels along quantum trajectories (channel.cu)
+// noise channels along quantum trajectories (channel.cu)
 // ===================================================================================
 
 namespace {
 
 int parse_channel_list(const qipb200_ctx *ctx, const std::string &who, uint32_t n, size_t n_channels,
-                       const uint64_t *qubits, const uint32_t *n_kraus, const double *kraus, ChannelSet *cs) {
+                       const uint32_t *arity, const uint64_t *qubits, const uint32_t *n_kraus, const double *kraus,
+                       ChannelSet *cs) {
   std::string err;
-  const int st = parse_channels(who, n, n_channels, qubits, n_kraus, kraus, cs, &err);
+  const uint32_t max_kraus = arity ? kChanMaxKrausMulti : kChanMaxKraus;
+  const int st = parse_channels(who, n, n_channels, arity, qubits, n_kraus, kraus, max_kraus, cs, &err);
   return st == QIPB200_OK ? st : set_err(ctx, st, err);
 }
 
-// x over the state-dependent channels' qubits in channel order: qipb200_state_sample's kernels with draws[0].
-int channels_sample(qipb200_state *s, const ChannelSet &cs, double draw, uint64_t *x) {
+// x over the state-dependent channels' qubits in channel order, each channel's in its qubit order:
+// qipb200_state_sample's kernels with draws[0].
+int channels_sample(qipb200_state *s, const std::string &who, const ChannelSet &cs, double draw, uint64_t *x) {
   qipb200_ctx *ctx = s->ctx;
   if (!layout_is_identity(s)) {  // the scan runs over canonical indices
     int st = restore_layout(s);
@@ -2450,8 +2453,9 @@ int channels_sample(qipb200_state *s, const ChannelSet &cs, double draw, uint64_
   }
   SampleBits bits;
   bits.n_bits = 0;
-  for (size_t c = 0; c < cs.qubits.size(); ++c)
-    if (cs.dep[c]) bits.bitpos[bits.n_bits++] = s->n - 1 - (uint32_t)cs.qubits[c];
+  for (size_t c = 0; c < cs.size(); ++c)
+    for (uint32_t i = cs.qfirst[c]; cs.dep[c] && i < cs.qfirst[c + 1]; ++i)
+      bits.bitpos[bits.n_bits++] = s->n - 1 - (uint32_t)cs.qubits[i];
   char *d = nullptr;
   CU(ctx, cudaMallocAsync((void **)&d, 16 + sample_scratch_bytes(s->n_local, 1), ctx->stream));
   cudaError_t e = cudaMemcpyAsync(d, &draw, sizeof(draw), cudaMemcpyHostToDevice, ctx->stream);
@@ -2460,26 +2464,30 @@ int channels_sample(qipb200_state *s, const ChannelSet &cs, double draw, uint64_
                       ctx->sm_count, ctx->stream, &ctx->launches);
   if (e == cudaSuccess) e = cudaMemcpyAsync(x, d + 8, sizeof(*x), cudaMemcpyDeviceToHost, ctx->stream);
   cudaError_t ef = cudaFreeAsync(d, ctx->stream);
-  if (e != cudaSuccess) return cuda_fail(ctx, e, "apply_channels: sample");
+  if (e != cudaSuccess) return cuda_fail(ctx, e, (who + ": sample").c_str());
   CU(ctx, ef);
   CU(ctx, cudaStreamSynchronize(ctx->stream));
   return QIPB200_OK;
 }
 
-int channels_impl(qipb200_state *s, const ChannelSet &cs, const double *draws, uint32_t *chosen, double *prob) {
+int channels_impl(qipb200_state *s, const std::string &who, const ChannelSet &cs, const double *draws,
+                  uint32_t *chosen, double *prob) {
   qipb200_ctx *ctx = s->ctx;
   int st = begin_device_work(s);
   if (st != QIPB200_OK) return st;
   uint64_t x = 0;
-  if (cs.n_dep && (st = channels_sample(s, cs, draws[0], &x)) != QIPB200_OK) return st;
+  if (cs.n_dep && (st = channels_sample(s, who, cs, draws[0], &x)) != QIPB200_OK) return st;
   // the choices, then the chosen operators that are not positive multiples of the identity
   std::vector<const ChannelOp *> rest;
   std::vector<uint64_t> rest_q;
   double dropped = 1.0, uniform = 1.0;
   bool nonuniform = false;
-  uint32_t k_dep = 0;
-  for (size_t c = 0; c < cs.qubits.size(); ++c) {
-    const uint32_t b = cs.dep[c] ? (uint32_t)((x >> k_dep++) & 1) : 0u;
+  uint32_t k_dep = 0;  // the bit of x of the next state-dependent channel's first qubit
+  for (size_t c = 0; c < cs.size(); ++c) {
+    const uint32_t k = cs.qfirst[c + 1] - cs.qfirst[c];
+    uint32_t b = 0;  // x's bits of the channel in the matrix convention: its first qubit the most significant
+    for (uint32_t i = 0; cs.dep[c] && i < k; ++i) b = (b << 1) | (uint32_t)((x >> (k_dep + i)) & 1);
+    k_dep += cs.dep[c] ? k : 0;
     chosen[c] = channel_choose(cs, c, b, draws[1 + c]);
     const ChannelOp &K = cs.ops[cs.first[c] + chosen[c]];
     if (channel_op_is_scaled_identity(K)) {
@@ -2487,8 +2495,10 @@ int channels_impl(qipb200_state *s, const ChannelSet &cs, const double *draws, u
       continue;
     }
     rest.push_back(&K);
-    rest_q.push_back(cs.qubits[c]);
-    if (K.e[0] != K.e[1])
+    rest_q.insert(rest_q.end(), cs.qubits.begin() + cs.qfirst[c], cs.qubits.begin() + cs.qfirst[c + 1]);
+    bool flat = true;
+    for (uint32_t v = 1; v < (1u << k); ++v) flat = flat && K.e[v] == K.e[0];
+    if (!flat)
       nonuniform = true;
     else
       uniform *= K.e[0];
@@ -2499,8 +2509,8 @@ int channels_impl(qipb200_state *s, const ChannelSet &cs, const double *draws, u
     return QIPB200_OK;
   }
   // A permuted layout (QIPB200_ROTATE, no state-dependent channel) is worked on where it is.
-  std::vector<uint32_t> pos(rest.size());
-  phys_positions(s, rest_q.data(), (uint32_t)rest.size(), pos.data());
+  std::vector<uint32_t> pos(rest_q.size());
+  phys_positions(s, rest_q.data(), (uint32_t)rest_q.size(), pos.data());
   ChannelTables t;
   build_channel_tables(pos.data(), rest.data(), rest.size(), &t);
   char *d = nullptr;
@@ -2516,7 +2526,7 @@ int channels_impl(qipb200_state *s, const ChannelSet &cs, const double *draws, u
     e = run_channel_apply(s->prec, s->buf, s->n_local, t, 1.0 / std::sqrt(q), d, ctx->sm_count, ctx->stream,
                           &ctx->launches);
   cudaError_t ef = cudaFreeAsync(d, ctx->stream);
-  if (e != cudaSuccess) return cuda_fail(ctx, e, "apply_channels");
+  if (e != cudaSuccess) return cuda_fail(ctx, e, who.c_str());
   CU(ctx, ef);
   CU(ctx, cudaStreamSynchronize(ctx->stream));
   *prob = q * dropped;
@@ -2536,7 +2546,7 @@ extern "C" int qipb200_state_apply_channels(qipb200_state *s, size_t n_channels,
     if (n_channels && (!draws || !chosen))
       return set_err(s->ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL draws or chosen");
     ChannelSet cs;
-    int st = parse_channel_list(s->ctx, who, s->n, n_channels, qubits, n_kraus, kraus, &cs);
+    int st = parse_channel_list(s->ctx, who, s->n, n_channels, nullptr, qubits, n_kraus, kraus, &cs);
     if (st != QIPB200_OK) return st;
     for (size_t k = 0; n_channels && k <= n_channels; ++k)
       if (!(draws[k] >= 0.0 && draws[k] < 1.0))
@@ -2546,7 +2556,7 @@ extern "C" int qipb200_state_apply_channels(qipb200_state *s, size_t n_channels,
       *prob = 1.0;
       return (int)QIPB200_OK;
     }
-    return channels_impl(s, cs, draws, chosen, prob);
+    return channels_impl(s, who, cs, draws, chosen, prob);
   });
 }
 
@@ -2556,7 +2566,53 @@ extern "C" int qipb200_channels_plan(qip_prec prec, uint32_t n_qubits, size_t n_
   return guarded(nullptr, [&]() -> int {
     ChannelSet cs;
     int st = check_plan_args(who, prec, n_qubits, out4, "out4");
-    if (st == QIPB200_OK) st = parse_channel_list(nullptr, who, n_qubits, n_channels, qubits, n_kraus, kraus, &cs);
+    if (st == QIPB200_OK)
+      st = parse_channel_list(nullptr, who, n_qubits, n_channels, nullptr, qubits, n_kraus, kraus, &cs);
+    if (st != QIPB200_OK) return st;
+    plan_channels(cs, out4);
+    return (int)QIPB200_OK;
+  });
+}
+
+extern "C" int qipb200_state_apply_multiqubit_channels(qipb200_state *s, size_t n_channels, const uint32_t *arity,
+                                                       const uint64_t *qubits, const uint32_t *n_kraus,
+                                                       const double *kraus, const double *draws, uint32_t *chosen,
+                                                       double *prob) {
+  const std::string who = "apply_multiqubit_channels";
+  if (!s) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, who + ": NULL state");
+  return guarded(s->ctx, [&]() -> int {
+    // every check runs before any device work: a refused call leaves the state (and a pending collapse) as it was
+    if (!prob) return set_err(s->ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL prob");
+    if (n_channels && (!draws || !chosen))
+      return set_err(s->ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL draws or chosen");
+    if (n_channels && !arity)
+      return set_err(s->ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL arity, qubits, n_kraus or kraus");
+    ChannelSet cs;
+    int st = parse_channel_list(s->ctx, who, s->n, n_channels, arity, qubits, n_kraus, kraus, &cs);
+    if (st != QIPB200_OK) return st;
+    for (size_t k = 0; n_channels && k <= n_channels; ++k)
+      if (!(draws[k] >= 0.0 && draws[k] < 1.0))
+        return set_err(s->ctx, QIPB200_ERR_INVALID_ARG, who + ": draw " + std::to_string(k) + " is not in [0, 1)");
+    if ((st = require_unsharded(s, who)) != QIPB200_OK) return st;
+    if (n_channels == 0) {
+      *prob = 1.0;
+      return (int)QIPB200_OK;
+    }
+    return channels_impl(s, who, cs, draws, chosen, prob);
+  });
+}
+
+extern "C" int qipb200_multiqubit_channels_plan(qip_prec prec, uint32_t n_qubits, size_t n_channels,
+                                                const uint32_t *arity, const uint64_t *qubits,
+                                                const uint32_t *n_kraus, const double *kraus, uint32_t *out4) {
+  const std::string who = "multiqubit_channels_plan";
+  return guarded(nullptr, [&]() -> int {
+    ChannelSet cs;
+    int st = check_plan_args(who, prec, n_qubits, out4, "out4");
+    if (st == QIPB200_OK && n_channels && !arity)
+      st = set_err(nullptr, QIPB200_ERR_INVALID_ARG, who + ": NULL arity, qubits, n_kraus or kraus");
+    if (st == QIPB200_OK)
+      st = parse_channel_list(nullptr, who, n_qubits, n_channels, arity, qubits, n_kraus, kraus, &cs);
     if (st != QIPB200_OK) return st;
     plan_channels(cs, out4);
     return (int)QIPB200_OK;

@@ -335,7 +335,8 @@ class State:
         chans = [channels] * qa.shape[0] if isinstance(channels, _ch.Channel) else list(channels)
         if len(chans) != qa.shape[0]:
             raise ValueError("apply_channels: %d channels but %d qubits" % (len(chans), qa.shape[0]))
-        n_kraus, kraus = _ch.marshal(chans)
+        _single_qubit("apply_channels", chans, "apply_multiqubit_channels")
+        _, n_kraus, kraus = _ch.marshal(chans)
         if draws is None:
             draws = (rng if rng is not None else np.random.default_rng()).random(1 + qa.shape[0])
         r = np.ascontiguousarray(np.asarray(draws, dtype=np.float64).reshape(-1))
@@ -349,6 +350,31 @@ class State:
                                                           _ptr(n_kraus) if n else None, _ptr(kraus) if n else None,
                                                           _ptr(r), _ptr(chosen), C.byref(prob)))
         return chosen[:n], float(prob.value)
+
+    def apply_multiqubit_channels(self, channels, qubit_groups, rng=None, draws=None):
+        """One quantum-trajectory step of channels on one to four qubits each, no qubit twice in the layer, computed
+        on the device as ``apply_channels`` does.  Returns (chosen, prob).
+
+        ``qubit_groups[c]`` lists the qubits of channel c, its first qubit the most significant bit of the channel's
+        matrices; ``channels`` is one ``channels.Channel`` for every group or one per group, each on as many qubits as
+        its group.  ``draws`` are 1 + len(qubit_groups) uniforms in [0, 1) (draws[0] samples the state-dependent
+        channels' qubits, draws[1 + c] picks channel c's operator); without them they are drawn from ``rng``.  At most
+        three read sweeps and one read-write sweep whatever the layer (``multiqubit_channels_plan``); synchronises.
+        A layer of single-qubit channels gives the same bits as ``apply_channels``."""
+        chans, qa = _channel_groups("apply_multiqubit_channels", channels, qubit_groups)
+        arity, n_kraus, kraus = _ch_marshal(chans)
+        nc = len(chans)
+        if draws is None:
+            draws = (rng if rng is not None else np.random.default_rng()).random(1 + nc)
+        r = np.ascontiguousarray(np.asarray(draws, dtype=np.float64).reshape(-1))
+        if r.shape[0] != 1 + nc:
+            raise ValueError("apply_multiqubit_channels: %d channels need %d draws, got %d" % (nc, 1 + nc, r.shape[0]))
+        chosen = np.zeros(max(1, nc), dtype=np.uint32)
+        prob = C.c_double()
+        self._chk(_lib.lib().qipb200_state_apply_multiqubit_channels(
+            self._h, nc, _ptr(arity) if nc else None, _ptr(qa) if nc else None, _ptr(n_kraus) if nc else None,
+            _ptr(kraus) if nc else None, _ptr(r), _ptr(chosen), C.byref(prob)))
+        return chosen[:nc], float(prob.value)
 
     def apply_function(self, fn: "Function", in_qubits: Sequence[int], out_qubits: Sequence[int] = ()):
         """Apply U|x>|y> = e^{i theta(x)} |x>|y XOR f(x)> of ``fn`` on the device: bit i of x is the value of qubit
@@ -694,11 +720,51 @@ def channels_plan(n: int, dtype, channels, qubits: Sequence[int]):
     chans = [channels] * qa.shape[0] if isinstance(channels, _ch.Channel) else list(channels)
     if len(chans) != qa.shape[0]:
         raise ValueError("channels_plan: %d channels but %d qubits" % (len(chans), qa.shape[0]))
-    n_kraus, kraus = _ch.marshal(chans)
+    _single_qubit("channels_plan", chans, "multiqubit_channels_plan")
+    _, n_kraus, kraus = _ch.marshal(chans)
     v = (C.c_uint32 * 4)()
     k = qa.shape[0]
     _lib.check(_lib.lib().qipb200_channels_plan(prec_of(dtype), int(n), k, _ptr(qa) if k else None,
                                                 _ptr(n_kraus) if k else None, _ptr(kraus) if k else None, v), None)
+    return tuple(int(x) for x in v)
+
+
+def _ch_marshal(chans):
+    from . import channels as _ch
+    return _ch.marshal(chans)
+
+
+def _single_qubit(who, chans, instead):
+    for c, chan in enumerate(chans):
+        if chan.n_qubits != 1:
+            raise ValueError("%s: channel %d acts on %d qubits; use %s" % (who, c, chan.n_qubits, instead))
+
+
+def _channel_groups(who, channels, qubit_groups):
+    """(channels, flat uint64 qubits) of a multi-qubit layer; one Channel stands for every group."""
+    from . import channels as _ch
+    groups = [[int(q) for q in g] for g in qubit_groups]
+    chans = [channels] * len(groups) if isinstance(channels, _ch.Channel) else list(channels)
+    if len(chans) != len(groups):
+        raise ValueError("%s: %d channels but %d qubit groups" % (who, len(chans), len(groups)))
+    for c, (chan, g) in enumerate(zip(chans, groups)):
+        if chan.n_qubits != len(g):
+            raise ValueError("%s: channel %d acts on %d qubits but its group has %d" % (who, c, chan.n_qubits, len(g)))
+    qa = np.ascontiguousarray(np.asarray([q for g in groups for q in g], dtype=np.uint64))
+    return chans, qa
+
+
+def multiqubit_channels_plan(n: int, dtype, channels, qubit_groups):
+    """(state-dependent channels, read sweeps at most, read-write sweeps at most, kernels at most) of
+    State.apply_multiqubit_channels on an unsharded n-qubit state with nothing pending (needs no GPU); validates as
+    the call does."""
+    chans, qa = _channel_groups("multiqubit_channels_plan", channels, qubit_groups)
+    arity, n_kraus, kraus = _ch_marshal(chans)
+    v = (C.c_uint32 * 4)()
+    k = len(chans)
+    _lib.check(_lib.lib().qipb200_multiqubit_channels_plan(
+        prec_of(dtype), int(n), k, _ptr(arity) if k else None, _ptr(qa) if k else None,
+        _ptr(n_kraus) if k else None, _ptr(kraus) if k else None, v), None)
     return tuple(int(x) for x in v)
 
 
