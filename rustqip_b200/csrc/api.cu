@@ -252,11 +252,6 @@ extern "C" void qipb200_shutdown(qipb200_ctx *ctx) {
   for (size_t i = 0; i < ctx->prof_pool.size(); ++i) cudaEventDestroy(ctx->prof_pool[i]);
   jit_unload(&ctx->jit_loaded);
   eig_handle_destroy(ctx->eig_solver);
-  for (int i = 0; i < 2; ++i) {
-    if (ctx->ev_pass[i]) cudaEventDestroy(ctx->ev_pass[i]);
-    if (ctx->ev_exch[i]) cudaEventDestroy(ctx->ev_exch[i]);
-  }
-  if (ctx->stream2) cudaStreamDestroy(ctx->stream2);
   if (ctx->stream) cudaStreamDestroy(ctx->stream);
   delete ctx;
 }
@@ -416,9 +411,7 @@ extern "C" int qipb200_profile_read(qipb200_ctx *ctx, double *out4) {
       ctx->prof_pool.push_back(ctx->prof_events[cat][i].second);
     }
     out4[2 * cat] = ms;
-    double n = 0.0;
-    for (size_t i = 0; i < ctx->prof_events[cat].size(); ++i) n += ctx->prof_events[cat][i].weight;
-    out4[2 * cat + 1] = n;
+    out4[2 * cat + 1] = (double)ctx->prof_events[cat].size();
     ctx->prof_events[cat].clear();
   }
   return QIPB200_OK;
@@ -519,11 +512,7 @@ int state_alloc(qipb200_ctx *ctx, qip_prec prec, uint32_t n, int rank, int world
     ctx->pool_buf = nullptr;
     ctx->pool_bytes = 0;
   } else {
-    // a sharded state carries the staging area of the push exchange behind its amplitudes: one allocation, so the
-    // one CUDA-IPC handle (or peer pointer) of the shard covers both
-    // (opt-in, QIPB200_STAGED_EXCHANGE=1; the default in-place pair exchange needs no staging area)
-    s->has_stage = world > 1 && getenv("QIPB200_STAGED_EXCHANGE") != nullptr;
-    e = cudaMalloc(&s->buf, s->has_stage ? 2 * s->bytes : s->bytes);
+    e = cudaMalloc(&s->buf, s->bytes);
   }
   if (e == cudaSuccess) e = cudaMemsetAsync(s->buf, 0, s->bytes, ctx->stream);
   if (e == cudaSuccess && world > 1) {
@@ -619,86 +608,40 @@ int check_barrier_error(qipb200_state *s) {
   return QIPB200_OK;
 }
 
-}  // namespace
-namespace qipb200 {
-int join_halves(qipb200_state *s);
-bool overlap_exchange_enabled();
-}
-namespace {
-
-// Swap physical rank bit R (>= n_local) with local bit l.
-// Protocol (push through staging, dist.cu): [barrier] every rank pushes the half it gives away (bit l == !rb) into
-// the partner's staging area [barrier] every rank copies its own staging half into the slots it gave away.  When the
-// last tile pass before the exchange already pushed the half (s->send_stage == 2, schedule.cu) only the tail runs.
-// Default (no staging area): the in-place pair exchange (k_pair_exchange), which moves the fewest bytes locally.
-int exchange_bits(qipb200_state *s, uint32_t R, uint32_t l) {
-  qipb200_ctx *ctx = s->ctx;
-  if (!s->ipc_ready)
-    return set_err(ctx, QIPB200_ERR_COMM, "sharded state: peers not mapped (call qipb200_state_ipc_import)");
-  if (s->halves_pending) {  // an overlapped migration is still in flight on the second stream
-    int stj = join_halves(s);
-    if (stj != QIPB200_OK) return stj;
-  }
-  const uint32_t r = R - s->n_local;
-  const int partner = s->rank ^ (1 << r);
-  const int rb = (s->rank >> r) & 1;
-  {
-    ProfileScope prof(ctx, 1);
-    if (s->has_stage) {
-      const int give = 1 - rb;
-      char *my_stage = (char *)s->buf + s->bytes;
-      char *peer_stage = (char *)s->peer_buf[partner] + s->bytes;
-      if (s->send_stage && (s->send_R != R || s->send_l != l))
-        return set_err(ctx, QIPB200_ERR_COMM, "internal: the tile pass pushed a different half than the exchange needs");
-      if (s->send_stage < 1)
-        CU(ctx, launch_flag_barrier(s->peer_flags.data(), s->flags, s->rank, s->world, ++s->epoch,
-                                    s->flags + kFlagErrorSlot, ctx->stream, &ctx->launches));
-      if (s->send_stage < 2) {
-        static const bool use_ce = []() {
-          const char *e = getenv("QIPB200_STAGED_EXCHANGE");
-          return e && !strcmp(e, "ce");
-        }();
-        if (use_ce) {
-          // the give-half as a strided copy on the copy engines: rows of 2^l amplitudes every 2^(l+1)
-          const size_t ab = amp_bytes(s->prec);
-          const size_t width = ab << l, pitch = ab << (l + 1);
-          const size_t height = (size_t)1 << (s->n_local - 1 - l);
-          const char *src = (const char *)s->buf + ((size_t)give << l) * ab;
-          char *dst = peer_stage + ((size_t)(1 - give) << l) * ab;
-          if (pitch <= ((size_t)1 << 30) && height > 1) {
-            CU(ctx, cudaMemcpy2DAsync(dst, pitch, src, pitch, width, height, cudaMemcpyDeviceToDevice, ctx->stream));
-          } else {
-            for (size_t r = 0; r < height; ++r)
-              CU(ctx, cudaMemcpyAsync(dst + r * pitch, src + r * pitch, width, cudaMemcpyDeviceToDevice, ctx->stream));
-          }
-        } else {
-          CU(ctx, launch_copy_half(s->prec, s->buf, peer_stage, s->n_local, l, give, true, ctx->stream, &ctx->launches));
-        }
-      }
-      s->send_stage = 0;
-      CU(ctx, launch_flag_barrier(s->peer_flags.data(), s->flags, s->rank, s->world, ++s->epoch,
-                                  s->flags + kFlagErrorSlot, ctx->stream, &ctx->launches));
-      CU(ctx, launch_copy_half(s->prec, my_stage, s->buf, s->n_local, l, give, false, ctx->stream, &ctx->launches));
-    } else {
-      uint32_t s_bit = s->n_local - 1;
-      if (s_bit == l) s_bit = s->n_local - 2;
-      CU(ctx, launch_flag_barrier(s->peer_flags.data(), s->flags, s->rank, s->world, ++s->epoch,
-                                  s->flags + kFlagErrorSlot, ctx->stream, &ctx->launches));
-      CU(ctx, launch_pair_exchange(s->prec, s->buf, s->peer_buf[partner], s->n_local, l, s_bit, rb, ctx->stream,
-                                   &ctx->launches));
-      CU(ctx, launch_flag_barrier(s->peer_flags.data(), s->flags, s->rank, s->world, ++s->epoch,
-                                  s->flags + kFlagErrorSlot, ctx->stream, &ctx->launches));
-    }
-    ++ctx->exchange_launches;
-  }
+// After a migration of physical rank bit R and local bit l: count the bytes this rank sent and let the logical bits
+// living at R and l trade places in the map.
+void record_migration(qipb200_state *s, uint32_t R, uint32_t l) {
   s->exchange_bytes += (uint64_t)amp_bytes(s->prec) << (s->n_local - 1);
-  // update the map: the logical bits living at R and l trade places
   for (uint32_t b = 0; b < s->n; ++b) {
     if (s->phys_of_logical[b] == R)
       s->phys_of_logical[b] = l;
     else if (s->phys_of_logical[b] == l)
       s->phys_of_logical[b] = R;
   }
+}
+
+// Swap physical rank bit R (>= n_local) with local bit l: the in-place pair exchange (dist.cu: k_pair_exchange)
+// between two flag barriers.
+int exchange_bits(qipb200_state *s, uint32_t R, uint32_t l) {
+  qipb200_ctx *ctx = s->ctx;
+  if (!s->ipc_ready)
+    return set_err(ctx, QIPB200_ERR_COMM, "sharded state: peers not mapped (call qipb200_state_ipc_import)");
+  const uint32_t r = R - s->n_local;
+  const int partner = s->rank ^ (1 << r);
+  const int rb = (s->rank >> r) & 1;
+  {
+    ProfileScope prof(ctx, 1);
+    uint32_t s_bit = s->n_local - 1;
+    if (s_bit == l) s_bit = s->n_local - 2;
+    CU(ctx, launch_flag_barrier(s->peer_flags.data(), s->flags, s->rank, s->world, ++s->epoch,
+                                s->flags + kFlagErrorSlot, ctx->stream, &ctx->launches));
+    CU(ctx, launch_pair_exchange(s->prec, s->buf, s->peer_buf[partner], s->n_local, l, s_bit, rb, ctx->stream,
+                                 &ctx->launches));
+    CU(ctx, launch_flag_barrier(s->peer_flags.data(), s->flags, s->rank, s->world, ++s->epoch,
+                                s->flags + kFlagErrorSlot, ctx->stream, &ctx->launches));
+    ++ctx->exchange_launches;
+  }
+  record_migration(s, R, l);
   return QIPB200_OK;
 }
 
@@ -866,10 +809,7 @@ static int choose_victim(const qipb200_state *s, const FlatOp &f, const uint64_t
   for (uint32_t j = 0; j < f.k; ++j) used |= 1ull << f.idx_bits[j];
   int best = -1;
   uint64_t best_key = 0;
-  // with overlapped migrations (opt-in) the top local bit is never evicted: it splits the shard into the two halves
-  // an overlapped migration works on
-  const uint32_t l_end = overlap_exchange_enabled() && s->n_local > 3 ? s->n_local - 1 : s->n_local;
-  for (uint32_t l = 0; l < l_end; ++l) {
+  for (uint32_t l = 0; l < s->n_local; ++l) {
     if ((used >> l) & 1ull) continue;
     uint64_t key = 1;
     if (next_use) {
@@ -905,107 +845,6 @@ bool peek_first_exchange(const qipb200_state *s, const qip_op *op, const uint64_
     return true;
   }
   return false;
-}
-
-// The flag barrier that opens an exchange (every rank has emptied its staging area), for the tile pass that pushes
-// the give-half itself; afterwards exchange_bits(R, l) only runs the tail of the protocol.
-int exchange_open_for_send(qipb200_state *s, uint32_t R, uint32_t l, void **peer_stage, int *give) {
-  qipb200_ctx *ctx = s->ctx;
-  if (!s->ipc_ready || !s->has_stage) return QIPB200_ERR_UNSUPPORTED;
-  const uint32_t r = R - s->n_local;
-  const int partner = s->rank ^ (1 << r);
-  *give = 1 - ((s->rank >> r) & 1);
-  *peer_stage = (char *)s->peer_buf[partner] + s->bytes;
-  CU(ctx, launch_flag_barrier(s->peer_flags.data(), s->flags, s->rank, s->world, ++s->epoch, s->flags + kFlagErrorSlot,
-                              ctx->stream, &ctx->launches));
-  s->send_stage = 1;  // the caller raises it to 2 once the pushing pass is launched
-  s->send_R = R;
-  s->send_l = l;
-  return QIPB200_OK;
-}
-
-// Overlapped migrations (two half exchanges on a second stream, passes on either side run in halves): the exchange
-// and the pass contend for the same HBM and SM slots.  Parity-green (sharded worker incl. generated kernels), but opt-in.
-bool overlap_exchange_enabled() {
-  static const bool on = getenv("QIPB200_OVERLAP_EXCHANGE") != nullptr;
-  return on;
-}
-
-int ensure_overlap_resources(qipb200_state *s) {
-  qipb200_ctx *ctx = s->ctx;
-  if (ctx->stream2) return QIPB200_OK;
-  // highest priority: the exchange needs few resident warps but must not queue behind the pass's thousands of CTAs
-  int prio_lo = 0, prio_hi = 0;
-  CU(ctx, cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
-  CU(ctx, cudaStreamCreateWithPriority(&ctx->stream2, cudaStreamNonBlocking, prio_hi));
-  for (int i = 0; i < 2; ++i) {
-    CU(ctx, cudaEventCreateWithFlags(&ctx->ev_pass[i], cudaEventDisableTiming));
-    CU(ctx, cudaEventCreateWithFlags(&ctx->ev_exch[i], cudaEventDisableTiming));
-  }
-  return QIPB200_OK;
-}
-
-// The migration R <-> l as TWO half exchanges (lower / upper half of the shard = top local bit 0 / 1) on the context's
-// second stream: half v starts when ctx->ev_pass[v] (recorded by the caller on the main stream: "this half is final")
-// has fired, and ctx->ev_exch[v] fires when it is done -- the tile pass before the migration overlaps the exchange of
-// the half it finished first, the pass after it starts on the half that arrived first.  Every rank runs exactly this
-// protocol (two barrier-exchange-barrier groups); what a rank overlaps with it is its own business.
-int exchange_bits_split(qipb200_state *s, uint32_t R, uint32_t l) {
-  qipb200_ctx *ctx = s->ctx;
-  if (!s->ipc_ready) return set_err(ctx, QIPB200_ERR_COMM, "sharded state: peers not mapped (call qipb200_state_ipc_import)");
-  if (s->n_local < 4 || l >= s->n_local - 1) return set_err(ctx, QIPB200_ERR_UNSUPPORTED, "internal: split exchange on the top local bit");
-  int st0 = ensure_overlap_resources(s);
-  if (st0 != QIPB200_OK) return st0;
-  const uint32_t r = R - s->n_local;
-  const int partner = s->rank ^ (1 << r);
-  const int rb = (s->rank >> r) & 1;
-  const uint32_t nh = s->n_local - 1;  // bits of a half
-  uint32_t s_bit = nh - 1;
-  if (s_bit == l) s_bit = nh - 2;
-  const size_t half_bytes = s->bytes >> 1;
-  for (int v = 0; v < 2; ++v) {
-    CU(ctx, cudaStreamWaitEvent(ctx->stream2, ctx->ev_pass[v], 0));
-    cudaEvent_t t0 = nullptr, t1 = nullptr;
-    if (ctx->profile) {
-      auto take = [&]() {
-        cudaEvent_t e = nullptr;
-        if (!ctx->prof_pool.empty()) {
-          e = ctx->prof_pool.back();
-          ctx->prof_pool.pop_back();
-        } else if (cudaEventCreate(&e) != cudaSuccess) {
-          e = nullptr;
-        }
-        return e;
-      };
-      t0 = take();
-      t1 = take();
-      if (t0) cudaEventRecord(t0, ctx->stream2);
-    }
-    CU(ctx, launch_flag_barrier(s->peer_flags.data(), s->flags, s->rank, s->world, ++s->epoch, s->flags + kFlagErrorSlot,
-                                ctx->stream2, &ctx->launches));
-    static const char *exch_ctas = getenv("QIPB200_EXCH_CTAS");
-    const unsigned split_ctas = exch_ctas ? (unsigned)atoi(exch_ctas) : 2u * (unsigned)ctx->sm_count;  // two CTAs per SM
-    CU(ctx, launch_pair_exchange(s->prec, (char *)s->buf + v * half_bytes, (char *)s->peer_buf[partner] + v * half_bytes, nh, l, s_bit,
-                                 rb, ctx->stream2, &ctx->launches, split_ctas));
-    CU(ctx, launch_flag_barrier(s->peer_flags.data(), s->flags, s->rank, s->world, ++s->epoch, s->flags + kFlagErrorSlot,
-                                ctx->stream2, &ctx->launches));
-    if (t0 && t1) {
-      cudaEventRecord(t1, ctx->stream2);
-      qipb200_ctx::ProfEvent pe = {t0, t1, 0.5};
-      ctx->prof_events[1].push_back(pe);
-    }
-    CU(ctx, cudaEventRecord(ctx->ev_exch[v], ctx->stream2));
-  }
-  ++ctx->exchange_launches;
-  s->halves_pending = true;
-  s->exchange_bytes += (uint64_t)amp_bytes(s->prec) << (s->n_local - 1);
-  for (uint32_t b = 0; b < s->n; ++b) {
-    if (s->phys_of_logical[b] == R)
-      s->phys_of_logical[b] = l;
-    else if (s->phys_of_logical[b] == l)
-      s->phys_of_logical[b] = R;
-  }
-  return QIPB200_OK;
 }
 
 // ---- migration fused into a tile pass, in place (paired send) ----
@@ -1049,23 +888,7 @@ int finish_paired_exchange(qipb200_state *s, uint32_t R, uint32_t l) {
                                 ctx->stream, &ctx->launches));
   }
   ++ctx->exchange_launches;
-  s->exchange_bytes += (uint64_t)amp_bytes(s->prec) << (s->n_local - 1);
-  for (uint32_t b = 0; b < s->n; ++b) {
-    if (s->phys_of_logical[b] == R)
-      s->phys_of_logical[b] = l;
-    else if (s->phys_of_logical[b] == l)
-      s->phys_of_logical[b] = R;
-  }
-  return QIPB200_OK;
-}
-
-// Make the main stream wait for an overlapped migration (both halves).
-int join_halves(qipb200_state *s) {
-  if (!s->halves_pending) return QIPB200_OK;
-  qipb200_ctx *ctx = s->ctx;
-  CU(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_exch[0], 0));
-  CU(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_exch[1], 0));
-  s->halves_pending = false;
+  record_migration(s, R, l);
   return QIPB200_OK;
 }
 

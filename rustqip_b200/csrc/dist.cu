@@ -11,11 +11,13 @@
 // read-old/write-new hazard.  Per rank and direction 2^(n_local-1) amplitudes cross
 // the link (half pulled by me, half pushed by the partner).
 //
+// The paired send (QIPB200_PAIRED_SEND=1) does the trade inside the epoch's last
+// tile pass instead (jit_codegen.cpp: QIP_PAIRED); k_paired_send below plays the
+// same per-tile protocol for a rank whose pass could not.
+//
 // Cross-GPU ordering is a flag barrier in peer-visible memory (system-scope
 // release/acquire), launched on the same stream before and after the trade.
 #include "dist.cuh"
-
-#include <cstdlib>
 
 namespace qipb200 {
 
@@ -65,7 +67,7 @@ __global__ void __launch_bounds__(kThreads)
 }
 
 cudaError_t launch_pair_exchange(qip_prec prec, void *mine, void *peer, uint32_t n_local, uint32_t l,
-                                 uint32_t s_bit, int rb, cudaStream_t s, uint64_t *launches, unsigned max_ctas) {
+                                 uint32_t s_bit, int rb, cudaStream_t s, uint64_t *launches) {
   if (n_local < 2 || l == s_bit || l >= n_local || s_bit >= n_local) return cudaErrorInvalidValue;
   ExArgs a;
   a.pos_lo = l < s_bit ? l : s_bit;
@@ -73,80 +75,11 @@ cudaError_t launch_pair_exchange(qip_prec prec, void *mine, void *peer, uint32_t
   a.fixed = ((uint64_t)(rb ? 0 : 1) << l) | ((uint64_t)(rb ? 1 : 0) << s_bit);
   a.flip = 1ull << l;
   a.n_items = 1ull << (n_local - 2);
-  static const int unroll = []() {
-    const char *e = getenv("QIPB200_EXCH_UNROLL");
-    const int u = e ? atoi(e) : 4;
-    return u == 1 || u == 2 || u == 4 || u == 8 ? u : 4;
-  }();
-#define QIP_EXCH(UU)                                                                                        \
-  {                                                                                                         \
-    unsigned grid = (unsigned)((a.n_items + (uint64_t)kThreads * UU - 1) / ((uint64_t)kThreads * UU));       \
-    if (max_ctas && grid > max_ctas) grid = max_ctas;                                                       \
-    if (prec == QIP_F32)                                                                                    \
-      k_pair_exchange<float2, UU><<<grid, kThreads, 0, s>>>((float2 *)mine, (float2 *)peer, a);             \
-    else                                                                                                    \
-      k_pair_exchange<double2, UU><<<grid, kThreads, 0, s>>>((double2 *)mine, (double2 *)peer, a);          \
-  }
-  switch (unroll) {
-    case 1: QIP_EXCH(1) break;
-    case 2: QIP_EXCH(2) break;
-    case 8: QIP_EXCH(8) break;
-    default: QIP_EXCH(4) break;
-  }
-#undef QIP_EXCH
-  ++*launches;
-  return cudaGetLastError();
-}
-
-// ---- push exchange through a staging buffer -----------------------------------------------------------
-// Half of the traffic of each direction of the in-place pair exchange above are responses to the partner's remote
-// LOADS.  Writes are posted: every rank PUSHES the half it gives away into the partner's staging buffer (slot of the
-// amplitude it becomes there: index with bit l flipped), a flag barrier later each rank copies its staging half into
-// the slots it gave away (local HBM traffic).  The push can also be done by the last tile pass before the exchange
-// (jit_codegen: tiles of the give-half are TMA-stored to the partner's staging buffer instead of the local state).
-struct HalfArgs {
-  uint32_t pos;      // the bit l
-  uint64_t fixed;    // give_val << l
-  uint64_t flip;     // 1 << l (0 for the unstage copy)
-  uint64_t n_items;  // 2^(n_local-1)
-};
-
-template <typename V, int U>
-__global__ void __launch_bounds__(kThreads) k_copy_half(const V *__restrict__ src, V *__restrict__ dst, const HalfArgs a) {
-  const uint64_t w0 = (uint64_t)blockIdx.x * (kThreads * U) + threadIdx.x;
-  V x[U];
-  uint64_t ii[U];
-  bool on[U];
-#pragma unroll
-  for (int u = 0; u < U; ++u) {
-    const uint64_t w = w0 + (uint64_t)u * kThreads;
-    on[u] = w < a.n_items;
-    uint64_t idx = on[u] ? w : 0;
-    idx = ((idx >> a.pos) << (a.pos + 1)) | (idx & ((1ull << a.pos) - 1ull));
-    ii[u] = idx | a.fixed;
-  }
-#pragma unroll
-  for (int u = 0; u < U; ++u)
-    if (on[u]) x[u] = src[ii[u]];
-#pragma unroll
-  for (int u = 0; u < U; ++u)
-    if (on[u]) dst[ii[u] ^ a.flip] = x[u];
-}
-
-// dst[i ^ flip] = src[i] for every i whose bit l equals give_val (flip_bit: push to the partner; else a plain half copy)
-cudaError_t launch_copy_half(qip_prec prec, const void *src, void *dst, uint32_t n_local, uint32_t l, int give_val, bool flip_bit,
-                             cudaStream_t s, uint64_t *launches) {
-  if (n_local < 1 || l >= n_local) return cudaErrorInvalidValue;
-  HalfArgs a;
-  a.pos = l;
-  a.fixed = (uint64_t)(give_val ? 1 : 0) << l;
-  a.flip = flip_bit ? (1ull << l) : 0ull;
-  a.n_items = 1ull << (n_local - 1);
   const unsigned grid = (unsigned)((a.n_items + (uint64_t)kThreads * 4 - 1) / ((uint64_t)kThreads * 4));
   if (prec == QIP_F32)
-    k_copy_half<float2, 4><<<grid, kThreads, 0, s>>>((const float2 *)src, (float2 *)dst, a);
+    k_pair_exchange<float2, 4><<<grid, kThreads, 0, s>>>((float2 *)mine, (float2 *)peer, a);
   else
-    k_copy_half<double2, 4><<<grid, kThreads, 0, s>>>((const double2 *)src, (double2 *)dst, a);
+    k_pair_exchange<double2, 4><<<grid, kThreads, 0, s>>>((double2 *)mine, (double2 *)peer, a);
   ++*launches;
   return cudaGetLastError();
 }

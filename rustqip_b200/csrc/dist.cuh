@@ -25,14 +25,7 @@ static const size_t kFlagAllocBytes = kPairFlagOffsetBytes + (sizeof(uint32_t) <
 // Trade the half-shard selected by local bit `l` with the partner's (see dist.cu).
 // rb = this rank's value of the rank bit being migrated; s_bit = pair-ownership bit.
 cudaError_t launch_pair_exchange(qip_prec prec, void *mine, void *peer, uint32_t n_local, uint32_t l,
-                                 uint32_t s_bit, int rb, cudaStream_t s, uint64_t *launches, unsigned max_ctas = 0);
-// max_ctas > 0: a persistent grid of at most that many CTAs (grid-stride): the exchange is NVLink-bound and needs few
-// resident warps, so that a tile pass running next to it keeps the SMs
-
-// dst[i ^ (flip_bit ? 1<<l : 0)] = src[i] for every i of the 2^n_local amplitudes whose bit l equals give_val:
-// the push of the half a rank gives away into the partner's staging buffer, and the copy out of a rank's own staging.
-cudaError_t launch_copy_half(qip_prec prec, const void *src, void *dst, uint32_t n_local, uint32_t l, int give_val, bool flip_bit,
-                             cudaStream_t s, uint64_t *launches);
+                                 uint32_t s_bit, int rb, cudaStream_t s, uint64_t *launches);
 
 // The protocol of a migration fused into a tile pass (jit_codegen.cpp: pair_*), played by a stand-alone kernel for a
 // rank whose last pass could not do it itself: every tile of the half this rank gives away is read, announced to the

@@ -751,10 +751,10 @@ bool jit_generate(const HostPass &pass, qip_prec prec, JitProgram *out, std::str
   src << "  unsigned hi_pos[8];\n";
   if (NPH) src << "  unsigned pt_begin[NPH + 1];\n";
   if (synth) src << "  unsigned init_lo, init_hi;\n";  // the basis index the tiles are built from
-  // multi-GPU: tiles whose index bit `send_bit` equals `send_val` are stored to `tmap_out` (the partner's staging
-  // area) at the index with that bit flipped -- the push half of a qubit migration; send_bit >= 64: off
+  // multi-GPU (paired send, below): tiles whose index bit `send_bit` equals `send_val` are stored to `tmap_out` (the
+  // partner's shard) at the index with that bit flipped; send_bit >= 64: off
   src << "  unsigned send_bit, send_val;\n";
-  // a launch may cover a contiguous part of the tile counter (half a pass around a multi-GPU migration)
+  // first tile of the launch in the tile counter (jit_runtime.cu writes 0: every launch covers the whole pass)
   src << "  unsigned tile_off_lo, tile_off_hi;\n";
   // tiles of this launch: a CTA walks the tile counter with stride gridDim.x (grid == tile count: one tile per CTA;
   // a grid of a few CTAs per SM: persistent CTAs, no CTA exit / launch / barrier init between tiles)

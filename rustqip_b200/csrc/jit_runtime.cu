@@ -331,7 +331,7 @@ void jit_wait_all(uint64_t *n_compiled, double *total_ms, uint64_t *n_from_disk)
 
 cudaError_t jit_launch(const std::shared_ptr<const JitCubin> &cubin, std::vector<std::pair<const JitCubin *, JitLoaded>> *loaded,
                        const JitProgram &prog, void *psi, uint32_t n_local, const CUtensorMap &tmap, cudaStream_t stream,
-                       std::string *err, const CUtensorMap *tmap_out, uint32_t send_bit, uint32_t send_val, uint32_t half,
+                       std::string *err, const CUtensorMap *tmap_out, uint32_t send_bit, uint32_t send_val,
                        const JitPair *pair) {
   Driver &d = driver();
   if (!d.ok || !cubin || !cubin->ok) {
@@ -366,14 +366,10 @@ cudaError_t jit_launch(const std::shared_ptr<const JitCubin> &cubin, std::vector
     memcpy(params.data() + prog.send_offset + 4, &send_val, 4);
   }
   void *args[4] = {&psi, params.data(), &tm, &tm_out};
-  uint64_t tiles = 1ull << (n_local - prog.tiles_log2_sub), off = 0;
+  const uint64_t tiles = 1ull << (n_local - prog.tiles_log2_sub);
   if (prog.send_offset + 64 > params.size()) return cudaErrorInvalidValue;
-  if (half < 2 && tiles >= 2) {
-    tiles >>= 1;
-    off = half ? tiles : 0ull;
-  }
   {
-    const uint32_t w[4] = {(uint32_t)off, (uint32_t)(off >> 32), (uint32_t)tiles, (uint32_t)(tiles >> 32)};
+    const uint32_t w[4] = {0u, 0u, (uint32_t)tiles, (uint32_t)(tiles >> 32)};  // tile offset 0, every tile
     memcpy(params.data() + prog.send_offset + 8, w, 16);
   }
   // QIPB200_JIT_PERSISTENT=<CTAs>: a fixed grid of persistent CTAs walking the tile counter instead of one CTA per tile

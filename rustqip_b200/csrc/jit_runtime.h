@@ -46,10 +46,10 @@ std::shared_ptr<const JitCubin> jit_request(const std::string &source, bool wait
 void jit_wait_all(uint64_t *n_compiled, double *total_ms, uint64_t *n_from_disk = nullptr);
 
 // Load (once per context) and launch.  `loaded` is the context's module cache keyed by the cubin pointer.
-// `tmap_out` / `send_bit` / `send_val` (optional): tiles whose index bit send_bit equals send_val are stored
-// through tmap_out at the index with that bit flipped (the push half of a multi-GPU qubit migration).
-// `pair` (optional, with tmap_out over the partner's SHARD): the migration is done in place, tile by tile, under a
-// per-tile flag handshake with the partner's pass (jit_codegen.cpp: pair_*).
+// `tmap_out` / `send_bit` / `send_val` / `pair` (optional, the paired send of a multi-GPU qubit migration): tiles whose
+// index bit send_bit equals send_val are stored through tmap_out, a map over the partner's SHARD, at the index with that
+// bit flipped; the migration is done in place, tile by tile, under a per-tile flag handshake with the partner's pass
+// (jit_codegen.cpp: pair_*).
 struct JitPair {
   uint32_t cbit = 0;              // position of index bit send_bit in the tile counter
   uint32_t seq = 0;               // value of this migration in the flag words
@@ -60,7 +60,6 @@ struct JitPair {
 cudaError_t jit_launch(const std::shared_ptr<const JitCubin> &cubin, std::vector<std::pair<const JitCubin *, JitLoaded>> *loaded,
                        const JitProgram &prog, void *psi, uint32_t n_local, const CUtensorMap &tmap, cudaStream_t stream,
                        std::string *err, const CUtensorMap *tmap_out = nullptr, uint32_t send_bit = 64, uint32_t send_val = 0,
-                       uint32_t half = 2,  // half: 0 / 1 = the lower / upper half of the tile counter only, 2 = all tiles
                        const JitPair *pair = nullptr);
 
 void jit_unload(std::vector<std::pair<const JitCubin *, JitLoaded>> *loaded);

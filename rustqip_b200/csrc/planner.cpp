@@ -1387,9 +1387,8 @@ void plan_passes(const std::vector<FlatOp> &ops, uint32_t n_local, qip_prec prec
       h.L = cfg.L;
       h.m = m;
       // pad the tile-bit set to exactly m bits with the highest unused bits
-      for (int round = 0; round < 2; ++round)  // first without the reserved bit, then with it if the tile is still short
-        for (int b = (int)n_local - 1; b >= (int)cfg.L && (uint32_t)popc(S_high) < m; --b)
-          if (!((S_high >> b) & 1) && (round == 1 || b != cfg.reserve_bit)) S_high |= 1ull << b;
+      for (int b = (int)n_local - 1; b >= (int)cfg.L && (uint32_t)popc(S_high) < m; --b)
+        if (!((S_high >> b) & 1)) S_high |= 1ull << b;
       uint32_t c = 0;
       for (uint32_t b = 0; b < 64; ++b)
         if ((S_high >> b) & 1) h.hi_pos[c++] = b;

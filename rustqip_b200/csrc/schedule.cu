@@ -46,11 +46,8 @@ bool needs_exchange(const qipb200_state *s, const FlatOp &f) {
   return false;
 }
 
-// The push half of the qubit migration that follows this epoch, to be done by the epoch's last tile pass.
+// The qubit migration that follows this epoch, to be done by the epoch's last tile pass.
 struct SendPlan {
-  bool on = false;       // staged protocol: the last pass pushes the give-half
-  bool overlap = false;  // in-place protocol in two halves on the second stream (exchange_bits_split): the last step
-                         // records "lower / upper half final" on the context's events, preferably half by half
   bool pair = false;     // in-place protocol fused into the last pass (paired send): tiles of the give-half go straight into
                          // the partner's shard under a per-tile flag handshake; a rank whose last pass cannot do it runs
                          // the pass normally and then the stand-in kernel -- the partner does not see the difference
@@ -64,7 +61,7 @@ int execute_steps(qipb200_state *s, const std::vector<PlanStep> &steps, const st
   PassParams *pp = new PassParams();
   // Generated kernels (jit_codegen / jit_runtime): every pass is turned into specialised source; a pass whose
   // cubin is ready runs it, the others run the interpreter kernel while the background workers compile.
-  bool halves_recorded = false, paired_done = false;
+  bool paired_done = false;
   uint32_t pair_cbit = 0, pair_seq = 0;
   if (send.pair && !steps.empty() && steps.back().is_pass) {
     const PassHeader &lh = steps.back().pass.hdr;
@@ -98,26 +95,11 @@ int execute_steps(qipb200_state *s, const std::vector<PlanStep> &steps, const st
         std::shared_ptr<const JitCubin> cubin = jit_request(progs[i].source, jmode == JIT_SYNC);
         if (cubin && !cubin->ok) ctx->jit_note = "NVRTC: " + cubin->log;
         if (cubin && cubin->ok) {
-          // Last pass before a migration: the tiles of the half this rank gives away go straight to the partner's
-          // staging area (TMA stores over NVLink), provided bit l is constant within a TMA box of this pass.
+          // Paired send: the give-half tiles go into the partner's shard, tile by tile under the flag handshake.
           alignas(64) CUtensorMap tmap_out;
           const CUtensorMap *tmo = nullptr;
           uint32_t send_bit = 64, send_val = 0;
           const PassHeader &ph = steps[i].pass.hdr;
-          if (send.on && i + 1 == steps.size() && send.l >= ph.L && send.l != ph.hi_pos[0] && send.l != ph.hi_pos[1] &&
-              send.l != ph.hi_pos[2]) {
-            void *peer_stage = nullptr;
-            int give = 0;
-            memset(&tmap_out, 0, sizeof(tmap_out));
-            if (exchange_open_for_send(s, send.R, send.l, &peer_stage, &give) == QIPB200_OK) {
-              if (make_tile_map(&tmap_out, s->prec, peer_stage, s->n_local, ph)) {
-                tmo = &tmap_out;
-                send_bit = send.l;
-                send_val = (uint32_t)give;
-              }  // else: the opening barrier stays queued (send_stage 1), exchange_bits pushes with its own kernel
-            }
-          }
-          // Paired send: the give-half tiles go into the partner's shard, tile by tile under the flag handshake.
           JitPair pair;
           // (test hook QIPB200_PAIRED_STANDIN_RANK=<rank | -1 for all>: that rank never fuses the send into its pass)
           static const int standin_rank = getenv("QIPB200_PAIRED_STANDIN_RANK") ? atoi(getenv("QIPB200_PAIRED_STANDIN_RANK")) : -2;
@@ -137,40 +119,16 @@ int execute_steps(qipb200_state *s, const std::vector<PlanStep> &steps, const st
               pair.error_word = s->flags + kFlagErrorSlot;
             }
           }
-          // A pass next to an overlapped migration runs in two halves of the tile counter (= top local bit 0 / 1,
-          // which must not be a tile bit): after a migration each half starts when its exchange is done, before one
-          // each half is reported final as soon as it is.
-          const bool top_free = ph.hi_pos[ph.m - 1] != s->n_local - 1 && s->n_local > ph.T;
-          const bool after_mig = s->halves_pending, before_mig = send.overlap && i + 1 == steps.size();
           std::string err;
-          cudaError_t e = cudaSuccess;
-          if ((after_mig || before_mig) && top_free) {
-            for (uint32_t v = 0; v < 2 && e == cudaSuccess; ++v) {
-              if (after_mig) e = cudaStreamWaitEvent(ctx->stream, ctx->ev_exch[v], 0);
-              if (e != cudaSuccess) break;
-              {
-                ProfileScope prof(ctx, 0, 0.5);
-                e = jit_launch(cubin, &ctx->jit_loaded, progs[i], s->buf, s->n_local, tmap, ctx->stream, &err, nullptr, 64, 0, v);
-              }
-              if (e == cudaSuccess && before_mig) e = cudaEventRecord(ctx->ev_pass[v], ctx->stream);
-            }
-            if (e == cudaSuccess) {
-              s->halves_pending = false;
-              if (before_mig) halves_recorded = true;
-              ++ctx->launches;  // two launches for this pass
-            }
-          } else {
-            if (after_mig && join_halves(s) != QIPB200_OK) return QIPB200_ERR_CUDA;
+          cudaError_t e;
+          {
             ProfileScope prof(ctx, 0);
-            e = jit_launch(cubin, &ctx->jit_loaded, progs[i], s->buf, s->n_local, tmap, ctx->stream, &err, tmo, send_bit, send_val, 2,
-                           pair_here && tmo ? &pair : nullptr);
+            e = jit_launch(cubin, &ctx->jit_loaded, progs[i], s->buf, s->n_local, tmap, ctx->stream, &err, tmo, send_bit, send_val,
+                           tmo ? &pair : nullptr);
           }
           if (e == cudaSuccess) {
             if (progs[i].synthesised) s->init_pending = false;
-            if (pair_here && tmo)
-              paired_done = true;
-            else if (tmo)
-              s->send_stage = 2;
+            if (tmo) paired_done = true;
             ++ctx->launches;
             ++ctx->tile_launches;
             ++ctx->jit_launches;
@@ -184,7 +142,6 @@ int execute_steps(qipb200_state *s, const std::vector<PlanStep> &steps, const st
     }
     // a step that reads the amplitudes: a pending basis state is written first (no generated synthesising pass ran)
     if (s->init_pending && (st = materialise_init(s)) != QIPB200_OK) break;
-    if (s->halves_pending && (st = join_halves(s)) != QIPB200_OK) break;  // this step sweeps the whole shard at once
     if (steps[i].is_pass) {
       if (!serialise_pass(steps[i].pass, pp)) {
         st = report_error(s, QIPB200_ERR_UNSUPPORTED, "internal: fused pass exceeds the kernel parameter space");
@@ -206,12 +163,6 @@ int execute_steps(qipb200_state *s, const std::vector<PlanStep> &steps, const st
   if (send.pair && getenv("QIPB200_PAIRED_DEBUG"))
     fprintf(stderr, "paired send: rank %d migration %u (R=%u l=%u) %s\n", s->rank, pair_seq, send.R, send.l,
             paired_done ? "fused into the pass" : "stand-in kernel");
-  if (st == QIPB200_OK && send.overlap && !halves_recorded) {
-    // the epoch's last step ran as one launch (or there was none): both halves are final now
-    if (s->halves_pending && (st = join_halves(s)) != QIPB200_OK) return st;
-    if (cudaEventRecord(ctx->ev_pass[0], ctx->stream) != cudaSuccess || cudaEventRecord(ctx->ev_pass[1], ctx->stream) != cudaSuccess)
-      return report_cuda_error(s, cudaGetLastError(), "cudaEventRecord");
-  }
   return st;
 }
 
@@ -227,13 +178,12 @@ int run_fused(qipb200_state *s, const qip_op *ops, size_t n_ops, const std::vect
     if (e != cudaSuccess) return report_cuda_error(s, e, "cudaFuncSetAttribute(tile pass)");
     s->ctx->tile_configured = true;
   }
-  PlanConfig cfg = default_plan_config(s->prec, s->n_local, s->world > 1);
-  if (s->world > 1 && overlap_exchange_enabled()) cfg.reserve_bit = (int)s->n_local - 1;  // passes splittable in halves
+  const PlanConfig cfg = default_plan_config(s->prec, s->n_local, s->world > 1);
   // Paired send (QIPB200_PAIRED_SEND=1): the migration that ends an epoch is fused into the epoch's last tile pass and done
   // in place, tile by tile, against the partner's copy of the same pass.  Tiles pair up across GPUs, so every rank must
   // choose the same tile bits: the planner then selects from rank-independent data only (op_uniform_info).
   static const bool paired_env = getenv("QIPB200_PAIRED_SEND") != nullptr && atoi(getenv("QIPB200_PAIRED_SEND")) != 0;
-  const bool paired_mode = paired_env && s->world > 1 && !s->has_stage && !overlap_exchange_enabled() && cfg.use_tma &&
+  const bool paired_mode = paired_env && s->world > 1 && cfg.use_tma &&
                            cfg.groups_per_thread == 1 && jit_mode_from_env(s->n_local) != JIT_OFF &&
                            cfg.T == (s->prec == QIP_F32 ? 13u : 12u) && s->n_local > cfg.T && s->n_local - cfg.T <= kPairFlagLog2;
   std::vector<size_t> remaining(n_ops);
@@ -291,33 +241,21 @@ int run_fused(qipb200_state *s, const qip_op *ops, size_t n_ops, const std::vect
         first_blocked = i;
         break;
       }
-    // The migration that ends this epoch is known before the epoch runs: its last tile pass can push the half this
-    // rank gives away while it stores its tiles (each rank decides for itself; a rank whose last step cannot do it
-    // pushes with the stand-alone kernel inside exchange_bits -- the partner does not care how its staging area fills).
+    // The migration that ends this epoch is known before the epoch runs: under the paired send the epoch's last tile
+    // pass does it.
     SendPlan send;
-    static const bool fused_send = !getenv("QIPB200_NO_FUSED_SEND");
-    const bool overlap_exchange = overlap_exchange_enabled();
-    if (first_blocked != left.size()) {
+    if (paired_mode && first_blocked != left.size()) {
       const size_t op_idx = remaining[left[first_blocked]];
       const uint64_t *nu = next_use.empty() ? nullptr : &next_use[(op_idx + 1) * s->n];
-      if (paired_mode) {
-        if (!steps.empty() && steps.back().is_pass && peek_first_exchange(s, &ops[op_idx], nu, &send.R, &send.l)) {
-          const PassHeader &ph = steps.back().pass.hdr;  // rank-independent geometry: bit l must be constant within a tile
-          bool ok = send.l >= ph.L && ph.T == cfg.T;
-          for (uint32_t k = 0; k < ph.m; ++k) ok = ok && ph.hi_pos[k] != send.l;
-          send.pair = ok;
-        }
-      } else if (s->has_stage) {
-        if (fused_send && !steps.empty() && steps.back().is_pass) send.on = peek_first_exchange(s, &ops[op_idx], nu, &send.R, &send.l);
-      } else if (overlap_exchange && s->world > 1 && s->n_local >= 8) {
-        // in-place exchange in two halves on the second stream, overlapping the passes on either side of it
-        send.overlap = peek_first_exchange(s, &ops[op_idx], nu, &send.R, &send.l) && send.l < s->n_local - 1 &&
-                       ensure_overlap_resources(s) == QIPB200_OK;
+      if (!steps.empty() && steps.back().is_pass && peek_first_exchange(s, &ops[op_idx], nu, &send.R, &send.l)) {
+        const PassHeader &ph = steps.back().pass.hdr;  // rank-independent geometry: bit l must be constant within a tile
+        bool ok = send.l >= ph.L && ph.T == cfg.T;
+        for (uint32_t k = 0; k < ph.m; ++k) ok = ok && ph.hi_pos[k] != send.l;
+        send.pair = ok;
       }
     }
     int st = execute_steps(s, steps, local, cfg, send);
     if (st != QIPB200_OK) return st;
-    if (send.overlap && (st = exchange_bits_split(s, send.R, send.l)) != QIPB200_OK) return st;
     if (send.pair && (st = finish_paired_exchange(s, send.R, send.l)) != QIPB200_OK) return st;
     if (left.empty()) break;
     if (first_blocked == left.size())
@@ -407,11 +345,7 @@ int run_schedule(qipb200_state *s, const qip_op *ops, size_t n_ops, uint32_t fla
     int st = QIPB200_OK;
     if (run_rotating(s, ops, n_ops, &st)) return st;
   }
-  if (fuse) {
-    const int st = run_fused(s, ops, n_ops, next_use);
-    const int stj = join_halves(s);  // whatever follows (download, measurement, the next schedule) sees one stream again
-    return st != QIPB200_OK ? st : stj;
-  }
+  if (fuse) return run_fused(s, ops, n_ops, next_use);
   if (n_ops) {  // one sweep per entry: the pending basis state is written first
     const int st = materialise_init(s);
     if (st != QIPB200_OK) return st;

@@ -22,11 +22,6 @@ int report_error(qipb200_state *s, int status, const std::string &msg);
 int report_cuda_error(qipb200_state *s, cudaError_t e, const char *what);
 int compile_and_localize(qipb200_state *s, const qip_op *op, FlatOp *f, const uint64_t *next_use);
 bool peek_first_exchange(const qipb200_state *s, const qip_op *op, const uint64_t *next_use, uint32_t *R, uint32_t *l);
-int exchange_open_for_send(qipb200_state *s, uint32_t R, uint32_t l, void **peer_stage, int *give);
-int exchange_bits_split(qipb200_state *s, uint32_t R, uint32_t l);
-int join_halves(qipb200_state *s);
-int ensure_overlap_resources(qipb200_state *s);
-bool overlap_exchange_enabled();
 // migration fused into the epoch's last tile pass, in place (paired send): who the partner is / what is left to do after
 // the pass (or its stand-in kernel) ran: the closing barrier and the bit-map update
 void paired_partner(const qipb200_state *s, uint32_t R, int *partner, int *give);

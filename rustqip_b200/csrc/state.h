@@ -24,10 +24,6 @@ struct qipb200_ctx {
   uint64_t jit_launches = 0;       // tile passes among `tile_launches` that ran a generated (specialised) kernel
   std::vector<std::pair<const qipb200::JitCubin *, qipb200::JitLoaded>> jit_loaded;  // modules loaded on this device
   std::string jit_note;            // why the generated-kernel path was not taken last time (diagnostics)
-  // second stream + events for the exchange that overlaps tile passes (api.cu: exchange_bits_split)
-  cudaStream_t stream2 = nullptr;
-  cudaEvent_t ev_pass[2] = {nullptr, nullptr};  // recorded on `stream`: the lower / upper half of the shard is final
-  cudaEvent_t ev_exch[2] = {nullptr, nullptr};  // recorded on `stream2`: that half has been exchanged
   // multi-device context (qipb200_init_multi): one child context per device, owned by the parent; states created
   // on the parent are sharded over the children inside this one process (peer access instead of CUDA IPC)
   std::vector<qipb200_ctx *> children;
@@ -44,7 +40,6 @@ struct qipb200_ctx {
   bool profile = false;
   struct ProfEvent {
     cudaEvent_t first, second;
-    double weight;  // 1 per launch; 0.5 for each half of a pass launched in two halves around a migration
   };
   std::vector<ProfEvent> prof_events[2];
   std::vector<cudaEvent_t> prof_pool;
@@ -63,13 +58,8 @@ struct qipb200_state {
   uint32_t n = 0;        // qubits of the whole state
   uint32_t n_local = 0;  // index bits held by this rank
   int rank = 0, world = 1;
-  void *buf = nullptr;      // 2^n_local amplitudes (sharded states: followed by a staging area of the same size)
-  bool has_stage = false;   // the allocation of `buf` is 2 * bytes: [state | staging of the push exchange]
-  uint32_t pair_seq = 0;        // migrations fused into a tile pass so far (value written into the per-tile flag words)
-  bool halves_pending = false;  // the two halves of the shard become valid at ctx->ev_exch[0/1] (an overlapped migration)
-  int send_stage = 0;       // pending exchange: 0 nothing yet, 1 its opening barrier is queued, 2 ... and the last tile
-                            // pass has pushed the give-half into the partner's staging area
-  uint32_t send_R = 0, send_l = 0;  // ... for this (rank bit, local bit) pair
+  void *buf = nullptr;      // 2^n_local amplitudes
+  uint32_t pair_seq = 0;    // migrations fused into a tile pass so far (value written into the per-tile flag words)
   void *scratch = nullptr;  // same size, lazily allocated (out-of-place row kernel only)
   size_t bytes = 0;
   // logical index bit b (= n-1-q) -> physical index bit.  Physical bits >= n_local are
@@ -126,8 +116,7 @@ struct ProfileScope {
   qipb200_ctx *ctx;
   int cat;
   cudaEvent_t e0 = nullptr, e1 = nullptr;
-  double weight = 1.0;
-  ProfileScope(qipb200_ctx *c, int category, double w = 1.0) : ctx(c), cat(category), weight(w) {
+  ProfileScope(qipb200_ctx *c, int category) : ctx(c), cat(category) {
     if (!ctx->profile) return;
     auto take = [&]() {
       cudaEvent_t e = nullptr;
@@ -146,7 +135,7 @@ struct ProfileScope {
   ~ProfileScope() {
     if (!e0 || !e1) return;
     cudaEventRecord(e1, ctx->stream);
-    qipb200_ctx::ProfEvent pe = {e0, e1, weight};
+    qipb200_ctx::ProfEvent pe = {e0, e1};
     ctx->prof_events[cat].push_back(pe);
   }
 };

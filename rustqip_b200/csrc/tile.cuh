@@ -258,8 +258,6 @@ struct PlanConfig {
                                 // 22 -> 20, at many times the planning time: worth it only for a circuit run many
                                 // times, hence opt-in
   uint32_t jit_group_bits = 0;     // > 0: also emit the pass as groups of this many bits for the generated kernels
-  int reserve_bit = -1;            // a local bit the tile-bit padding avoids (sharded states keep their top local bit out
-                                   // of the tiles so that a pass can be run in two halves around a migration)
   int groups_per_thread = 1;       // register-resident groups per interpreter decode (1: 3 CTAs/SM, 2: 2 CTAs/SM)
   uint32_t compose_threshold = 8;  // >= this many 2x2 gates in one group: compose them into one 8x8
 };
