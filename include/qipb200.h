@@ -478,6 +478,58 @@ int qipb200_multiqubit_channels_plan(qip_prec prec, uint32_t n_qubits, size_t n_
                                      const uint64_t *qubits, const uint32_t *n_kraus, const double *kraus,
                                      uint32_t *out4);
 
+/* One quantum-trajectory step of channels on k = 1..4 qubits each with ANY complete set of Kraus operators (absent in
+ * the reference): Kraus sets fitted by process tomography, noisy gates given as one channel ({(A_i (x) A_j) CNOT},
+ * {sqrt(p_i) P_i U}), relaxation with a coherent part, damping along any axis.  Channels are encoded as for
+ * qipb200_state_apply_multiqubit_channels (arity 1..4, 1..256 operators, 2^k x 2^k matrices in the qip_op MAT
+ * convention, no qubit twice in the layer), but any finite nonzero operator is accepted.  Complete: every entry of
+ * sum_i K_i^dagger K_i - I (computed in double, operators in order, K^dagger K summed over rows in ascending order) has
+ * real and imaginary parts within 1e-12.  draws (HOST, n_channels uniforms in [0, 1), one per channel; there is no
+ * sample draw), chosen (HOST, n_channels) and cond (HOST, n_channels, may be NULL) are arrays of the caller; chosen[c]
+ * is the operator chosen for channel c, cond[c] the conditional probability of that choice given the earlier ones as
+ * computed here, and *prob the product of the cond values in channel order.  Monomial layers (every operator
+ * K|b> = d(b)|b ^ f>) are cheaper through qipb200_state_apply_multiqubit_channels (its draws differ: 1 + n).
+ *   1. State-independent channels: every K_i^dagger K_i within 1e-12 (per part) of w_i I, w_i = Tr(K_i^dagger K_i) /
+ *      2^k (mixed-unitary channels: Pauli and depolarizing channels, {sqrt(p_i) P_i U}).  Drawn without reading the
+ *      state: chosen[c] = the rule of step 3 on the w_i, cond[c] = w_i; the operator K / sqrt(w_i) is unitary.
+ *   2. Groups: the other channels, cut in channel order into runs of consecutive ones with at most 4 qubits in all (a
+ *      group closes when the next channel would exceed 4).
+ *   3. Drawing group g on the host in double: rho_g is the reduced density matrix of the group's qubits, indexed in
+ *      the matrix convention over the group's qubits in channel order.  Channel by channel, numerator_i =
+ *      Re Tr[(M_{i_1} (x) .. (x) M_{i_{j-1}} (x) M_i (x) I) rho_g], M = K^dagger K of the choices already made in the
+ *      group and the identity on its later channels, each numerator clamped at 0; S = sum_i numerator_i in order; the
+ *      choice is the smallest i with draw S < sum_{i' <= i} numerator_i', else the last i with numerator_i > 0; cond =
+ *      numerator_i / S.
+ *   4. Sweeps: one read sweep (qipb200_state_reduced_density's kernels) gives rho_1; then one read-write sweep per
+ *      group applies its chosen operators, each as K / sqrt(cond[c]), and accumulates rho_{g+1} from the amplitudes
+ *      as stored (fixed grid and order, no atomics: deterministic).  After the groups, the state-independent channels'
+ *      operators K / sqrt(w_i) run through qipb200_state_apply_schedule as MAT ops in channel order (the planner fuses
+ *      them); a chosen operator that is a positive real multiple of the identity is dropped.  They commute with the
+ *      groups: the qubits are disjoint.
+ *   5. Arithmetic of a group's apply: each scaled operator K' = K * (1 / sqrt(cond)) is computed in double on the host
+ *      and each part rounded once to the state's precision; per channel, in channel order, every fibre x of its
+ *      physical bits (x_b at column b in the matrix convention) becomes y_r = ((t_r0 + t_r1) + t_r2) + ...,
+ *      t_rb = (RN(RN(K'_re x_re) - RN(K'_im x_im)), RN(RN(K'_re x_im) + RN(K'_im x_re))), in the state's precision
+ *      without FMA, columns ascending.  So the state can be reproduced bit for bit from chosen and cond.
+ *   6. When some group finds S = 0 (a zero state, or one that became zero), the call stops there: chosen and cond are
+ *      0 for every channel, *prob = 0, and a zero input state is left untouched.
+ * Errors, all before any device work (a refused call leaves the state and anything pending as they were): NULL state
+ * or prob, NULL arrays with n_channels > 0, an arity not in 1..4, n_kraus not in 1..256, a non-finite entry, the zero
+ * matrix, an incomplete channel (the message names the channel and the matrix entry) and a draw outside [0, 1) give
+ * QIPB200_ERR_INVALID_ARG; a qubit >= n or repeated anywhere in the layer QIPB200_ERR_BAD_INDEX; sharded and
+ * multi-device states QIPB200_ERR_UNSUPPORTED.  n_channels == 0 is a no-op (*prob = 1).  A pending collapse is
+ * applied first and a pending set_basis state written first; a permuted layout is worked on in physical bits.
+ * Synchronises.  qipb200_kraus_channels_plan gives the counts. */
+int qipb200_state_apply_kraus_channels(qipb200_state *state, size_t n_channels, const uint32_t *arity,
+                                       const uint64_t *qubits, const uint32_t *n_kraus, const double *kraus,
+                                       const double *draws, uint32_t *chosen, double *cond, double *prob);
+/* Host-only (no GPU, ctx-free): validates as the call does.  out4 = {groups r, read sweeps (1 if r > 0), read-write
+ * sweeps of the groups (r), kernels of the groups (2r + 1 if r > 0)} on an unsharded n-qubit state with nothing
+ * pending; the passes of the state-independent channels' schedule are not counted.  NULL out4, a bad precision or
+ * n_qubits not in 1..40 give QIPB200_ERR_INVALID_ARG. */
+int qipb200_kraus_channels_plan(qip_prec prec, uint32_t n_qubits, size_t n_channels, const uint32_t *arity,
+                                const uint64_t *qubits, const uint32_t *n_kraus, const double *kraus, uint32_t *out4);
+
 /* Classical functions applied to a register: U |x>|y> = e^{i theta(x)} |x>|y XOR f(x)> for a function given as a table
  * (the row rule of the reference's FunctionOpIterator, qip-iterators/src/iterators/qubit_iterators.rs:221-271, which
  * no MatrixOp reaches): Grover and Shor oracles, modular arithmetic, cost-table phases.

@@ -24,6 +24,7 @@
 #include <optional>
 #include <stdexcept>
 #include <string>
+#include <tuple>
 #include <utility>
 #include <vector>
 
@@ -394,6 +395,20 @@ class B200State {
     ctx_.check(qipb200_state_apply_multiqubit_channels(st_, arity.size(), arity.data(), qubits.data(), n_kraus.data(),
                                                        kraus.data(), draws.data(), chosen.data(), &p));
     return {chosen, p};
+  }
+  // The same for any complete Kraus sets on 1..4 qubits each, one draw per channel; returns (chosen, cond, prob).
+  std::tuple<std::vector<uint32_t>, std::vector<double>, double> apply_kraus_channels(
+      const std::vector<uint32_t> &arity, const std::vector<uint64_t> &qubits, const std::vector<uint32_t> &n_kraus,
+      const std::vector<double> &kraus, const std::vector<double> &draws) {
+    if (n_kraus.size() != arity.size() || draws.size() != arity.size())
+      throw CircuitError("apply_kraus_channels: " + std::to_string(arity.size()) +
+                         " channels need as many n_kraus and draws");
+    std::vector<uint32_t> chosen(arity.size());
+    std::vector<double> cond(arity.size());
+    double p = 0.0;
+    ctx_.check(qipb200_state_apply_kraus_channels(st_, arity.size(), arity.data(), qubits.data(), n_kraus.data(),
+                                                  kraus.data(), draws.data(), chosen.data(), cond.data(), &p));
+    return std::make_tuple(chosen, cond, p);
   }
   // psi <- U psi for U|x>|y> = e^{i theta(x)} |x>|y ^ f(x)>: x on in_qubits, y on out_qubits (absent from the
   // reference's MatrixOp)

@@ -36,6 +36,7 @@ EXPORTS = [
     "qipb200_state_entanglement_spectrum", "qipb200_entanglement_spectrum_plan",
     "qipb200_state_apply_pauli_rotations", "qipb200_pauli_rotation_plan", "qipb200_state_apply_channels",
     "qipb200_channels_plan", "qipb200_state_apply_multiqubit_channels", "qipb200_multiqubit_channels_plan",
+    "qipb200_state_apply_kraus_channels", "qipb200_kraus_channels_plan",
     "qipb200_function_new",
     "qipb200_function_free", "qipb200_state_apply_function", "qipb200_function_plan", "qipb200_function_new_code",
     "qipb200_function_set_params", "qipb200_function_code_compile", "qipb200_function_tabulate",
@@ -175,6 +176,11 @@ def lib():
                                                           C.POINTER(C.c_double)]
     L.qipb200_multiqubit_channels_plan.restype = i32
     L.qipb200_multiqubit_channels_plan.argtypes = [i32, u32, C.c_size_t, vp, vp, vp, vp, vp]
+    L.qipb200_state_apply_kraus_channels.restype = i32
+    L.qipb200_state_apply_kraus_channels.argtypes = [vp, C.c_size_t, vp, vp, vp, vp, vp, vp, vp,
+                                                     C.POINTER(C.c_double)]
+    L.qipb200_kraus_channels_plan.restype = i32
+    L.qipb200_kraus_channels_plan.argtypes = [i32, u32, C.c_size_t, vp, vp, vp, vp, vp]
     L.qipb200_function_new.restype = i32
     L.qipb200_function_new.argtypes = [vp, u32, u32, vp, vp, C.POINTER(vp)]
     L.qipb200_function_free.restype, L.qipb200_function_free.argtypes = None, [vp]

@@ -1,13 +1,15 @@
 """Noise channels on one to four qubits for quantum-trajectory simulation (State.apply_channels,
-State.apply_multiqubit_channels).
+State.apply_multiqubit_channels, State.apply_kraus_channels).
 
 A ``Channel`` on k qubits holds Kraus operators K_i of the form K|b> = d(b)|b ^ f>, one XOR mask f per operator (every
 column has at most one nonzero entry, on the same shifted diagonal; for k = 1 that is diagonal or anti-diagonal), and
 is complete (sum_i K_i^dagger K_i = I to 1e-12).  That covers amplitude and phase damping, every Pauli channel (the two-
 qubit depolarizing channel included), reset, the Z measurement, and their compositions and tensor products, and lets a
 layer of such channels be drawn jointly with one sample of the state (include/qipb200.h:
-qipb200_state_apply_channels, qipb200_state_apply_multiqubit_channels).  Matrices use the qip_op MAT convention: rows
-as outputs, the channel's first qubit the most significant bit of the index."""
+qipb200_state_apply_channels, qipb200_state_apply_multiqubit_channels).  A ``KrausChannel`` holds any complete set of
+Kraus operators (State.apply_kraus_channels: one read sweep plus about one read-write sweep per four qubits of
+state-dependent channels); monomial layers are cheaper as ``Channel``.  Matrices use the qip_op MAT convention: rows as
+outputs, the channel's first qubit the most significant bit of the index."""
 from __future__ import annotations
 
 import itertools
@@ -182,6 +184,115 @@ def two_qubit_depolarizing(p: float) -> Channel:
     """rho -> (1 - p) rho + p/15 sum_{P != II} P rho P: each of the 15 two-qubit Pauli errors with probability p/15."""
     p = float(p)
     return pauli_string_channel({a + b: p / 15 for a, b in itertools.product("IXYZ", repeat=2) if a + b != "II"})
+
+
+def _gram(k):
+    """K^dagger K in double, each entry summed over the rows in ascending order (the library's order)."""
+    D = k.shape[0]
+    m = np.zeros((D, D), dtype=np.complex128)
+    for r in range(D):
+        for c in range(D):
+            re = im = 0.0
+            for a in range(D):
+                x, y = k[a, r], k[a, c]
+                re += float(x.real) * float(y.real) + float(x.imag) * float(y.imag)
+                im += float(x.real) * float(y.imag) - float(x.imag) * float(y.real)
+            m[r, c] = complex(re, im)
+    return m
+
+
+def _trace_weight(m):
+    """Tr(M) / 2^k, the trace summed in ascending order."""
+    t = 0.0
+    for r in range(m.shape[0]):
+        t += float(m[r, r].real)
+    return t / m.shape[0]
+
+
+class KrausChannel:
+    """A channel on k = 1..4 qubits given by ANY complete set of Kraus operators (State.apply_kraus_channels): a
+    sequence of 2^k x 2^k complex matrices in the qip_op MAT convention, or a ``Channel``.  Raises ValueError unless
+    there are 1 to 256 operators, each finite and nonzero, and every entry of sum_i K_i^dagger K_i - I has real and
+    imaginary parts within 1e-12: the checks the library makes.  A single unitary is a valid channel, so a noisy gate
+    is ``KrausChannel([U]).compose(noise)``."""
+
+    def __init__(self, kraus):
+        if isinstance(kraus, (Channel, KrausChannel)):
+            kraus = kraus.kraus
+        mats = [np.asarray(k, dtype=np.complex128) for k in kraus]
+        D = mats[0].shape[-1] if mats else 2
+        if D not in (2, 4, 8, 16) or any(m.shape != (D, D) for m in mats):
+            raise ValueError("KrausChannel: operators must be 2^k x 2^k for k = 1..4, got %r"
+                             % (mats[0].shape if mats else (),))
+        ks = np.array(mats, dtype=np.complex128).reshape(-1, D, D)
+        if not 1 <= ks.shape[0] <= MAX_KRAUS_MULTI:
+            raise ValueError("KrausChannel: 1 to %d Kraus operators, got %d" % (MAX_KRAUS_MULTI, ks.shape[0]))
+        total = np.zeros((D, D), dtype=np.complex128)
+        grams = []
+        for i, k in enumerate(ks):
+            if not np.all(np.isfinite(k.view(np.float64))):
+                raise ValueError("KrausChannel: operator %d has a non-finite entry" % i)
+            if not np.any(k != 0):
+                raise ValueError("KrausChannel: operator %d is the zero matrix" % i)
+            g = _gram(k)
+            grams.append(g)
+            total = total + g
+        dev = total - np.eye(D)
+        for r in range(D):
+            for c in range(D):
+                x = dev[r, c]
+                if not (abs(x.real) <= COMPLETE_TOL and abs(x.imag) <= COMPLETE_TOL):
+                    raise ValueError("KrausChannel: the operators are not complete (entry (%d, %d) of sum K^dagger K"
+                                     " - I is %.3g%+.3gi)" % (r, c, x.real, x.imag))
+        self.kraus = ks
+        self._grams = grams
+
+    def __len__(self):
+        return self.kraus.shape[0]
+
+    def __repr__(self):
+        return "KrausChannel(%d qubits, %d Kraus operators)" % (self.n_qubits, len(self))
+
+    @property
+    def n_qubits(self) -> int:
+        return self.kraus.shape[1].bit_length() - 1
+
+    @property
+    def weights(self):
+        """w_i = Tr(K_i^dagger K_i) / 2^k in double, as the library computes them."""
+        return [_trace_weight(g) for g in self._grams]
+
+    @property
+    def state_independent(self) -> bool:
+        """Every K_i^dagger K_i is within 1e-12 (per part) of w_i I: the choice does not depend on the state (mixed-
+        unitary channels such as Pauli and depolarizing channels, or {sqrt(p_i) P_i U})."""
+        D = self.kraus.shape[1]
+        for g in self._grams:
+            d = g - _trace_weight(g) * np.eye(D)
+            if not (np.all(np.abs(d.real) <= COMPLETE_TOL) and np.all(np.abs(d.imag) <= COMPLETE_TOL)):
+                return False
+        return True
+
+    def compose(self, other) -> "KrausChannel":
+        """This channel, then ``other`` (a KrausChannel or Channel) on the same qubits: the Kraus operators B_j A_i
+        (j major), zero products left out."""
+        other = other if isinstance(other, KrausChannel) else KrausChannel(other)
+        if other.n_qubits != self.n_qubits:
+            raise ValueError("compose: channels on %d and %d qubits" % (self.n_qubits, other.n_qubits))
+        ks = [b @ a for b in other.kraus for a in self.kraus]
+        return KrausChannel([k for k in ks if np.any(k != 0)])
+
+    def tensor(self, other) -> "KrausChannel":
+        """This channel on the first qubits and ``other`` on the ones after them: A_i (x) B_j (i major), at most four
+        qubits in all."""
+        other = other if isinstance(other, KrausChannel) else KrausChannel(other)
+        if self.n_qubits + other.n_qubits > MAX_QUBITS:
+            raise ValueError("tensor: %d + %d qubits, at most 4" % (self.n_qubits, other.n_qubits))
+        return KrausChannel([np.kron(a, b) for a in self.kraus for b in other.kraus])
+
+    def superop(self, rho: np.ndarray) -> np.ndarray:
+        """sum_i K_i rho K_i^dagger on a 2^k x 2^k density matrix (for checks)."""
+        return sum(k @ rho @ k.conj().T for k in self.kraus)
 
 
 def marshal(channels: Sequence[Channel]):

@@ -23,6 +23,7 @@
 #include "dist.cuh"
 #include "expect.h"
 #include "kernels.cuh"
+#include "kraus.h"
 #include "opcompile.h"
 #include "evolve.h"
 #include "lanczos.h"
@@ -2438,6 +2439,159 @@ extern "C" int qipb200_multiqubit_channels_plan(qip_prec prec, uint32_t n_qubits
       st = parse_channel_list(nullptr, who, n_qubits, n_channels, arity, qubits, n_kraus, kraus, &cs);
     if (st != QIPB200_OK) return st;
     plan_channels(cs, out4);
+    return (int)QIPB200_OK;
+  });
+}
+
+// ===================================================================================
+// general Kraus channels along quantum trajectories (kraus.cu)
+// ===================================================================================
+
+namespace {
+
+// K * (1 / sqrt(p)) in double, each part rounded once to the state's precision: 4^k complex<prec>, row-major.
+std::vector<unsigned char> kraus_scaled(qip_prec prec, const double *K, uint32_t k, double p) {
+  const double inv = 1.0 / std::sqrt(p);
+  const size_t E = 2ull << (2 * k);
+  std::vector<unsigned char> out(E * (prec == QIP_F32 ? sizeof(float) : sizeof(double)));
+  for (size_t i = 0; i < E; ++i) {
+    const double v = K[i] * inv;
+    if (prec == QIP_F32)
+      ((float *)out.data())[i] = (float)v;
+    else
+      ((double *)out.data())[i] = v;
+  }
+  return out;
+}
+
+int kraus_impl(qipb200_state *s, const std::string &who, const KrausSet &ks, const double *draws, uint32_t *chosen,
+               double *cond) {
+  qipb200_ctx *ctx = s->ctx;
+  int st = begin_device_work(s);
+  if (st != QIPB200_OK) return st;
+  const size_t nc = ks.size();
+  std::fill(cond, cond + nc, 0.0);
+  std::fill(chosen, chosen + nc, 0u);
+  // the rdm positions of a group: bit i of the matrix index <-> its (m - 1 - i)-th qubit, so that the index is in
+  // the matrix convention over the group's qubits in channel order
+  auto group_pos = [&](const std::vector<size_t> &g, uint32_t *pos) {
+    std::vector<uint64_t> q;
+    for (size_t c : g) q.insert(q.end(), ks.qubits.begin() + ks.qfirst[c], ks.qubits.begin() + ks.qfirst[c + 1]);
+    std::reverse(q.begin(), q.end());
+    phys_positions(s, q.data(), (uint32_t)q.size(), pos);
+    return (uint32_t)q.size();
+  };
+  const std::vector<std::vector<size_t>> groups = kraus_groups(ks);
+  if (!groups.empty()) {
+    std::vector<double> rho(2 << (2 * kKrausGroupBits));
+    uint32_t pos[kKrausGroupBits];
+    uint32_t m = group_pos(groups[0], pos);
+    CU(ctx, run_reduced_density(s->prec, s->buf, s->n_local, pos, m, rho.data(), ctx->stream, &ctx->launches));
+    char *d = nullptr;
+    CU(ctx, cudaMallocAsync((void **)&d, kraus_scratch_bytes(), ctx->stream));
+    cudaError_t e = cudaSuccess;
+    bool zero = false;
+    for (size_t gi = 0; gi < groups.size() && e == cudaSuccess; ++gi) {
+      if (!kraus_draw_group(ks, groups[gi], rho.data(), draws, chosen, cond)) {  // Tr rho = 0: a zero state
+        zero = true;
+        break;
+      }
+      std::vector<KrausApplyOp> ops;
+      for (size_t c : groups[gi]) {
+        KrausApplyOp o;
+        o.k = ks.arity(c);
+        phys_positions(s, ks.qubits.data() + ks.qfirst[c], o.k, o.pos);
+        o.mat = kraus_scaled(s->prec, ks.mat[ks.first[c] + chosen[c]], o.k, cond[c]);
+        ops.push_back(std::move(o));
+      }
+      m = gi + 1 < groups.size() ? group_pos(groups[gi + 1], pos) : 0;
+      e = run_kraus_sweep(s->prec, s->buf, s->n_local, ops, pos, m, rho.data(), d, ctx->stream, &ctx->launches);
+    }
+    const cudaError_t ef = cudaFreeAsync(d, ctx->stream);
+    if (e != cudaSuccess) return cuda_fail(ctx, e, who.c_str());
+    CU(ctx, ef);
+    if (zero) {
+      std::fill(cond, cond + nc, 0.0);
+      std::fill(chosen, chosen + nc, 0u);
+      CU(ctx, cudaStreamSynchronize(ctx->stream));
+      return QIPB200_OK;
+    }
+  }
+  // the state-independent channels: drawn from their weights, K / sqrt(w) through the fused schedule
+  std::vector<qip_op> sched;
+  std::vector<std::vector<unsigned char>> dense;
+  dense.reserve(nc);
+  for (size_t c = 0; c < nc; ++c) {
+    if (!ks.indep[c]) continue;
+    const uint32_t f = ks.first[c], k = ks.arity(c);
+    chosen[c] = kraus_choose(ks.w.data() + f, ks.first[c + 1] - f, draws[c]);
+    cond[c] = ks.w[f + chosen[c]];
+    const double *K = ks.mat[f + chosen[c]];
+    if (kraus_is_scaled_identity(K, k)) continue;
+    dense.push_back(kraus_scaled(s->prec, K, k, cond[c]));
+    qip_op op;
+    memset(&op, 0, sizeof(op));
+    op.kind = QIP_OP_MATRIX;
+    op.n_indices = k;
+    op.n_entries = 1ull << (2 * k);
+    op.indices = ks.qubits.data() + ks.qfirst[c];
+    op.dense = dense.back().data();
+    sched.push_back(op);
+  }
+  if (!sched.empty() && (st = qipb200_state_apply_schedule(s, sched.data(), sched.size(), 0)) != QIPB200_OK)
+    return st;
+  CU(ctx, cudaStreamSynchronize(ctx->stream));
+  return QIPB200_OK;
+}
+
+}  // namespace
+
+extern "C" int qipb200_state_apply_kraus_channels(qipb200_state *s, size_t n_channels, const uint32_t *arity,
+                                                  const uint64_t *qubits, const uint32_t *n_kraus,
+                                                  const double *kraus, const double *draws, uint32_t *chosen,
+                                                  double *cond, double *prob) {
+  const std::string who = "apply_kraus_channels";
+  if (!s) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, who + ": NULL state");
+  return guarded(s->ctx, [&]() -> int {
+    // every check runs before any device work: a refused call leaves the state (and a pending collapse) as it was
+    if (!prob) return set_err(s->ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL prob");
+    if (n_channels && (!draws || !chosen))
+      return set_err(s->ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL draws or chosen");
+    KrausSet ks;
+    std::string err;
+    int st = parse_kraus_channels(who, s->n, n_channels, arity, qubits, n_kraus, kraus, &ks, &err);
+    if (st != QIPB200_OK) return set_err(s->ctx, st, err);
+    for (size_t k = 0; k < n_channels; ++k)
+      if (!(draws[k] >= 0.0 && draws[k] < 1.0))
+        return set_err(s->ctx, QIPB200_ERR_INVALID_ARG, who + ": draw " + std::to_string(k) + " is not in [0, 1)");
+    if ((st = require_unsharded(s, who)) != QIPB200_OK) return st;
+    if (n_channels == 0) {
+      *prob = 1.0;
+      return (int)QIPB200_OK;
+    }
+    std::vector<double> cd(n_channels, 0.0);
+    if ((st = kraus_impl(s, who, ks, draws, chosen, cd.data())) != QIPB200_OK) return st;
+    double p = 1.0;
+    for (size_t c = 0; c < n_channels; ++c) p *= cd[c];
+    *prob = p;
+    if (cond) std::copy(cd.begin(), cd.end(), cond);
+    return (int)QIPB200_OK;
+  });
+}
+
+extern "C" int qipb200_kraus_channels_plan(qip_prec prec, uint32_t n_qubits, size_t n_channels,
+                                           const uint32_t *arity, const uint64_t *qubits, const uint32_t *n_kraus,
+                                           const double *kraus, uint32_t *out4) {
+  const std::string who = "kraus_channels_plan";
+  return guarded(nullptr, [&]() -> int {
+    KrausSet ks;
+    std::string err;
+    int st = check_plan_args(who, prec, n_qubits, out4, "out4");
+    if (st != QIPB200_OK) return st;
+    if ((st = parse_kraus_channels(who, n_qubits, n_channels, arity, qubits, n_kraus, kraus, &ks, &err)) !=
+        QIPB200_OK)
+      return set_err(nullptr, st, err);
+    plan_kraus_channels(ks, out4);
     return (int)QIPB200_OK;
   });
 }

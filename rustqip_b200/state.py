@@ -376,6 +376,33 @@ class State:
             _ptr(kraus) if nc else None, _ptr(r), _ptr(chosen), C.byref(prob)))
         return chosen[:nc], float(prob.value)
 
+    def apply_kraus_channels(self, channels, qubit_groups, rng=None, draws=None):
+        """One quantum-trajectory step of channels with any complete Kraus sets on one to four qubits each, no qubit
+        twice in the layer, computed on the device.  Returns (chosen, cond, prob): chosen[c] indexes the operator of
+        channel c, cond[c] is the probability of that choice given the earlier ones, prob their product.
+
+        ``qubit_groups[c]`` lists the qubits of channel c, its first qubit the most significant bit of the channel's
+        matrices; ``channels`` is one ``channels.KrausChannel`` (or ``Channel``) for every group or one per group.
+        ``draws`` are len(qubit_groups) uniforms in [0, 1), one per channel; without them they are drawn from ``rng``.
+        State-independent channels (mixed-unitary ones) are drawn without reading the state and applied through
+        ``apply_schedule``; the others cost one read sweep plus one read-write sweep per group of at most four qubits
+        (``kraus_channels_plan``).  Monomial layers are cheaper through ``apply_multiqubit_channels``.  Synchronises."""
+        chans, qa = _kraus_groups("apply_kraus_channels", channels, qubit_groups)
+        arity, n_kraus, kraus = _ch_marshal(chans)
+        nc = len(chans)
+        if draws is None:
+            draws = (rng if rng is not None else np.random.default_rng()).random(nc)
+        r = np.ascontiguousarray(np.asarray(draws, dtype=np.float64).reshape(-1))
+        if r.shape[0] != nc:
+            raise ValueError("apply_kraus_channels: %d channels need %d draws, got %d" % (nc, nc, r.shape[0]))
+        chosen = np.zeros(max(1, nc), dtype=np.uint32)
+        cond = np.zeros(max(1, nc), dtype=np.float64)
+        prob = C.c_double()
+        self._chk(_lib.lib().qipb200_state_apply_kraus_channels(
+            self._h, nc, _ptr(arity) if nc else None, _ptr(qa) if nc else None, _ptr(n_kraus) if nc else None,
+            _ptr(kraus) if nc else None, _ptr(r) if nc else None, _ptr(chosen), _ptr(cond), C.byref(prob)))
+        return chosen[:nc], cond[:nc], float(prob.value)
+
     def apply_function(self, fn: "Function", in_qubits: Sequence[int], out_qubits: Sequence[int] = ()):
         """Apply U|x>|y> = e^{i theta(x)} |x>|y XOR f(x)> of ``fn`` on the device: bit i of x is the value of qubit
         ``in_qubits[i]`` and bit i of f(x) is XORed into qubit ``out_qubits[i]`` (the convention of
@@ -763,6 +790,31 @@ def multiqubit_channels_plan(n: int, dtype, channels, qubit_groups):
     v = (C.c_uint32 * 4)()
     k = len(chans)
     _lib.check(_lib.lib().qipb200_multiqubit_channels_plan(
+        prec_of(dtype), int(n), k, _ptr(arity) if k else None, _ptr(qa) if k else None,
+        _ptr(n_kraus) if k else None, _ptr(kraus) if k else None, v), None)
+    return tuple(int(x) for x in v)
+
+
+def _kraus_groups(who, channels, qubit_groups):
+    """(KrausChannels, flat uint64 qubits) of a Kraus layer; one channel stands for every group, and a Channel is
+    taken as the KrausChannel of its operators."""
+    from . import channels as _ch
+    qubit_groups = [list(g) for g in qubit_groups]
+    one = isinstance(channels, (_ch.Channel, _ch.KrausChannel))
+    chans = [channels] * len(qubit_groups) if one else list(channels)
+    chans = [c if isinstance(c, _ch.KrausChannel) else _ch.KrausChannel(c) for c in chans]
+    return _channel_groups(who, chans, qubit_groups)
+
+
+def kraus_channels_plan(n: int, dtype, channels, qubit_groups):
+    """(groups r, read sweeps, read-write sweeps, kernels) of State.apply_kraus_channels on an unsharded n-qubit state
+    with nothing pending (needs no GPU); the state-independent channels' schedule is not counted.  Validates as the
+    call does."""
+    chans, qa = _kraus_groups("kraus_channels_plan", channels, qubit_groups)
+    arity, n_kraus, kraus = _ch_marshal(chans)
+    v = (C.c_uint32 * 4)()
+    k = len(chans)
+    _lib.check(_lib.lib().qipb200_kraus_channels_plan(
         prec_of(dtype), int(n), k, _ptr(arity) if k else None, _ptr(qa) if k else None,
         _ptr(n_kraus) if k else None, _ptr(kraus) if k else None, v), None)
     return tuple(int(x) for x in v)
