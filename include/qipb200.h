@@ -530,6 +530,69 @@ int qipb200_state_apply_kraus_channels(qipb200_state *state, size_t n_channels, 
 int qipb200_kraus_channels_plan(qip_prec prec, uint32_t n_qubits, size_t n_channels, const uint32_t *arity,
                                 const uint64_t *qubits, const uint32_t *n_kraus, const double *kraus, uint32_t *out4);
 
+/* ---- Exact noisy simulation on density matrices (absent in the reference) ------------------------------------------
+ * The exact mixed state of a noisy circuit, where the trajectory calls above give one pure sample: purity, entropy
+ * and fidelity are not averages of trajectory quantities, and effects of 1e-3 noise are below the statistical error
+ * of thousands of trajectories.
+ * Representation: a density matrix rho of n >= 1 qubits is a qipb200_state of 2n qubits (no new handle).  Row qubit q
+ * is state qubit q and column qubit q is state qubit n + q, so in the qip_op convention rho_rc is the amplitude at
+ * index r * 2^n + c: rows are contiguous and the downloaded vector, read as a row-major 2^n x 2^n matrix, is rho.
+ * |i><i| is qipb200_state_set_basis(rho, i * 2^n + i) (it stays pending: the first fused pass is load-free), and
+ * Tr rho^2 = sum |rho_rc|^2 is qipb200_state_norm2 of the vector for Hermitian rho.  The qipb200_state_* entries keep
+ * their meaning on the raw vector.  The qipb200_density_* entries take the 2n-qubit state: an odd qubit count gives
+ * QIPB200_ERR_INVALID_ARG, sharded and multi-device states QIPB200_ERR_UNSUPPORTED; all checks run before any device
+ * work, so a refused call leaves rho (and anything pending on it) as it was.  A pending set_basis or collapse is
+ * applied first, and a permuted layout (QIPB200_ROTATE) is read where it is.  The readouts synchronise; those computed
+ * by this library's kernels are deterministic (fixed grids and orders, no atomics); the spectrum's eigen-solve is
+ * cuSOLVER's, whose bits are not promised to repeat. */
+
+/* Gates and channels, interleaved, in one fused schedule on vec(rho).  Channel c runs after ops[0 .. channel_pos[c]);
+ * channels at one position run in channel order; channel_pos is non-decreasing and at most n_ops.  Channels are
+ * encoded and checked as for qipb200_state_apply_kraus_channels (arity 1..4, 1..256 operators, complete to 1e-12),
+ * except that a qubit may appear in several channels: they run one after the other.  Ops are checked by
+ * qipb200_validate_op on n qubits.  The doubled schedule: each op, then its conjugate on the column qubits (every
+ * index + n, MAT and sparse values conjugated, Swap and Control structure unchanged); each channel one MAT op on
+ * [q_1..q_k, q_1 + n..q_k + n] with S = sum_i kron(K_i, conj K_i), formed in double, terms added in ascending i, each
+ * part rounded once to the state's precision.  It runs through qipb200_state_apply_schedule with flags, so the result
+ * is bit-identical to that call on the schedule qipb200_density_schedule writes when both run the same kernels (with
+ * the default QIPB200_JIT=async a pass may run on the interpreter kernel while its generated kernel compiles, and the
+ * two may round differently).  Errors: QIPB200_ERR_INVALID_ARG for
+ * NULL arrays, a bad channel_pos and the channel refusals of apply_kraus_channels; a qubit >= n gives
+ * QIPB200_ERR_BAD_INDEX (channels) or validate_op's status (ops). */
+int qipb200_density_apply(qipb200_state *rho, const qip_op *ops, size_t n_ops, size_t n_channels,
+                          const uint64_t *channel_pos, const uint32_t *arity, const uint64_t *qubits,
+                          const uint32_t *n_kraus, const double *kraus, uint32_t flags);
+/* Host-only (no GPU, ctx-free): checks as qipb200_density_apply does for an n-qubit rho (n in 1..20, a known
+ * precision) and writes the doubled schedule in the QIPS v1 format (n_qubits = 2n) to buf.  *len is set to the size;
+ * when buf is NULL or cap is smaller the call returns QIPB200_ERR_SIZE_MISMATCH.  A Rust or C caller exports a noisy
+ * circuit with it. */
+int qipb200_density_schedule(qip_prec prec, uint32_t n, const qip_op *ops, size_t n_ops, size_t n_channels,
+                             const uint64_t *channel_pos, const uint32_t *arity, const uint64_t *qubits,
+                             const uint32_t *n_kraus, const double *kraus, void *buf, size_t cap, size_t *len);
+/* rho = |psi><psi| (not normalised): psi has n qubits, rho's context and precision, and is unsharded (else
+ * QIPB200_ERR_SIZE_MISMATCH / QIPB200_ERR_UNSUPPORTED).  rho's pending work is dropped and its layout becomes the
+ * canonical one; a permuted psi is restored first.  One write sweep of rho. */
+int qipb200_density_from_state(qipb200_state *rho, qipb200_state *psi);
+/* out[m] = sum of Re rho_rr over the r whose bits on indices equal m; bit i of m is indices[i] (the convention of
+ * qipb200_state_measure_probs); n_indices = 0 gives out[0] = Tr rho.  Reads only the 2^n diagonal entries.  A qubit
+ * >= n or repeated gives QIPB200_ERR_BAD_INDEX. */
+int qipb200_density_measure_probs(qipb200_state *rho, const uint64_t *indices, uint32_t n_indices, double *out);
+/* out[t] = Re Tr(rho P_t) for Pauli strings encoded and checked as for qipb200_state_expect_paulis on n qubits.  Each
+ * term gathers 2^n entries of rho; up to 4096 terms per launch. */
+int qipb200_density_expect_paulis(qipb200_state *rho, const uint64_t *qubits, const char *paulis,
+                                  const uint32_t *term_len, size_t n_terms, double *out);
+/* rho_A = Tr_B rho for k = 1..min(n, 10) kept qubits: out is row-major 2^k x 2^k, interleaved re/im, bit i of the
+ * indices the value of qubits[i] (the layout of qipb200_state_reduced_density).  Exactly Hermitian: the entries a <= a'
+ * are summed and mirrored, the diagonal's imaginary part is 0.0.  k > 10 gives QIPB200_ERR_UNSUPPORTED. */
+int qipb200_density_reduced(qipb200_state *rho, const uint64_t *qubits, uint32_t k, double *out);
+/* out2 = {Re, Im} <psi|rho|psi>, psi as for qipb200_density_from_state.  One read sweep of rho, accumulated in double;
+ * the fidelity of a normalised rho with a unit vector psi is out2[0]. */
+int qipb200_density_fidelity(qipb200_state *rho, qipb200_state *psi, double *out2);
+/* The 2^n eigenvalues of rho in descending order into eigs (HOST, 2^n doubles), for n <= 13 (else
+ * QIPB200_ERR_UNSUPPORTED): rho is widened to double on the device and solved by cuSOLVER (as
+ * qipb200_state_entanglement_spectrum); when cuSOLVER cannot be loaded the call returns QIPB200_ERR_UNSUPPORTED. */
+int qipb200_density_spectrum(qipb200_state *rho, double *eigs);
+
 /* Classical functions applied to a register: U |x>|y> = e^{i theta(x)} |x>|y XOR f(x)> for a function given as a table
  * (the row rule of the reference's FunctionOpIterator, qip-iterators/src/iterators/qubit_iterators.rs:221-271, which
  * no MatrixOp reaches): Grover and Shor oracles, modular arithmetic, cost-table phases.

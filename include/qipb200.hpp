@@ -410,6 +410,53 @@ class B200State {
                                                   kraus.data(), draws.data(), chosen.data(), cond.data(), &p));
     return std::make_tuple(chosen, cond, p);
   }
+  // ---- this state as the vec of an n-qubit density matrix (2n qubits; rho_rc at index r 2^n + c) ----
+  // gates and channels interleaved in one fused schedule: channel c runs after ops[0 .. channel_pos[c]), channels
+  // encoded as for apply_kraus_channels (a qubit may appear in several)
+  void density_apply(const std::vector<qip_op> &ops, const std::vector<uint64_t> &channel_pos,
+                     const std::vector<uint32_t> &arity, const std::vector<uint64_t> &qubits,
+                     const std::vector<uint32_t> &n_kraus, const std::vector<double> &kraus, bool fusion = true) {
+    if (channel_pos.size() != arity.size() || n_kraus.size() != arity.size())
+      throw CircuitError("density_apply: " + std::to_string(arity.size()) +
+                         " channels need as many positions and n_kraus");
+    ctx_.check(qipb200_density_apply(st_, ops.data(), ops.size(), arity.size(), channel_pos.data(), arity.data(),
+                                     qubits.data(), n_kraus.data(), kraus.data(),
+                                     fusion ? QIPB200_SCHED_DEFAULT : QIPB200_SCHED_NO_FUSION));
+  }
+  // rho = |psi><psi| for a state psi of n qubits
+  void density_from_state(const B200State &psi) { ctx_.check(qipb200_density_from_state(st_, psi.st_)); }
+  // out[m] = sum of rho_rr over the r whose bits on indices equal m (bit i of m is indices[i])
+  std::vector<double> density_measure_probs(const std::vector<uint64_t> &indices) {
+    std::vector<double> out(1ull << indices.size());
+    ctx_.check(qipb200_density_measure_probs(st_, indices.empty() ? nullptr : indices.data(),
+                                             (uint32_t)indices.size(), out.data()));
+    return out;
+  }
+  // Re Tr(rho P_t), terms as for expect_paulis
+  std::vector<double> density_expect_paulis(const std::vector<std::vector<std::pair<char, uint64_t>>> &terms) {
+    Flat f(terms);
+    std::vector<double> out(terms.size());
+    ctx_.check(qipb200_density_expect_paulis(st_, f.q(), f.l(), f.lens.data(), terms.size(), out.data()));
+    return out;
+  }
+  // rho_A of 1..10 kept qubits: row-major 2^k x 2^k complex values
+  std::vector<std::complex<double>> density_reduced(const std::vector<uint64_t> &qubits) {
+    std::vector<std::complex<double>> out(1ull << (2 * std::min<size_t>(qubits.size(), 10)));
+    ctx_.check(qipb200_density_reduced(st_, qubits.data(), (uint32_t)qubits.size(), (double *)out.data()));
+    return out;
+  }
+  // <psi|rho|psi>
+  std::complex<double> density_fidelity(const B200State &psi) {
+    double out2[2] = {0.0, 0.0};
+    ctx_.check(qipb200_density_fidelity(st_, psi.st_, out2));
+    return {out2[0], out2[1]};
+  }
+  // the 2^n eigenvalues of rho, descending (n <= 13)
+  std::vector<double> density_spectrum(uint32_t n) {
+    std::vector<double> eigs(1ull << std::min<uint32_t>(n, 13));
+    ctx_.check(qipb200_density_spectrum(st_, eigs.data()));
+    return eigs;
+  }
   // psi <- U psi for U|x>|y> = e^{i theta(x)} |x>|y ^ f(x)>: x on in_qubits, y on out_qubits (absent from the
   // reference's MatrixOp)
   void apply_function(const B200Function &fn, const std::vector<uint64_t> &in_qubits,

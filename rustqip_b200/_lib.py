@@ -19,6 +19,7 @@ SCHED_DEFAULT = 0
 SCHED_NO_FUSION = 1
 MEASURE_FORCED = 1
 MEASURE_FORCED_PROB = 2
+ERR_SIZE_MISMATCH = 2
 
 _lib = None
 
@@ -37,6 +38,8 @@ EXPORTS = [
     "qipb200_state_apply_pauli_rotations", "qipb200_pauli_rotation_plan", "qipb200_state_apply_channels",
     "qipb200_channels_plan", "qipb200_state_apply_multiqubit_channels", "qipb200_multiqubit_channels_plan",
     "qipb200_state_apply_kraus_channels", "qipb200_kraus_channels_plan",
+    "qipb200_density_apply", "qipb200_density_schedule", "qipb200_density_from_state", "qipb200_density_measure_probs",
+    "qipb200_density_expect_paulis", "qipb200_density_reduced", "qipb200_density_fidelity", "qipb200_density_spectrum",
     "qipb200_function_new",
     "qipb200_function_free", "qipb200_state_apply_function", "qipb200_function_plan", "qipb200_function_new_code",
     "qipb200_function_set_params", "qipb200_function_code_compile", "qipb200_function_tabulate",
@@ -181,6 +184,19 @@ def lib():
                                                      C.POINTER(C.c_double)]
     L.qipb200_kraus_channels_plan.restype = i32
     L.qipb200_kraus_channels_plan.argtypes = [i32, u32, C.c_size_t, vp, vp, vp, vp, vp]
+    sz = C.c_size_t
+    L.qipb200_density_apply.restype = i32
+    L.qipb200_density_apply.argtypes = [vp, opp, sz, sz, vp, vp, vp, vp, vp, u32]
+    L.qipb200_density_schedule.restype = i32
+    L.qipb200_density_schedule.argtypes = [i32, u32, opp, sz, sz, vp, vp, vp, vp, vp, vp, sz, C.POINTER(sz)]
+    L.qipb200_density_from_state.restype, L.qipb200_density_from_state.argtypes = i32, [vp, vp]
+    L.qipb200_density_measure_probs.restype = i32
+    L.qipb200_density_measure_probs.argtypes = [vp, vp, u32, vp]
+    L.qipb200_density_expect_paulis.restype = i32
+    L.qipb200_density_expect_paulis.argtypes = [vp, vp, vp, vp, sz, vp]
+    L.qipb200_density_reduced.restype, L.qipb200_density_reduced.argtypes = i32, [vp, vp, u32, vp]
+    L.qipb200_density_fidelity.restype, L.qipb200_density_fidelity.argtypes = i32, [vp, vp, vp]
+    L.qipb200_density_spectrum.restype, L.qipb200_density_spectrum.argtypes = i32, [vp, vp]
     L.qipb200_function_new.restype = i32
     L.qipb200_function_new.argtypes = [vp, u32, u32, vp, vp, C.POINTER(vp)]
     L.qipb200_function_free.restype, L.qipb200_function_free.argtypes = None, [vp]

@@ -69,6 +69,23 @@ def random_circuit(n: int, depth: int, seed: int, gate_set: str = "H,T,CNOT") ->
     return h_layer(n) + random_layers(seed, n, depth, oneq, twoq)
 
 
+def noisy_random_circuit(n: int, depth: int, seed: int, gamma: float = 1e-3, lam: float = 1e-3,
+                         cnot_depolarizing: float = 0.0) -> list:
+    """Items of DensityMatrix.apply: H on every qubit, then `depth` random {H, T, CNOT} layers (layer l generated as
+    random_layers(seed + l, n, 1, ...)), each followed by amplitude damping (gamma) and dephasing (lam) on every qubit;
+    with cnot_depolarizing > 0, two-qubit depolarizing noise follows each CNOT."""
+    from . import channels as ch
+    damp, deph = ch.amplitude_damping(gamma), ch.phase_damping(lam)
+    items: list = h_layer(n)
+    for layer in range(depth):
+        for op in random_layers(seed + layer, n, 1, [gates.h, gates.t], [gates.cnot]):
+            items.append(op)
+            if cnot_depolarizing > 0 and op.kind == "control":
+                items.append((ch.two_qubit_depolarizing(cnot_depolarizing), op.indices()))
+        items += [(damp, [q]) for q in range(n)] + [(deph, [q]) for q in range(n)]
+    return items
+
+
 def config2(n: int = 28, depth: int = 40) -> List[MatrixOp]:
     return random_circuit(n, depth, 0x5EED0002, "H,T,CNOT")
 

@@ -20,6 +20,7 @@
 
 #include "../../include/qipb200.h"
 #include "channel.h"
+#include "density.h"
 #include "dist.cuh"
 #include "expect.h"
 #include "kernels.cuh"
@@ -2592,6 +2593,264 @@ extern "C" int qipb200_kraus_channels_plan(qip_prec prec, uint32_t n_qubits, siz
         QIPB200_OK)
       return set_err(nullptr, st, err);
     plan_kraus_channels(ks, out4);
+    return (int)QIPB200_OK;
+  });
+}
+
+// ===================================================================================
+// density matrices (density.cu)
+// ===================================================================================
+
+namespace {
+
+// The n of a density matrix held by rho (2n qubits), or the refusal: a sharded state, an odd qubit count.
+int density_qubits(const qipb200_state *rho, const std::string &who, uint32_t *n) {
+  int st = require_unsharded(rho, who);
+  if (st != QIPB200_OK) return st;
+  if (rho->n % 2)
+    return set_err(rho->ctx, QIPB200_ERR_INVALID_ARG,
+                   who + ": a density matrix is a state of an even number of qubits, got " + std::to_string(rho->n));
+  *n = rho->n / 2;
+  return QIPB200_OK;
+}
+
+// psi of n qubits in rho's context and precision, unsharded.
+int density_check_psi(const qipb200_state *rho, const qipb200_state *psi, uint32_t n, const std::string &who) {
+  if (psi->ctx != rho->ctx || psi->prec != rho->prec || psi->n != n)
+    return set_err(rho->ctx, QIPB200_ERR_SIZE_MISMATCH,
+                   who + ": psi must have the density matrix's context and precision and " + std::to_string(n) +
+                       " qubits");
+  return require_unsharded(psi, who);
+}
+
+// psi's pending work applied and its qubits back in the canonical layout.
+int density_prepare_psi(qipb200_state *psi) {
+  int st = materialise_pending(psi);
+  if (st == QIPB200_OK && !layout_is_identity(psi)) st = restore_layout(psi);
+  return st;
+}
+
+// k distinct qubits below n (k == 0 allowed when zero_ok).
+int density_check_qubits(const qipb200_state *rho, const std::string &who, uint32_t n, const uint64_t *qubits,
+                         uint32_t k, bool zero_ok) {
+  if ((k && !qubits) || (!zero_ok && k == 0) || k > n)
+    return set_err(rho->ctx, QIPB200_ERR_INVALID_ARG, who + ": bad qubit list");
+  uint64_t seen = 0;
+  for (uint32_t i = 0; i < k; ++i) {
+    if (qubits[i] >= n) return set_err(rho->ctx, QIPB200_ERR_BAD_INDEX, who + ": qubit index out of range");
+    if ((seen >> qubits[i]) & 1) return set_err(rho->ctx, QIPB200_ERR_BAD_INDEX, who + ": repeated qubit index");
+    seen |= 1ull << qubits[i];
+  }
+  return QIPB200_OK;
+}
+
+// Physical index bits of row qubit q (state qubit q) and of column qubit q (state qubit n + q).
+uint64_t row_bit(const qipb200_state *rho, uint32_t n, uint64_t q) { return 1ull << rho->phys_of_logical[2 * n - 1 - q]; }
+uint64_t col_bit(const qipb200_state *rho, uint32_t n, uint64_t q) { return 1ull << rho->phys_of_logical[n - 1 - q]; }
+
+// The traced qubits (every qubit not in qubits[0..k)), ascending: the low key bits of run_density_sums.
+std::vector<uint64_t> density_trace_masks(const qipb200_state *rho, uint32_t n, const uint64_t *qubits, uint32_t k) {
+  uint64_t kept = 0;
+  for (uint32_t i = 0; i < k; ++i) kept |= 1ull << qubits[i];
+  std::vector<uint64_t> m;
+  for (uint32_t q = 0; q < n; ++q)
+    if (!((kept >> q) & 1)) m.push_back(row_bit(rho, n, q) | col_bit(rho, n, q));
+  return m;
+}
+
+}  // namespace
+
+extern "C" int qipb200_density_apply(qipb200_state *rho, const qip_op *ops, size_t n_ops, size_t n_channels,
+                                     const uint64_t *channel_pos, const uint32_t *arity, const uint64_t *qubits,
+                                     const uint32_t *n_kraus, const double *kraus, uint32_t flags) {
+  const std::string who = "density_apply";
+  if (!rho) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, who + ": NULL state");
+  return guarded(rho->ctx, [&]() -> int {
+    // every check runs before any device work: a refused call leaves rho (and anything pending) as it was
+    uint32_t n = 0;
+    int st = density_qubits(rho, who, &n);
+    if (st != QIPB200_OK) return st;
+    DensitySchedule d;
+    std::string err;
+    st = build_density_schedule(who, rho->prec, n, ops, n_ops, n_channels, channel_pos, arity, qubits, n_kraus, kraus,
+                                &d, &err);
+    if (st != QIPB200_OK) return set_err(rho->ctx, st, err);
+    return qipb200_state_apply_schedule(rho, d.ops.data(), d.ops.size(), flags);
+  });
+}
+
+extern "C" int qipb200_density_schedule(qip_prec prec, uint32_t n, const qip_op *ops, size_t n_ops, size_t n_channels,
+                                        const uint64_t *channel_pos, const uint32_t *arity, const uint64_t *qubits,
+                                        const uint32_t *n_kraus, const double *kraus, void *buf, size_t cap,
+                                        size_t *len) {
+  const std::string who = "density_schedule";
+  return guarded(nullptr, [&]() -> int {
+    if (!len) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, who + ": NULL len");
+    DensitySchedule d;
+    std::string err;
+    int st = build_density_schedule(who, prec, n, ops, n_ops, n_channels, channel_pos, arity, qubits, n_kraus, kraus,
+                                    &d, &err);
+    if (st != QIPB200_OK) return set_err(nullptr, st, err);
+    const size_t need = qipb200_schedule_serialise(prec, 2 * n, d.ops.data(), d.ops.size(), nullptr, 0);
+    if (need == 0) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, who + ": the schedule could not be written");
+    *len = need;
+    if (!buf || cap < need)
+      return set_err(nullptr, QIPB200_ERR_SIZE_MISMATCH,
+                     who + ": the schedule needs " + std::to_string(need) + " bytes, cap is " + std::to_string(cap));
+    qipb200_schedule_serialise(prec, 2 * n, d.ops.data(), d.ops.size(), buf, cap);
+    return (int)QIPB200_OK;
+  });
+}
+
+extern "C" int qipb200_density_from_state(qipb200_state *rho, qipb200_state *psi) {
+  const std::string who = "density_from_state";
+  if (!rho || !psi) return set_err(rho ? rho->ctx : nullptr, QIPB200_ERR_INVALID_ARG, who + ": NULL state");
+  return guarded(rho->ctx, [&]() -> int {
+    uint32_t n = 0;
+    int st = density_qubits(rho, who, &n);
+    if (st == QIPB200_OK) st = density_check_psi(rho, psi, n, who);
+    if (st != QIPB200_OK) return st;
+    qipb200_ctx *ctx = rho->ctx;
+    CU(ctx, cudaSetDevice(ctx->device));
+    if ((st = density_prepare_psi(psi)) != QIPB200_OK) return st;
+    // every amplitude of rho is written: its pending work is dropped and its layout becomes the canonical one
+    rho->collapse_pending = rho->init_pending = false;
+    for (uint32_t b = 0; b < rho->n; ++b) rho->phys_of_logical[b] = b;
+    CU(ctx, run_density_from_state(rho->prec, rho->buf, psi->buf, n, ctx->stream, &ctx->launches));
+    CU(ctx, cudaStreamSynchronize(ctx->stream));
+    return (int)QIPB200_OK;
+  });
+}
+
+extern "C" int qipb200_density_measure_probs(qipb200_state *rho, const uint64_t *indices, uint32_t n_indices,
+                                             double *out) {
+  const std::string who = "density_measure_probs";
+  if (!rho) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, who + ": NULL state");
+  return guarded(rho->ctx, [&]() -> int {
+    uint32_t n = 0;
+    int st = density_qubits(rho, who, &n);
+    if (st == QIPB200_OK) st = density_check_qubits(rho, who, n, indices, n_indices, true);
+    if (st != QIPB200_OK) return st;
+    if (!out) return set_err(rho->ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL out");
+    qipb200_ctx *ctx = rho->ctx;
+    if ((st = begin_device_work(rho)) != QIPB200_OK) return st;
+    std::vector<uint64_t> masks = density_trace_masks(rho, n, indices, n_indices);
+    const uint32_t nb = (uint32_t)masks.size();
+    for (uint32_t i = 0; i < n_indices; ++i) masks.push_back(row_bit(rho, n, indices[i]) | col_bit(rho, n, indices[i]));
+    std::vector<double> sums(2ull << n_indices);
+    CU(ctx, run_density_sums(rho->prec, rho->buf, masks, nb, n_indices, 0, sums.data(), ctx->stream, &ctx->launches));
+    for (size_t m = 0; m < (1ull << n_indices); ++m) out[m] = sums[2 * m];
+    return (int)QIPB200_OK;
+  });
+}
+
+extern "C" int qipb200_density_expect_paulis(qipb200_state *rho, const uint64_t *qubits, const char *paulis,
+                                             const uint32_t *term_len, size_t n_terms, double *out) {
+  const std::string who = "density_expect_paulis";
+  if (!rho) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, who + ": NULL state");
+  return guarded(rho->ctx, [&]() -> int {
+    uint32_t n = 0;
+    int st = density_qubits(rho, who, &n);
+    std::vector<PauliTerm> terms;
+    if (st == QIPB200_OK) st = parse_terms(rho->ctx, n, qubits, paulis, term_len, n_terms, &terms);
+    if (st != QIPB200_OK) return st;
+    if (n_terms == 0) return (int)QIPB200_OK;
+    if (!out) return set_err(rho->ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL out");
+    qipb200_ctx *ctx = rho->ctx;
+    if ((st = begin_device_work(rho)) != QIPB200_OK) return st;
+    CU(ctx, run_density_expect(rho->prec, rho->buf, n, rho->phys_of_logical, terms, out, ctx->stream, &ctx->launches));
+    return (int)QIPB200_OK;
+  });
+}
+
+extern "C" int qipb200_density_reduced(qipb200_state *rho, const uint64_t *qubits, uint32_t k, double *out) {
+  const std::string who = "density_reduced";
+  if (!rho) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, who + ": NULL state");
+  return guarded(rho->ctx, [&]() -> int {
+    uint32_t n = 0;
+    int st = density_qubits(rho, who, &n);
+    if (st == QIPB200_OK) st = density_check_qubits(rho, who, n, qubits, k, false);
+    if (st != QIPB200_OK) return st;
+    if (!out) return set_err(rho->ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL out");
+    if (k > kRdmMaxKept)
+      return set_err(rho->ctx, QIPB200_ERR_UNSUPPORTED, who + ": at most 10 kept qubits, got " + std::to_string(k));
+    qipb200_ctx *ctx = rho->ctx;
+    if ((st = begin_device_work(rho)) != QIPB200_OK) return st;
+    // key = b | a << nb | a' << (nb + k): a on the kept row qubits, a' on the kept column qubits
+    std::vector<uint64_t> masks = density_trace_masks(rho, n, qubits, k);
+    const uint32_t nb = (uint32_t)masks.size();
+    for (uint32_t i = 0; i < k; ++i) masks.push_back(row_bit(rho, n, qubits[i]));
+    for (uint32_t i = 0; i < k; ++i) masks.push_back(col_bit(rho, n, qubits[i]));
+    std::vector<double> sums(2ull << (2 * k));
+    CU(ctx, run_density_sums(rho->prec, rho->buf, masks, nb, 2 * k, k, sums.data(), ctx->stream, &ctx->launches));
+    const size_t K = 1ull << k;
+    for (size_t a = 0; a < K; ++a)
+      for (size_t b = a; b < K; ++b) {
+        const double *v = &sums[2 * (a | (b << k))];
+        out[2 * (a * K + b)] = v[0];
+        out[2 * (a * K + b) + 1] = a == b ? 0.0 : v[1];
+        out[2 * (b * K + a)] = v[0];
+        out[2 * (b * K + a) + 1] = a == b ? 0.0 : -v[1];
+      }
+    return (int)QIPB200_OK;
+  });
+}
+
+extern "C" int qipb200_density_fidelity(qipb200_state *rho, qipb200_state *psi, double *out2) {
+  const std::string who = "density_fidelity";
+  if (!rho || !psi) return set_err(rho ? rho->ctx : nullptr, QIPB200_ERR_INVALID_ARG, who + ": NULL state");
+  return guarded(rho->ctx, [&]() -> int {
+    uint32_t n = 0;
+    int st = density_qubits(rho, who, &n);
+    if (st == QIPB200_OK) st = density_check_psi(rho, psi, n, who);
+    if (st != QIPB200_OK) return st;
+    if (!out2) return set_err(rho->ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL out2");
+    qipb200_ctx *ctx = rho->ctx;
+    if ((st = begin_device_work(rho)) != QIPB200_OK) return st;
+    if ((st = density_prepare_psi(psi)) != QIPB200_OK) return st;
+    CU(ctx, run_density_fidelity(rho->prec, rho->buf, psi->buf, n, rho->phys_of_logical, out2, ctx->stream,
+                                 &ctx->launches));
+    return (int)QIPB200_OK;
+  });
+}
+
+extern "C" int qipb200_density_spectrum(qipb200_state *rho, double *eigs) {
+  const std::string who = "density_spectrum";
+  if (!rho) return set_err(nullptr, QIPB200_ERR_INVALID_ARG, who + ": NULL state");
+  return guarded(rho->ctx, [&]() -> int {
+    uint32_t n = 0;
+    int st = density_qubits(rho, who, &n);
+    if (st != QIPB200_OK) return st;
+    if (!eigs) return set_err(rho->ctx, QIPB200_ERR_INVALID_ARG, who + ": NULL eigs");
+    if (n > kDensitySpectrumMax)
+      return set_err(rho->ctx, QIPB200_ERR_UNSUPPORTED,
+                     who + ": " + std::to_string(n) + " qubits; at most 13 are supported (the matrix of 14 is 4 GiB)");
+    std::string why;
+    if (!eig_solver_available(&why))
+      return set_err(rho->ctx, QIPB200_ERR_UNSUPPORTED, who + ": the eigen-solver is unavailable: " + why);
+    qipb200_ctx *ctx = rho->ctx;
+    const size_t K = 1ull << n;
+    // the solver's buffers come before rho is touched: a refusal for memory leaves it and anything pending as it was
+    CU(ctx, cudaSetDevice(ctx->device));
+    EigWork w;
+    std::string err;
+    st = eig_work_alloc(&ctx->eig_solver, (uint32_t)K, &w, ctx->stream, &err);
+    if (st != QIPB200_OK) return set_err(ctx, st, who + ": " + err);
+    struct Release {
+      EigWork *w;
+      cudaStream_t s;
+      ~Release() {
+        eig_work_free(w, s);
+        cudaStreamSynchronize(s);
+      }
+    } release{&w, ctx->stream};
+    if ((st = begin_device_work(rho)) != QIPB200_OK) return st;
+    CU(ctx, run_density_widen(rho->prec, rho->buf, n, rho->phys_of_logical, w.G, ctx->stream, &ctx->launches));
+    std::vector<double> asc(K);
+    st = eig_solve(ctx->eig_solver, &w, ctx->stream, asc.data(), &err);
+    if (st != QIPB200_OK) return set_err(ctx, st, who + ": " + err);
+    std::sort(asc.begin(), asc.end());
+    for (size_t i = 0; i < K; ++i) eigs[i] = asc[K - 1 - i];
     return (int)QIPB200_OK;
   });
 }

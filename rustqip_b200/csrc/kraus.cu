@@ -292,7 +292,7 @@ const size_t kMatBytes = kKrausMatEntries * sizeof(double2);
 
 int parse_kraus_channels(const std::string &who, uint32_t n, size_t n_channels, const uint32_t *arity,
                          const uint64_t *qubits, const uint32_t *n_kraus, const double *kraus, KrausSet *out,
-                         std::string *err) {
+                         std::string *err, bool sequential) {
   if (n_channels && (!arity || !qubits || !n_kraus || !kraus)) {
     *err = who + ": NULL arity, qubits, n_kraus or kraus";
     return QIPB200_ERR_INVALID_ARG;
@@ -309,6 +309,7 @@ int parse_kraus_channels(const std::string &who, uint32_t n, size_t n_channels, 
       return QIPB200_ERR_INVALID_ARG;
     }
     ks.qfirst.push_back((uint32_t)ks.qubits.size());
+    if (sequential) seen = 0;
     for (uint32_t i = 0; i < k; ++i) {
       const uint64_t q = qubits[ks.qubits.size()];
       if (q >= n) {

@@ -36,10 +36,11 @@ struct KrausSet {
 };
 
 // Validate n_channels channels of an n-qubit state (the rules of include/qipb200.h) into *out.  Returns QIPB200_OK,
-// or the status with the message (prefixed by who) in *err.
+// or the status with the message (prefixed by who) in *err.  A layer names no qubit twice; with sequential set, the
+// channels run one after the other (qipb200_density_apply), so only a qubit repeated inside one channel is refused.
 int parse_kraus_channels(const std::string &who, uint32_t n, size_t n_channels, const uint32_t *arity,
                          const uint64_t *qubits, const uint32_t *n_kraus, const double *kraus, KrausSet *out,
-                         std::string *err);
+                         std::string *err, bool sequential = false);
 
 // The groups of the state-dependent channels: runs of consecutive ones, in channel order, with at most
 // kKrausGroupBits qubits each (a group closes when the next channel would exceed them).

@@ -717,6 +717,189 @@ FUNCTION_TILE, FUNCTION_PAIR = 0, 1
 FN_CODE_THETA = 1  # QIPB200_FN_CODE_THETA
 
 
+class DensityMatrix:
+    """The exact mixed state of n qubits on the device, for noisy circuits (qipb200_density_*).
+
+    It owns a ``State`` of 2n qubits (``.state``) that holds vec(rho): row qubit q is state qubit q, column qubit q is
+    state qubit n + q, so rho[r, c] is amplitude r * 2^n + c and ``download()`` is the 2^n x 2^n matrix.  Gates and
+    Kraus channels run interleaved in one fused schedule (``apply``); the readouts honour a permuted layout, work on
+    rho as it is (not renormalised) and are deterministic, except the bits of ``spectrum``, which come from cuSOLVER.
+    Unsharded states only."""
+
+    def __init__(self, n: int, dtype=np.complex128, ctx: Optional[Context] = None):
+        if int(n) < 1:
+            raise ValueError("DensityMatrix: n must be at least 1, got %d" % int(n))
+        self.n = int(n)
+        self.state = State(2 * self.n, dtype, ctx)
+        self.ctx, self.prec, self.dtype = self.state.ctx, self.state.prec, self.state.dtype
+
+    def free(self):
+        self.state.free()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.free()
+
+    def _chk(self, st):
+        _lib.check(st, self.ctx.handle)
+
+    def set_basis(self, i: int):
+        """rho = |i><i| (pending, like State.set_basis: the next fused apply builds it in its first pass)."""
+        i = int(i)
+        if not 0 <= i < (1 << self.n):
+            raise ValueError("set_basis: %d is not an index of %d qubits" % (i, self.n))
+        self.state.set_basis(i + (i << self.n))
+
+    def set_pure(self, psi: State):
+        """rho = |psi><psi| (not normalised) for a State of n qubits in this context and precision: one write sweep."""
+        self._chk(_lib.lib().qipb200_density_from_state(self.state._h, psi._h))
+
+    def apply(self, items, fusion: bool = True):
+        """Run ``items`` in order in one schedule: each is a ``MatrixOp`` (rho -> U rho U^dagger) or a pair
+        ``(channel, qubits)`` with a ``channels.KrausChannel`` or ``Channel`` on 1..4 qubits (rho -> sum K rho
+        K^dagger, the channel's first qubit the most significant bit of its matrices).  ``fusion`` as for
+        ``State.apply_schedule``; the result is bit-identical to ``state.apply_schedule(density_schedule(...))`` when both
+        run the same kernels (QIPB200_JIT: a pass may run on the interpreter kernel while its generated kernel
+        compiles)."""
+        args, keep = _density_args(self.prec, items)
+        flags = _lib.SCHED_DEFAULT if fusion else _lib.SCHED_NO_FUSION
+        self._chk(_lib.lib().qipb200_density_apply(self.state._h, *args, flags))
+
+    def measure_probs(self, qubits: Sequence[int]) -> np.ndarray:
+        """out[m] = sum of rho_rr over the r whose bits on ``qubits`` equal m (bit i of m is qubits[i]); reads only the
+        diagonal.  No qubits gives [Tr rho]."""
+        idx = np.ascontiguousarray(np.asarray(list(qubits), dtype=np.uint64))
+        out = np.zeros(1 << len(idx), dtype=np.float64)
+        self._chk(_lib.lib().qipb200_density_measure_probs(self.state._h, _ptr(idx) if len(idx) else None, len(idx),
+                                                           _ptr(out)))
+        return out
+
+    def trace(self) -> float:
+        return float(self.measure_probs([])[0])
+
+    def sample(self, qubits: Sequence[int], shots: int, rng=None) -> np.ndarray:
+        """``shots`` outcomes of measuring ``qubits`` (bit i of each is qubits[i]), drawn on the host from
+        ``measure_probs`` (at most 2^n values) with ``rng`` (a fresh ``np.random.default_rng()`` when None)."""
+        p = np.clip(self.measure_probs(qubits), 0.0, None)
+        rng = rng if rng is not None else np.random.default_rng()
+        return rng.choice(p.shape[0], size=int(shots), p=p / p.sum()).astype(np.uint64)
+
+    def measure(self, qubits: Sequence[int], rng=None):
+        """Selective measurement of ``qubits``: draws the outcome m with probability p = measure_probs(qubits)[m] and
+        leaves rho = Pi rho Pi / p.  Pi is applied as one single-qubit projector per measured qubit through ``apply``,
+        the first scaled by 1/sqrt(p).  Returns (m, p)."""
+        qubits = [int(q) for q in qubits]
+        probs = np.clip(self.measure_probs(qubits), 0.0, None)
+        total = float(probs.sum())
+        if not total > 0.0:
+            raise CircuitError("measure: the density matrix has no weight on these qubits")
+        u = (rng if rng is not None else np.random.default_rng()).random() * total
+        m = int(min(np.searchsorted(np.cumsum(probs), u, side="right"), probs.shape[0] - 1))
+        while probs[m] == 0.0:  # rounding at the end of the cumulative sum
+            m -= 1
+        p = float(probs[m])
+        ops = []
+        for j, q in enumerate(qubits):
+            proj = np.zeros((2, 2), dtype=np.complex128)
+            proj[(m >> j) & 1, (m >> j) & 1] = 1.0 / np.sqrt(p) if j == 0 else 1.0
+            ops.append(MatrixOp.new_matrix([q], proj.reshape(-1)))
+        self.apply(ops)
+        return m, p
+
+    def expect_paulis(self, terms) -> np.ndarray:
+        """Re Tr(rho P_t) for Pauli strings encoded as for ``State.expect_paulis``."""
+        qs, ls, lens = _marshal_paulis(terms)
+        out = np.zeros(max(1, lens.shape[0]), dtype=np.float64)
+        self._chk(_lib.lib().qipb200_density_expect_paulis(self.state._h, _ptr(qs), ls, _ptr(lens), lens.shape[0],
+                                                           _ptr(out)))
+        return out[: lens.shape[0]]
+
+    def reduced_density(self, qubits: Sequence[int]) -> np.ndarray:
+        """Tr_B rho for 1..10 kept ``qubits``: complex128 (2^k, 2^k), bit i of the indices qubits[i] (the convention
+        of ``State.reduced_density``); exactly Hermitian."""
+        idx = np.ascontiguousarray(np.asarray(list(qubits), dtype=np.uint64))
+        k = len(idx)
+        out = np.zeros((1 << min(k, 10)) ** 2 if k else 1, dtype=np.complex128)
+        self._chk(_lib.lib().qipb200_density_reduced(self.state._h, _ptr(idx) if k else None, k, _ptr(out)))
+        return out.reshape(1 << k, 1 << k)
+
+    def fidelity(self, psi: State) -> float:
+        """<psi|rho|psi> for a State of n qubits (its real part; the imaginary part is rounding only): one read sweep
+        of rho."""
+        out2 = np.zeros(2)
+        self._chk(_lib.lib().qipb200_density_fidelity(self.state._h, psi._h, _ptr(out2)))
+        return float(out2[0])
+
+    def purity(self) -> float:
+        """Tr rho^2 = sum |rho_rc|^2: ``norm2`` of the vector."""
+        return self.state.norm2()
+
+    def spectrum(self) -> np.ndarray:
+        """The 2^n eigenvalues of rho in descending order (n <= 13), solved on the device by cuSOLVER."""
+        eigs = np.zeros(1 << min(self.n, 13))
+        _lib.preload_cusolver()
+        self._chk(_lib.lib().qipb200_density_spectrum(self.state._h, _ptr(eigs)))
+        return eigs
+
+    def entropy(self) -> float:
+        """von Neumann entropy -sum p ln p in nats of p = lambda / Tr rho over the eigenvalues > 0."""
+        eigs = self.spectrum()
+        tr = self.trace()
+        p = eigs[eigs > 0] / tr
+        return float(-np.sum(p * np.log(p)))
+
+    def download(self) -> np.ndarray:
+        side = 1 << self.n
+        return self.state.download().reshape(side, side)
+
+
+def _density_args(prec, items):
+    """((ops, n_ops, n_channels, channel_pos, arity, qubits, n_kraus, kraus), keep): the C arguments of a list of
+    MatrixOps and (channel, qubits) pairs, and the arrays they point into (hold keep for the call)."""
+    from . import channels as _ch
+    ops, chans, groups, pos = [], [], [], []
+    for item in items:
+        if isinstance(item, MatrixOp):
+            ops.append(item)
+            continue
+        chan, qs = item
+        chan = chan if isinstance(chan, _ch.KrausChannel) else _ch.KrausChannel(chan)
+        qs = [int(q) for q in qs]
+        if chan.n_qubits != len(qs):
+            raise ValueError("density: channel %d acts on %d qubits but is given %d" % (len(chans), chan.n_qubits,
+                                                                                    len(qs)))
+        chans.append(chan)
+        groups.append(qs)
+        pos.append(len(ops))
+    arr, keep = marshal_ops(ops, prec)
+    arity, n_kraus, kraus = _ch_marshal(chans)
+    qa = np.ascontiguousarray(np.asarray([q for g in groups for q in g], dtype=np.uint64))
+    cp = np.ascontiguousarray(np.asarray(pos, dtype=np.uint64))
+    nc = len(chans)
+    args = (arr, len(ops), nc, _ptr(cp) if nc else None, _ptr(arity) if nc else None, _ptr(qa) if nc else None,
+            _ptr(n_kraus) if nc else None, _ptr(kraus) if nc else None)
+    return args, (keep, arity, n_kraus, kraus, qa, cp)
+
+
+def density_schedule(n: int, dtype, items):
+    """The doubled schedule of ``DensityMatrix.apply(items)`` on an n-qubit rho, as MatrixOps on 2n qubits, written by
+    the library (qipb200_density_schedule, QIPS v1) and decoded here; needs no GPU.  Validates as the call does."""
+    from .wire import loads_schedule
+    prec = prec_of(dtype)
+    args, keep = _density_args(prec, items)
+    need = C.c_size_t(0)
+    L = _lib.lib()
+    st = L.qipb200_density_schedule(prec, int(n), *args, None, 0, C.byref(need))
+    if st != _lib.ERR_SIZE_MISMATCH or need.value == 0:
+        _lib.check(st, None)
+    buf = (C.c_ubyte * need.value)()
+    _lib.check(L.qipb200_density_schedule(prec, int(n), *args, buf, need.value, C.byref(need)), None)
+    _, _, ops = loads_schedule(bytes(buf))
+    return ops
+
+
 def function_code_compile(n_in: int, n_out: int, source: str, theta: bool = False, n_params: int = 0) -> str:
     """Compile the program of ``Function.from_code`` with NVRTC without a context or GPU; returns the NVRTC log
     (warnings, if any) and raises ``CircuitError`` (with the log) on a compile error or refused sizes."""

@@ -108,6 +108,21 @@ def load_schedule(path: str) -> Tuple[int, type, List[MatrixOp]]:
         return n, dt, [_r_op(f, dt) for _ in range(n_ops)]
 
 
+def loads_schedule(data: bytes) -> Tuple[int, type, List[MatrixOp]]:
+    """load_schedule of QIPS bytes held in memory."""
+    import io
+
+    f = io.BytesIO(data)
+    magic, version, prec, n, n_ops = struct.unpack("<IIIIQ", _r_exact(f, 24))
+    if magic != MAGIC_SCHEDULE or version != 1 or prec not in (QIP_F32, QIP_F64):
+        raise CircuitError("not a QIPS version-1 schedule")
+    dt = cdtype(prec)
+    ops = [_r_op(f, dt) for _ in range(n_ops)]
+    if f.read(1):
+        raise CircuitError("schedule: trailing bytes after the last record")
+    return n, dt, ops
+
+
 class ParsedSchedule:
     """A QIPS buffer parsed by the C ABI (`qipb200_schedule_parse`, rustqip_b200/csrc/wire.cpp): the library owns
     the `qip_op` records; `State.apply_marshalled(sched.ops, sched.n_ops)` runs them without a Python op tree."""
